@@ -2,7 +2,7 @@
 """bench.py — hash-join probe rows/s on the BASELINE.json workload (lineitem JOIN orders, synthetic SF100,
 BIGINT key), plus the Q1 GROUP-BY input rows/s, through the C ABI of libtrino_gpu.so.
 
-  python bench.py --gpus 1 --steps K --warmup W            # this repo's sm_100a operators
+  python bench.py --gpus 1 --steps K --warmup W            # this repo's sm_90a operators
   python bench.py --impl reference --gpus N ...            # the reference's CPU algorithm (C++ restatement, all host threads)
   torchrun ... bench.py --gpus N ...                       # partitioned join: hash exchange over NCCL + local probe
 
@@ -31,10 +31,6 @@ ALG_BYTES_PROBE_FUSED = 40          # fused probe + gather, this workload: 24 + 
 ALG_BYTES_Q1_CODES = 38             # shipdate 4 + 4 x FLOAT64 32 + 2 INT8 key codes
 ALG_BYTES_Q1_UTF8 = 46              # the reference's key types: 2 x VARCHAR(1) = 2 x (4 offset + 1 byte) instead of the 2 code bytes (SURVEY.md §8d)
 ALG_BYTES_GROUPBY_BIGINT = 36       # SURVEY.md §8d: 8 key + 8 value + 20 table entry touched
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures (profiles/r02_kernels.md),
-# quoted only for the configuration they were captured on
-NCU_TRAFFIC_PROBE_FUSED_SF100 = 8.429180e9 + 7.174483e9      # 600 000 003 rows: 26.0 B/row (join_probe_lean_kernel<2,1,8>, dense order-preserving table)
-NCU_TRAFFIC_Q1_SF300 = 68.400325e9 + 4.218368e6               # 1.8 G rows: 38.0 B/row (tg_agg_small_jit, profiles/r02_kernels.md, capture r3k)
 
 
 def bind_to_gpu_numa_node(local):
@@ -65,11 +61,11 @@ def measured_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p))["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not a measured peak)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -185,7 +181,7 @@ def workload_config(args, n_orders, probe_rows, world):
                              "by SM stores into peer HBM (NVLink)" if os.environ.get("TGPU_BENCH_SERIAL") else
                              "into peer HBM over NVLink by the copy engines, two half-pages per step, split-phase: SMs partition page k+1 and probe page k "
                              "while page k+1 is in flight")) if world > 1 else "single GPU",
-            "l2": "inputs (9.6 GB probe side, 4.3 GB table at SF100) are far larger than the 126 MB L2; no flush needed"}
+            "l2": "inputs (9.6 GB probe side, 4.3 GB table at SF100) are far larger than the 50 MB L2 of an H100; no flush needed"}
 
 
 def device_col(ctx, nbytes):
@@ -203,7 +199,7 @@ def main():
     ap.add_argument("--sf", type=float, default=None, help="TPC-H scale factor per GPU (default 100 for the join workload, 37.5 = SF300 / 8 for q3way)")
     ap.add_argument("--ds-sf", type=float, default=125.0, help="TPC-DS scale factor per GPU of the star workload (125 = SF1000 / 8)")
     ap.add_argument("--star-chunks", type=int, default=4, help="pages the fact shard is fed in per step (bounds the intermediate pages)")
-    ap.add_argument("--q1-sf", type=float, default=300.0, help="scale factor of the Q1 GROUP-BY side measurement (0 = skip)")
+    ap.add_argument("--q1-sf", type=float, default=100.0, help="scale factor of the Q1 GROUP-BY side measurement (0 = skip; 100 keeps it within 80 GB beside the join)")
     ap.add_argument("--shuffle-probe", action="store_true", help="variant B: uniformly shuffled probe keys")
     ap.add_argument("--cpu-sample-rows", type=int, default=200_000_000)
     ap.add_argument("--e2e-rows", type=int, default=0, help="probe rows fed from host per e2e step (0 = all)")
@@ -213,7 +209,13 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="skip the FilterAndProject / PartitionedOutput blocks (secondary_operators)")
     ap.add_argument("--no-e2e", action="store_true", help="skip the end-to-end (host pages) measurement: kernel experiments only")
     ap.add_argument("--l2-fetch", type=int, default=0, help="cudaLimitMaxL2FetchGranularity to set (32/64/128; 0 = leave the default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write a fixed sample of the joined page of the last timed step to DIR/<column>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "b200" or args.workload != "join" or dist_env()[1] > 1):
+        ap.error("--dump-outputs covers the single-GPU join workload")
     if args.sf is None:
         args.sf = 37.5 if args.workload == "q3way" else 100.0
     if args.impl == "reference":
@@ -257,7 +259,6 @@ def main():
     d_okeys = ctx.malloc(n_orders * 8)
     ctx.check(lib.tgpu_synth_orders_keys(ctx.h, total_orders, o_first, n_orders, SEED_ORDERS, 1, C.c_void_p(d_okeys)))
     d_lkeys = ctx.malloc(l_count * 8)
-    d_lprice = ctx.malloc(l_count * 8)
     ctx.check(lib.tgpu_synth_lineitem_keys(ctx.h, total_orders, l_first, l_count, SEED_LINEITEM, int(args.shuffle_probe), C.c_void_p(d_lkeys)))
     # payload columns: o_orderdate = key % 2557 (INT32), l_extendedprice = key * 0.5 (FLOAT64); produced by the filter/project operator
     def project(ptr, n, dtype_expr, out_type):
@@ -390,7 +391,9 @@ def main():
         probe_op.add_input(inp.as_device_page())
         inflight.append(inp)
 
-    def step():
+    held = []      # the output of the last timed step, when it is dumped
+
+    def step(hold=False):
         if overlap:
             step_overlapped()
         elif partitioner is not None:
@@ -411,7 +414,10 @@ def main():
             out = probe_op.get_output_device()
             out_rows_seen[0] = out.rows if out else 0
             if out:
-                out.release()
+                if hold:
+                    held.append(out)
+                else:
+                    out.release()
 
     for _ in range(args.warmup):
         step()
@@ -427,8 +433,8 @@ def main():
     step_rows[0] = 0
     launches0 = ctx.kernel_launches + 0
     ctx.timer_start()
-    for _ in range(args.steps):
-        step()
+    for i in range(args.steps):
+        step(hold=args.dump_outputs is not None and i == args.steps - 1)
     if overlap:
         # pipeline drain: the last exchange is ended and probed, its output taken (host-synchronised) before the stop event
         while handles:
@@ -438,6 +444,9 @@ def main():
     ms = ctx.timer_stop_ms()
     launches = ctx.kernel_launches + 0 - launches0
     clocks = sampler.stop()
+    for out in held:
+        dump_join_output(ctx, out, args.dump_outputs)
+        out.release()
     barrier()
     if dist is not None:
         import torch
@@ -486,15 +495,12 @@ def main():
         peak, peak_src = measured_peak()
         kms = float(np.mean(kernel_ms))
         achieved = ALG_BYTES_PROBE_FUSED * l_count / (kms * 1e-3) / 1e9
-        traffic = NCU_TRAFFIC_PROBE_FUSED_SF100 if (args.sf == 100.0 and not args.shuffle_probe and not os.environ.get("TGPU_JOIN_HASH")) else None
         roofline = {"kernel": "join_probe_lean_kernel<2,true> (fused probe + payload gather, order-preserving table lines)", "bound": "hbm", "achieved": achieved, "peak": peak,
-                    "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                    "traffic_source": "ncu --set full capture of this kernel on this configuration, profiles/r02_kernels.md (bytes per launch)",
-                    "frac_of_traffic": (traffic / (kms * 1e-3) / 1e9 / peak) if traffic else None,
+                    "unit": "GB/s", "frac": achieved / peak,
                     "note": "algorithmic_bytes_per_row 40 = 8 key + 12 table entry + 4 position + 8 build payload read + 8 written: SURVEY §8(d)'s 52 minus the probe columns, "
                             "which pass through as views (LookupJoinPageBuilder.java:144-150), with an 8-byte BIGINT build payload instead of the survey's INT32.  "
                             "frac can exceed 1: the model charges one table entry per probe ROW, but the ~4 rows of an order share one entry and the "
-                            "order-preserving layout reads every table line once; frac_of_traffic = measured DRAM bytes (ncu) / kernel time / peak is the physical utilisation",
+                            "order-preserving layout reads every table line once",
                     "peak_source": peak_src, "algorithmic_bytes_per_row": ALG_BYTES_PROBE_FUSED, "rows_per_launch": l_count,
                     "kernel_ms": kms, "kernel_share_of_step": kms / ms_per_step, "launches_timed": len(kernel_ms)}
         d_pos = ctx.malloc(l_count * 4)
@@ -539,10 +545,9 @@ def main():
                     "line_floor_rows_per_sec": peak * 1e9 / (8 + 128 + 4 + 8),
                     "frac_of_line_floor": (l_count / (sm * 1e-3)) / (peak * 1e9 / (8 + 128 + 4 + 8)),
                     "note": "every probe row reads its own random 32-byte wide slot (key, head and the payload cell in one sector; the 16-byte slots + "
-                            "slot-ordered payload array of the key-ordered case cost two random accesses per row: 33 ms).  ncu (profiles/r02_kernels.md): the "
-                            "L2 fills a whole 128-byte line from HBM for every random sector (134 DRAM bytes per row, whatever cudaLimitMaxL2FetchGranularity "
-                            "or the load's L2 fetch-size qualifier say), so the floor of this access pattern is line_floor = copy peak / (8 key + 128 line + "
-                            "4 position + 8 payload written), not sector_floor"}
+                            "slot-ordered payload array of the key-ordered case cost two random accesses per row).  If the L2 fills a whole 128-byte line "
+                            "from HBM for every random sector, the floor of this access pattern is line_floor = peak / (8 key + 128 line + 4 position + "
+                            "8 payload written); sector_floor assumes 32-byte fills"}
         ctx.free(d_skeys)
 
     # ---------------- Q1 GROUP-BY side measurement (BASELINE.json configs[2]) on rank 0 at N=1
@@ -601,6 +606,28 @@ def main():
         dist.destroy_process_group()
     ctx.close()
     return 0
+
+
+def dump_join_output(ctx, out, outdir, block_rows=4096, blocks=256, seed=0x7C05):
+    """Writes a fixed sample of one joined page (probe key, probe price, build payload) to outdir as float64 .npy files (the BIGINT
+    values are below 2**53): `blocks` runs of `block_rows` consecutive output rows whose starts are drawn with `seed`, so the same
+    arguments give the same rows.  The join keeps the probe page's row order, so two builds can be compared row for row."""
+    n = out.rows
+    nblocks = -(-n // block_rows)
+    starts = np.sort(np.random.default_rng(seed).choice(nblocks, min(blocks, nblocks), replace=False)) * block_rows
+    runs = [(int(lo), int(min(n, lo + block_rows))) for lo in starts]
+    arrays = {"output_rows": np.array([n], np.float64),
+              "row_index": np.concatenate([np.arange(lo, hi) for lo, hi in runs]).astype(np.float64)}
+    for name, c, dtype in (("probe_orderkey", 0, np.int64), ("probe_extendedprice", 1, np.float64), ("build_orderdate", 2, np.int64)):
+        host = np.empty(sum(hi - lo for lo, hi in runs), dtype)
+        at = 0
+        for lo, hi in runs:
+            ctx.check(ctx.lib.tgpu_memcpy_d2h(ctx.h, C.c_void_p(host[at:].ctypes.data), C.c_void_p(out.column(c).ptr + lo * 8), (hi - lo) * 8))
+            at += hi - lo
+        arrays[name] = host.astype(np.float64)
+    os.makedirs(outdir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(outdir, name + ".npy"), a)
 
 
 def bench_e2e(ctx, args, bridge, d_keys, d_price, n, drivers=int(os.environ.get("TGPU_E2E_DRIVERS", "4"))):
@@ -878,7 +905,7 @@ def bench_q1(ctx, args):
     factory = q1_factory(ctx, fused=True)
     peak, peak_src = measured_peak()
 
-    def measure(pg, alg, label, traffic):
+    def measure(pg, alg, label):
         def run():
             op = factory.create_operator()
             op.add_input(pg)
@@ -903,12 +930,12 @@ def bench_q1(ctx, args):
         return {"metric": "groupby_input_rows_per_sec", "value": n / (ms * 1e-3), "unit": "rows/s", "ms_per_step": ms, "rows": n, "groups": len(rows),
                 "config": f"TPC-H Q1 GROUP-BY, synthetic SF{args.q1_sf:g} lineitem, {label}, fused filter+project+aggregate (BASELINE.json configs[2])",
                 "roofline": {"kernel": "tg_agg_small_jit", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "peak_source": peak_src, "algorithmic_bytes_per_row": alg, "traffic": traffic, "kernel_ms": kms, "kernel_share_of_step": kms / ms,
+                             "peak_source": peak_src, "algorithmic_bytes_per_row": alg, "kernel_ms": kms, "kernel_share_of_step": kms / ms,
                              "step_frac": step_achieved / peak},
                 "result_count_order": [int(r[-1]) for r in rows]}
 
-    q1 = measure(page, ALG_BYTES_Q1_CODES, "INT8 key codes", NCU_TRAFFIC_Q1_SF300 if args.q1_sf == 300.0 else None)
-    q1["utf8_keys"] = measure(page_utf8, ALG_BYTES_Q1_UTF8, "VARCHAR(1) keys (the reference's types: offsets + bytes, device string dictionary)", None)
+    q1 = measure(page, ALG_BYTES_Q1_CODES, "INT8 key codes")
+    q1["utf8_keys"] = measure(page_utf8, ALG_BYTES_Q1_UTF8, "VARCHAR(1) keys (the reference's types: offsets + bytes, device string dictionary)")
     assert q1["utf8_keys"]["result_count_order"] == q1["result_count_order"]
     ctx.free(d_off)
     for p in ptrs:

@@ -1,12 +1,12 @@
 /*
- * trino_gpu.h — C ABI of libtrino_gpu.so: the B200 (sm_100a) implementation of Trino's
+ * trino_gpu.h — C ABI of libtrino_gpu.so: the H100 (sm_90a) implementation of Trino's
  * columnar operator hot path.
  *
  * The reference has no FFI for this path (SURVEY.md §8b): operators are Java classes that
  * implement io.trino.operator.Operator / OperatorFactory.  Every entry point below is what a
  * thin Java Operator (see INTEGRATION.md, java/) binds through Panama/JNI, and each cites the
  * reference interface it stands in for (paths relative to
- * /root/reference/core/trino-main/src/main/java/io/trino/ = M/, .../trino-spi/.../spi/ = S/).
+ * trinodb/trino/core/trino-main/src/main/java/io/trino/ = M/, .../trino-spi/.../spi/ = S/).
  *
  * Conventions
  *   - plain C, plain pointers and sizes; no C++/torch types.
@@ -291,7 +291,7 @@ int tgpu_agg_rows_with_partial_aggregation_disabled(tgpu_op* op, int64_t* out);
 
 int tgpu_agg_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op** out);
 /* diagnostics (needs no GPU): generate the kernel specialised for `spec` over input channels of the given tgpu_types
- * (bit c of nullable_mask = channel c carries NULLs), compile it with NVRTC for sm_100a; returns the cubin size and
+ * (bit c of nullable_mask = channel c carries NULLs), compile it with NVRTC for sm_90a; returns the cubin size and
  * the generated source (or the compiler log on failure) */
 int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* channel_types, int32_t num_channels, uint32_t nullable_mask,
                           int64_t* cubin_bytes, char* source_out, int64_t source_cap);

@@ -63,7 +63,7 @@ inline uint64_t hash_real(float f)
 inline uint64_t rd64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
 inline uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 
-// public XXH64 algorithm (io.airlift.slice.XxHash64; not vendored under /root/reference)
+// public XXH64 algorithm (io.airlift.slice.XxHash64; not vendored under trinodb/trino)
 uint64_t xxh64(const uint8_t* p, int64_t len, uint64_t seed)
 {
     const uint8_t* end = p + len;

@@ -9,7 +9,7 @@
  * Parity pinning status (see DESIGN.md §Oracle):
  *   - XXH64: pinned on the reference's own golden vectors
  *     (core/trino-main/src/test/java/io/trino/operator/scalar/TestVarbinaryFunctions.java:776-780)
- *     plus the published xxHash vectors (io.airlift:slice is not vendored under /root/reference).
+ *     plus the published xxHash vectors (io.airlift:slice is not vendored under trinodb/trino).
  *   - murmur3 fmix64: restated in-repo at M/operator/join/PagesHash.java:44-50 (pinned by source).
  *   - group ids / join rows / partition lists: pinned on the behavioural cases of the reference's unit
  *     tests (TestGroupByHash, TestHashJoinOperator, TestPagePartitioner) restated in tests/golden/.

@@ -451,8 +451,8 @@ def test_wide_slots_carry_every_payload_width(ctx, monkeypatch, join_type, paylo
 
 def test_build_over_a_random_half_of_a_dense_domain_stays_fast(ctx):
     # what a 2-way hash exchange leaves on a rank: a hash-selected half of the order keys.  The dense trial geometry does not suit it
-    # (lines of 32 key values expect exactly 8 keys) and used to degenerate into chains thousands of lines long - 174 s for 75 M rows
-    # on a B200; trial geometries are bounded now and the build falls through to the roomy / scattered layouts in milliseconds.
+    # (lines of 32 key values expect exactly 8 keys) and used to degenerate into chains thousands of lines long; trial geometries are
+    # bounded now and the build falls through to the roomy / scattered layouts in milliseconds.
     import time
     n_orders = 12_000_000
     okeys = o.synth_orders_keys(n_orders, 0, n_orders, 0x7C02, True)

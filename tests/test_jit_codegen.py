@@ -1,5 +1,5 @@
 """The NVRTC specialisation path needs no GPU to compile: generate the fused Q1 kernel (and variants with NULL-able
-channels) and compile it for sm_100a on the CPU box.  The launch itself is covered by the -m gpu suites."""
+channels) and compile it for sm_90a on the CPU box.  The launch itself is covered by the -m gpu suites."""
 import ctypes as C
 
 import pytest

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Turn `.ncu-rep` captures into the markdown tables kept under profiles/ (reads them with `ncu -i … --page raw --csv`).
+"""Turn `.ncu-rep` captures into markdown tables (reads them with `ncu -i … --page raw --csv`).
 usage: tools/ncu_summary.py <rep> [<rep> …]   -> markdown on stdout"""
 import csv
 import io

@@ -1,6 +1,6 @@
 // Micro-benchmark (diagnostics, not part of the library): what store pattern does NVLink want?
 // One process, two devices; kernels on device 0 write into a buffer on device 1 (and, for reference, into local memory).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/p2p_write_bench tools/p2p_write_bench.cu && build/p2p_write_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/p2p_write_bench tools/p2p_write_bench.cu && build/p2p_write_bench
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
@@ -80,7 +80,7 @@ int main(int argc, char** argv)
         CK(cudaEventElapsedTime(&ms, e0, e1));
         printf("%-44s %8.1f GB/s written\n", name, n * 8.0 * 5 / ms / 1e6);
     };
-    const int grid = 148 * 8, bs = 256;
+    const int grid = 132 * 8, bs = 256;      // 8 CTAs on each of an H100's 132 SMs
     for (int where = quick ? 1 : 0; where < (remote ? 2 : 1); where++) {
         long long* dst = where ? remote : local;
         printf("---- destination: %s (device %d)\n", where ? "peer GPU over NVLink" : "local HBM", where ? peer : 0);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""`cuobjdump -res-usage` of the library as the markdown table kept under profiles/.  usage: tools/resource_table.py > profiles/rNN_resources.md"""
+"""`cuobjdump -res-usage` of the library as a markdown table.  usage: tools/resource_table.py > resources.md"""
 import re
 import subprocess
 
@@ -19,7 +19,7 @@ out = []
 for (fn, reg, stack, sh), nm in zip(rows, names):
     nm = nm.replace("(anonymous namespace)::", "").split("(")[0].replace("void ", "")
     out.append((nm, reg, stack, sh))
-print("# r02 — static resource usage (`cuobjdump -res-usage trino_b200/libtrino_gpu.so`, sm_100a, nvcc 12.9 -O3 -fmad=false)\n")
+print("# static resource usage (`cuobjdump -res-usage trino_b200/libtrino_gpu.so`, sm_90a, nvcc 12.9 -O3 -fmad=false)\n")
 print("Registers, local stack and static shared memory per kernel, and how many 256-thread CTAs the register file (64 K x 32-bit per SM) admits.  "
       "NVRTC kernels (`tg_agg_small_jit`: 76 registers + 49.2 KB dynamic smem for the Q1 program; `tg_agg_general_jit`: `__launch_bounds__(256, 4)`; "
       "`tg_fp_*_jit`: 19 / 32 registers) are compiled at run time and appear in `r02_kernels.md` instead.\n")

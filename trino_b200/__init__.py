@@ -1,4 +1,4 @@
-"""trino_b200 — B200-native (sm_100a) implementation of Trino's columnar operator hot path.
+"""trino_b200 — H100-native (sm_90a) implementation of Trino's columnar operator hot path.
 
 The product is trino_b200/libtrino_gpu.so (hand-written CUDA behind the C ABI of include/trino_gpu.h);
 this package is the thin host-side mirror of the reference's Operator/OperatorFactory interface.

@@ -1,7 +1,7 @@
-"""Build recipe for libtrino_gpu.so (sm_100a).
+"""Build recipe for libtrino_gpu.so (sm_90a).
 
 `python -m trino_b200._build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.
-The library is built IN-TREE (trino_b200/libtrino_gpu.so) so that it travels to the GPU box.
+The library is built IN-TREE (trino_b200/libtrino_gpu.so) so that the package imports from the repository tree.
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(ROOT, "trino_b200", "csrc")
 LIB = os.path.join(ROOT, "trino_b200", "libtrino_gpu.so")
 SOURCES = ["core.cu", "join.cu", "groupby.cu", "expr.cu", "partition.cu", "synth.cu", "jit.cu", "serde.cu", "dynfilter.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",            # Java never contracts a*b+c (M/type/DoubleOperators.java:66-86)
     "-Xcompiler", "-fPIC",
@@ -59,7 +59,7 @@ def build_gpu(force=False, verbose=False):
             sys.stderr.write(f"--- nvcc {src} ---\n{out}\n")
     if failed:
         raise RuntimeError("nvcc failed")
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-ldl"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

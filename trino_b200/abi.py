@@ -268,7 +268,7 @@ def load_library(path=None):
     p = path or LIB_PATH
     if not os.path.exists(p):
         raise RuntimeError(
-            f"{p} is missing: build it with `python -m trino_b200._build` (nvcc, sm_100a). "
+            f"{p} is missing: build it with `python -m trino_b200._build` (nvcc, sm_90a). "
             "trino_b200 has no CPU fallback.")
     lib = C.CDLL(p, mode=C.RTLD_GLOBAL)
     for name, (res, args) in SIGNATURES.items():

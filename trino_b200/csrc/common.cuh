@@ -31,7 +31,7 @@ struct tgpu_ctx {
     bool kev_valid = false;
     void* flush_buf = nullptr;
     size_t flush_bytes = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     size_t smem_optin = 0;
     // pinned staging ring for host pages
     void* staging = nullptr;
@@ -62,7 +62,9 @@ struct tgpu_ctx {
 int tg_fail(tgpu_ctx* ctx, int status, const char* fmt, ...);
 
 constexpr size_t TG_BIG_BLOCK = (size_t)32 << 20;            // blocks at least this large go through the ctx cache
-constexpr size_t TG_BIG_CACHE_LIMIT = (size_t)64 << 30;      // bytes the cache may hold before blocks go back to the pool
+// bytes the cache may hold before blocks go back to the pool: a fifth of an H100's 80 GB, so that cached blocks do not starve
+// allocations of other sizes
+constexpr size_t TG_BIG_CACHE_LIMIT = (size_t)16 << 30;
 
 #define TG_CUDA(ctx, call)                                                                           \
     do {                                                                                             \
@@ -98,7 +100,7 @@ constexpr size_t TG_BIG_CACHE_LIMIT = (size_t)64 << 30;      // bytes the cache 
 
 static inline int64_t tg_div_up(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// grid size for a grid-stride kernel: whole waves of 148 SMs x resident CTAs, capped by the work
+// grid size for a grid-stride kernel: whole waves of the SMs x resident CTAs, capped by the work
 static inline int tg_grid(const tgpu_ctx* ctx, int64_t work_items, int items_per_block, int ctas_per_sm)
 {
     int64_t need = tg_div_up(work_items, items_per_block);

@@ -195,7 +195,7 @@ __global__ void tg_flush_l2_kernel(int4* buf, int64_t n, int v)
 extern "C" int tgpu_flush_l2(tgpu_ctx* ctx)
 {
     if (ctx) cudaSetDevice(ctx->device);     // callable from any thread: the calling thread's current device may differ
-    // 256 MiB > 126 MB L2
+    // 256 MiB > the 50 MB L2 of an H100
     if (!ctx->flush_buf) {
         ctx->flush_bytes = (size_t)256 << 20;
         TG_CUDA(ctx, cudaMalloc(&ctx->flush_buf, ctx->flush_bytes));

@@ -444,7 +444,7 @@ __device__ __forceinline__ void agg_small_body(P& prog, const DColumns& cols, in
 // tickets layout: [0, WAYS) claims per way, [WAYS] deferred rows, [WAYS + 1] special groups born.
 // P supplies, besides load() / row(): accumulate_global(unsigned long long* acc) - reductions on the record's accumulator words.
 #define TGD_TICKET_WAYS 64
-#define TGD_G_ROWS 2      // (swept on B200 with __launch_bounds__(256, 4): 1 -> 8.3 ms, 2 -> 6.9, 4 -> 8.1, 8 -> 11.1 for 150 M rows / 10 M groups)
+#define TGD_G_ROWS 2      // rows in flight per thread with __launch_bounds__(256, 4)
 
 // {a, b} = the two 64-bit words at p (16-byte aligned) in one L2 transaction, never served from the L1
 __device__ __forceinline__ void tgd_ld_pair(const unsigned long long* p, unsigned long long& a, unsigned long long& b)

@@ -1,4 +1,4 @@
-// groupby.cu — HashAggregationOperator / GroupByHash / grouped accumulators for sm_100a.
+// groupby.cu — HashAggregationOperator / GroupByHash / grouped accumulators for sm_90a.
 //
 // Reference semantics reproduced:
 //   - GroupByHash contract (M/operator/GroupByHash.java:118-125): group ids are dense, 0-based and assigned in
@@ -674,12 +674,12 @@ __global__ void relayout_state_kernel(const unsigned long long* __restrict__ old
 // after the table has grown (their accumulators are untouched, so nothing is counted twice).
 // =====================================================================================================
 // Slot records are AoS: {key, first-row stamp, accumulator words...} padded to a power-of-two number of 8-byte words (W),
-// so one row touches ONE 32/64/128-byte line for its key, stamp and every accumulator (measured with SoA state: 4-5
-// scattered lines per row, 37 ms per 150 M rows with 10 M groups — DRAM read-modify-write bound).
+// so one row touches ONE 32/64/128-byte line for its key, stamp and every accumulator (SoA state would scatter a
+// row over 4-5 lines: DRAM read-modify-write bound).
 __device__ __forceinline__ unsigned long long* gf_rec(unsigned long long* base, int64_t s, int W) { return base + (size_t)s * W; }
 
-// one thread per 16 bytes of the record array: consecutive threads write consecutive addresses (the per-record form - one thread
-// per record, word by word - ran at a tenth of the copy bandwidth: 1.7 ms for a 1 GB table)
+// one thread per 16 bytes of the record array: consecutive threads write consecutive addresses (not one thread per record, word
+// by word, whose stores do not coalesce)
 __global__ void gf_init_kernel(unsigned long long* __restrict__ recs, int64_t cap, int W, AggPlan plan)
 {
     __shared__ unsigned long long init[64];      // W <= 64 (2 + MAX_ACCS words, padded to a power of two)
@@ -796,8 +796,6 @@ __global__ void __launch_bounds__(256) gf_page_kernel(AggPlan plan, DColumns col
             bool have_ticket = false;
             while (true) {
                 unsigned long long* kp = gf_rec(recs, (int64_t)pos, W);
-                // (measured: probing with an atomic "load" instead, to keep the line at its home L2 slice for the reductions
-                //  that follow, was 13 % slower)
                 unsigned long long cur = *((volatile unsigned long long*)kp);
                 if (cur == EMPTY_KEY) {
                     if (!have_ticket) {
@@ -2098,7 +2096,7 @@ struct AggOp : tgpu_op {
         int L = s_L, A = plan.num_accs;
         // (the specialised kernel of a multi-key plan carries no accumulator sets for the special groups)
         const size_t jit_smem = jit_available() && plan.num_keys > 1 ? s_smem - 2 * s_per_slot : s_smem;
-        // at most 3 CTAs per SM: the fourth would cap the kernel at 64 registers (Q1: spills, 15.9 ms instead of 11.2 ms at SF300)
+        // at most 3 CTAs per SM: the fourth would cap the kernel at 64 registers, and Q1 spills there
         int ctas_per_sm = (int)std::max<size_t>(1, std::min<size_t>(3, (smem_limit() + 2048) / (jit_smem + 1024)));
         if (const char* e = getenv("TGPU_AGG_S_MINB")) ctas_per_sm = std::max(1, std::min(4, atoi(e)));
         int grid = tg_grid(ctx, n, S_THREADS * 4, ctas_per_sm);

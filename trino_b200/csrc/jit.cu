@@ -1,4 +1,4 @@
-// jit.cu — run-time specialisation of kernels with NVRTC for sm_100a.
+// jit.cu — run-time specialisation of kernels with NVRTC for sm_90a.
 //
 // Trino compiles every filter/projection/accumulator into JVM bytecode at plan time
 // (M/sql/gen/ExpressionCompiler.java:50-85, M/operator/aggregation/AccumulatorCompiler.java).  The GPU analogue is
@@ -93,7 +93,7 @@ const char* jit_unavailable_reason()
     return g_api.why.c_str();
 }
 
-// compile (prelude + body) for sm_100a; returns the cubin.  Needs no GPU: used by the CPU tests as well.
+// compile (prelude + body) for sm_90a; returns the cubin.  Needs no GPU: used by the CPU tests as well.
 int jit_compile_cubin(tgpu_ctx* ctx, const std::string& body, std::string* cubin)
 {
     {
@@ -105,7 +105,7 @@ int jit_compile_cubin(tgpu_ctx* ctx, const std::string& body, std::string* cubin
     nvrtcProgram prog = nullptr;
     int r = g_api.nvrtcCreateProgram(&prog, src.c_str(), "tgpu_jit.cu", 0, nullptr, nullptr);
     if (r != 0) return tg_fail(ctx, TGPU_ERR_CUDA, "nvrtcCreateProgram failed (%d)", r);
-    const char* opts[] = {"--gpu-architecture=sm_100a", "--std=c++17", "--fmad=false", "-lineinfo", "-default-device"};
+    const char* opts[] = {"--gpu-architecture=sm_90a", "--std=c++17", "--fmad=false", "-lineinfo", "-default-device"};
     r = g_api.nvrtcCompileProgram(prog, 5, opts);
     if (r != 0) {
         size_t n = 0;

@@ -8,7 +8,7 @@ namespace tg {
 
 bool jit_available();
 const char* jit_unavailable_reason();
-// compile device_lib.cuh + body for sm_100a and return the cubin (works without a GPU)
+// compile device_lib.cuh + body for sm_90a and return the cubin (works without a GPU)
 int jit_compile_cubin(tgpu_ctx* ctx, const std::string& body, std::string* cubin);
 // compiled + loaded + cached kernel handle (CUfunction) for the current device
 int jit_get_function(tgpu_ctx* ctx, const std::string& body, const char* kernel_name, void** fn_out);

@@ -1,4 +1,4 @@
-// join.cu — hash join build + probe for sm_100a.
+// join.cu — hash join build + probe for sm_90a.
 //
 // Reference semantics reproduced (bit-exact on address indices and output row order):
 //   build : PagesIndex.addPage (M/operator/PagesIndex.java:224-256) keeps every build row; the address
@@ -13,7 +13,7 @@
 //           LookupJoinPageBuilder.build (LookupJoinPageBuilder.java:119-160): output rows in probe order,
 //           within one probe row in chain order; probe columns first, then build output columns.
 //
-// B200 design: the table is an open-addressing array of 16-byte slots {int64 key, int32 head} so that one
+// Design: the table is an open-addressing array of 16-byte slots {int64 key, int32 head} so that one
 // probe touches exactly one 32-byte sector; the deterministic "head = highest row" of the sequential
 // reference insert order is obtained with atomicMax, and duplicate chains are materialised by a radix sort
 // of (slot,row) pairs only when duplicates exist.  Slot placement (mix(key) & mask, linear probing) is not
@@ -216,8 +216,7 @@ __global__ void __launch_bounds__(256) join_probe_kernel(ColRef key, int kind, i
             if (ok[j] && k[j] != EMPTY_KEY) s[j] = __ldg((const int4*)&table[pos[j]]);
             else s[j] = make_int4(0, (int)0x80000000, -1, 0);
         }
-        // each row walks its probe sequence on its own (measured alternative: lock-step rounds over the ROWS rows of a
-        // thread were ~15 % slower on B200)
+        // each row walks its probe sequence on its own rather than in lock-step rounds over the ROWS rows of a thread
 #pragma unroll
         for (int j = 0; j < ROWS; j++) {
             int64_t i = base + (int64_t)j * blockDim.x;
@@ -704,11 +703,10 @@ static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
                        unsigned long long* matches)
 {
     const unsigned int mask32 = (unsigned int)geo.mask;
-    // 8 CTAs per SM (32 registers): full occupancy is worth more than the registers (measured 4.9 -> 3.4 ms at SF100)
+    // 8 CTAs per SM (32 registers): full occupancy is worth more than the registers
     if (geo.mode == 2 && getenv("TGPU_JOIN_SPAN")) {
-        // TMA-staged table spans (falls back per tile when the keys are not clustered).  Opt-in: measured 9 % SLOWER than the lean kernel on
-        // the SF100 workload (2.73 vs 2.50 ms) - with the dense table the lean kernel already moves its 15.6 GB at 0.95 of the measured copy
-        // bandwidth, and the span kernel pays a block-wide span reduction plus a second dependent DRAM round trip per tile
+        // TMA-staged table spans (falls back per tile when the keys are not clustered).  Opt-in: with the dense table the lean kernel
+        // already streams the table once, and the span kernel pays a block-wide span reduction plus a second dependent DRAM round trip per tile
         auto k = join_probe_span_kernel<GATHER>;
         TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, geo.kmin, geo.shift, special_head, out, g, matches);
     }
@@ -731,7 +729,7 @@ static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
 // A probe page without key locality (the survey's variant B, or any join whose probe side is not clustered on the join key) pays one
 // random DRAM sector per array it touches for a row: the 16-byte slot, then one sector per slot-ordered payload column.  The wide table
 // holds the same slots at a 32-byte stride with up to two payload cells (8 bytes each) behind key and head, so that a row costs ONE
-// random sector whatever the number of payload columns - and one 256-bit load (LDG.E.256) instead of three dependent-address loads.
+// random sector whatever the number of payload columns - and two independent 128-bit loads instead of three dependent-address loads.
 // On a key-ordered probe page the bytes are the same as slot table + slot-ordered payload arrays, read front to back.
 // Built next to the 16-byte table (which the index-only probe, the duplicate chains and every generic kernel keep using).
 struct __align__(32) WideSlot {
@@ -741,18 +739,21 @@ struct __align__(32) WideSlot {
     unsigned long long cell[2];
 };
 
-// LD: 0 = one 256-bit read-only load; 3 = the same with an explicit 64-byte L2 fetch size (LDG...LTC64B); 5 = two 128-bit loads
+// sm_90 has no 256-bit load: a slot is read as the two 128-bit halves of its 32-byte sector, which costs one DRAM sector all the same.
+// LD: 0 = plain read-only loads; 3 = the same with an explicit 64-byte L2 fetch size
 template <int LD>
 __device__ __forceinline__ WideSlot wide_load(const WideSlot* p)
 {
     WideSlot w;
     unsigned long long kh;
-    if (LD == 3) asm("ld.global.nc.L2::64B.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(w.key), "=l"(kh), "=l"(w.cell[0]), "=l"(w.cell[1]) : "l"(p));
-    else if (LD == 5) {
+    if (LD == 3) {
+        asm("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2];" : "=l"(w.key), "=l"(kh) : "l"(p));
+        asm("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2+16];" : "=l"(w.cell[0]), "=l"(w.cell[1]) : "l"(p));
+    }
+    else {
         asm("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(w.key), "=l"(kh) : "l"(p));
         asm("ld.global.nc.v2.u64 {%0,%1}, [%2+16];" : "=l"(w.cell[0]), "=l"(w.cell[1]) : "l"(p));
     }
-    else asm("ld.global.nc.v4.u64 {%0,%1,%2,%3}, [%4];" : "=l"(w.key), "=l"(kh), "=l"(w.cell[0]), "=l"(w.cell[1]) : "l"(p));
     w.head = (int)(unsigned int)kh;
     w.pad = 0;
     return w;
@@ -901,9 +902,8 @@ static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
     const char* e = getenv("TGPU_JOIN_WIDE_SHAPE");
     int shape = e ? atoi(e) : 28;
     const char* le = getenv("TGPU_JOIN_WIDE_LOAD");
-    int ld = le ? atoi(le) : 3;       // measured on the shuffled SF100 probe: 0 -> 17.87 ms, 3 -> 17.37 ms, 5 -> 19.5 ms
+    int ld = le ? atoi(le) : 3;
     if (shape == 28 && ld == 3) return launch_wide_shape<2, 8, 3>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
-    if (shape == 28 && ld == 5) return launch_wide_shape<2, 8, 5>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
     switch (shape) {
         case 18: return launch_wide_shape<1, 8>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
         case 26: return launch_wide_shape<2, 6>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
@@ -1340,7 +1340,7 @@ struct JoinBuildOp : tgpu_op {
             int64_t need = (int64_t)((double)rows / lf) + 1;
             cap = 8;   // at least one 8-slot line
             while (cap < need) cap <<= 1;
-            // line layouts (modes 1 / 2) want lines at most about half full (measured: exp_join_summary in profiles/), unless the keys
+            // line layouts (modes 1 / 2) want lines at most about half full, unless the keys
             // fill their lines evenly: candidates are tried in this order, each judged by the rows that had to leave their home line
             //   mode 2, base capacity  : "dense" - e.g. TPC-H order keys: every line of 32 key values holds exactly its 8 keys
             //   mode 2, 2 x capacity   : a line expects ~4 keys (random subsets of a dense domain: what a hash exchange leaves on a rank)

@@ -774,8 +774,8 @@ struct XchgGeom {
 };
 
 // Local destinations and <= 8 partitions: warp-granular kernels.  Peer destinations: CTA-granular kernels - a warp-granular
-// scatter keeps 8 x more destination streams open per SM, and on 8 GPUs (7 peer apertures) that fell off a cliff
-// (340 ms instead of 15 ms per 600 M rows, measured), most likely peer-aperture TLB reach.
+// scatter keeps 8 x more destination streams open per SM, which on 8 GPUs (7 peer apertures) overruns the reach of the
+// peer-aperture TLBs.
 static XchgGeom xchg_geom(tgpu_ctx* ctx, int64_t n, int P, bool remote)
 {
     XchgGeom g;

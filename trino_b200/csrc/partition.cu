@@ -1,4 +1,4 @@
-// partition.cu — PagePartitioner / PartitionedOutputOperator for sm_100a, and the NCCL all-to-all exchange.
+// partition.cu — PagePartitioner / PartitionedOutputOperator for sm_90a, and the NCCL all-to-all exchange.
 //
 // Reference semantics reproduced:
 //   - partition id = bucketToPartition[ processRawHash(rowHash, bucketCount) ] with rowHash folded as

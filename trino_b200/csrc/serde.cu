@@ -12,7 +12,7 @@
 //                     VARIABLE_WIDTH: int32 nonNullCount | ending offsets of the non-NULL positions (from 0) | bytes
 //                     (S/block/VariableWidthBlockEncoding.java:57-146)
 //
-// B200 shape: the byte stream lives in HOST memory (it goes to / comes from the HTTP exchange), so the device only does the two
+// Shape: the byte stream lives in HOST memory (it goes to / comes from the HTTP exchange), so the device only does the two
 // data-parallel pieces per column — the NULL bit transform (Arrow LSB-first validity <-> MSB-first is-NULL bits: one byte in, one
 // byte out) and the NULL compaction / expansion of the values (ordered stream compaction, CUB) — and every piece is copied
 // straight between its place in the pinned stream and the device with cudaMemcpyAsync.  Small fields are written by the host.
