@@ -2,6 +2,7 @@
 // translation units of libtrino_gpu.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <cub/cub.cuh>
 #include <stdint.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -17,6 +18,38 @@
 #include "device_lib.cuh"
 
 struct ncclComm;
+
+// ------------------------------------------------------------------------------------------------
+// device scratch: the small counters and flags operators read back after a kernel.  Every user owns its own words, so
+// no operator can overwrite a value another one has yet to read.
+// ------------------------------------------------------------------------------------------------
+constexpr size_t TG_SCRATCH_BYTES = 1024;     // ctx->d_scratch and ctx->h_scratch
+
+struct TgScratch {
+    // join build
+    int32_t join_build_flags[4];      // [0] special_head, [1] dup flag, [2] rows off their home line, [3] rows more than 8 lines off
+    uint32_t join_gave_up[2];         // rows a trial geometry could not place within its bound
+    long long join_key_range[2];      // min / max insertable key
+    int32_t join_moved[2];            // fingerprint rows that move on to their next hash function
+    // join probe / lookup outer
+    long long join_probe_count;       // matched probe rows
+    long long join_outer_count;       // unvisited build rows
+    // FilterAndProject
+    uint32_t fp_flags[2];             // [0] error bits, [1] any-NULL bit per computed column
+    long long fp_count;               // selected rows
+    // aggregation
+    int32_t agg_small_flags[2];       // path S: [0] table overflow, [1] error bits
+    int32_t agg_tickets[2];           // path G insert: [0] claimed slots, [1] overflow
+    int32_t agg_retry_count[2];       // path G verify: rows that move on to their next hash function
+    uint32_t agg_output_flags[4];     // output: [0] error bits, [2..3] any-NULL bit per column
+    long long agg_finalize_count;     // fused path: used slots
+    uint32_t agg_slice_counts[64];    // fused path: rows per table slice
+    // string dictionary insert: [0] claims / retry count / new strings, [1] overflow, [2..3] new bytes
+    int32_t strdict_counts[4];
+    // page serializer
+    long long serde_count;            // non-NULL positions
+};
+static_assert(sizeof(TgScratch) <= TG_SCRATCH_BYTES, "the scratch words must fit the scratch allocation");
 
 // ------------------------------------------------------------------------------------------------
 // context
@@ -36,9 +69,9 @@ struct tgpu_ctx {
     // pinned staging ring for host pages
     void* staging = nullptr;
     size_t staging_bytes = 0;
-    // 64-byte pinned + device scratch for small readbacks (counters, flags)
+    // pinned staging of small readbacks (tg_read) and the device words they come from
     int64_t* h_scratch = nullptr;
-    int64_t* d_scratch = nullptr;
+    TgScratch* d_scratch = nullptr;
     cudaEvent_t fence_ev = nullptr;     // recorded on this context's stream by an exchange that must not outrun this consumer
     // cache of large device buffers released by operators (all work of a ctx is ordered on its one stream, so a block
     // can be handed to the next request without waiting): multi-GB cudaMallocAsync calls cost milliseconds even from a
@@ -247,6 +280,56 @@ int tg_concat_columns(tgpu_ctx* ctx, const std::vector<const DevColumn*>& parts,
 int tg_slice_column(tgpu_ctx* ctx, const DevColumn& src, int64_t first, int64_t count, DevColumn* out);
 // append `src` to a growing owned column (used by the build-side store)
 int tg_read_i64(tgpu_ctx* ctx, const void* d_ptr, int64_t* out);   // synchronous small readback
+int tg_read(tgpu_ctx* ctx, const void* d_ptr, size_t bytes, void* host_out);   // the same for up to TG_SCRATCH_BYTES
+
+// small utility kernels, enqueued on the ctx stream
+// byte null map (1 = NULL) -> Arrow validity bitmap (1 = valid); *d_any (if given) is or-ed with 1 when a NULL was seen
+int tg_pack_nullmap(tgpu_ctx* ctx, const uint8_t* is_null, int64_t n, uint8_t* bitmap, unsigned int* d_any = nullptr);
+int tg_iota(tgpu_ctx* ctx, int32_t* out, int64_t n, int32_t first = 0);                         // out[i] = first + i
+int tg_add_i32(tgpu_ctx* ctx, const int32_t* in, int64_t n, int32_t delta, int32_t* out);      // out[i] = in[i] + delta
+int tg_fill16(tgpu_ctx* ctx, int4* out, int64_t n, int4 value);                                // out[i] = value
+
+// CUB device-wide algorithms: size query, temporary storage from the pool, run.  Either call failing is TGPU_ERR_CUDA.
+// Iterator and item-count types pass through unchanged: they select the CUB kernels that get instantiated.
+template <typename Call>
+int tg_cub(tgpu_ctx* ctx, Call call)
+{
+    size_t bytes = 0;
+    TG_CUDA(ctx, call(nullptr, bytes));
+    DevBuf tmp;
+    TG_TRY(tmp.alloc(ctx, bytes));
+    TG_CUDA(ctx, call(tmp.p, bytes));
+    return TGPU_OK;
+}
+
+template <typename InIt, typename OutIt, typename NumT>
+int tg_exclusive_sum(tgpu_ctx* ctx, InIt in, OutIt out, NumT n)
+{
+    return tg_cub(ctx, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, n, ctx->stream); });
+}
+
+template <typename InIt, typename FlagIt, typename OutIt, typename CountIt, typename NumT>
+int tg_select_flagged(tgpu_ctx* ctx, InIt in, FlagIt flags, OutIt out, CountIt d_count, NumT n)
+{
+    return tg_cub(ctx, [&](void* tmp, size_t& bytes) { return cub::DeviceSelect::Flagged(tmp, bytes, in, flags, out, d_count, n, ctx->stream); });
+}
+
+template <typename K, typename V, typename NumT>
+int tg_sort_pairs(tgpu_ctx* ctx, const K* keys_in, K* keys_out, const V* values_in, V* values_out, NumT n, int begin_bit, int end_bit)
+{
+    return tg_cub(ctx, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, keys_in, keys_out, values_in, values_out, n, begin_bit, end_bit, ctx->stream);
+    });
+}
+
+template <typename K, typename NumT>
+int tg_sort_keys(tgpu_ctx* ctx, const K* keys_in, K* keys_out, NumT n, int begin_bit, int end_bit)
+{
+    return tg_cub(ctx, [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortKeys(tmp, bytes, keys_in, keys_out, n, begin_bit, end_bit, ctx->stream); });
+}
+
+// int32 positions of the rows whose flag is set, in row order, into `positions` (allocated here); their count into *d_count
+int tg_flagged_positions(tgpu_ctx* ctx, uint8_t* flags, int64_t n, DevBuf* positions, long long* d_count);
 
 // ------------------------------------------------------------------------------------------------
 // operator base (M/operator/Operator.java:21-102)

@@ -1,6 +1,6 @@
 // core.cu — context lifecycle, device memory helpers, page ingestion / gather / readback, and the
 // generic Operator-protocol entry points of the C ABI (include/trino_gpu.h).
-#include <cub/cub.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 #include <map>
 #include <mutex>
@@ -84,9 +84,9 @@ extern "C" int tgpu_ctx_create(int device, tgpu_ctx** out)
     TG_CUDA(ctx, cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t threshold = UINT64_MAX;
     TG_CUDA(ctx, cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &threshold));
-    TG_CUDA(ctx, cudaMallocHost((void**)&ctx->h_scratch, 1024));
-    TG_CUDA(ctx, cudaMalloc((void**)&ctx->d_scratch, 1024));
-    TG_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, 1024, ctx->stream));
+    TG_CUDA(ctx, cudaMallocHost((void**)&ctx->h_scratch, TG_SCRATCH_BYTES));
+    TG_CUDA(ctx, cudaMalloc((void**)&ctx->d_scratch, TG_SCRATCH_BYTES));
+    TG_CUDA(ctx, cudaMemsetAsync(ctx->d_scratch, 0, TG_SCRATCH_BYTES, ctx->stream));
     *out = ctx;
     return TGPU_OK;
 }
@@ -234,35 +234,94 @@ extern "C" int tgpu_ctx_last_kernel_ms(tgpu_ctx* ctx, float* ms)
     return TGPU_OK;
 }
 
-int tg_read_i64(tgpu_ctx* ctx, const void* d_ptr, int64_t* out)
+int tg_read(tgpu_ctx* ctx, const void* d_ptr, size_t bytes, void* host_out)
 {
-    TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (bytes > TG_SCRATCH_BYTES) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "readback of %zu bytes exceeds the %zu-byte staging buffer", bytes, TG_SCRATCH_BYTES);
+    TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_ptr, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = ctx->h_scratch[0];
+    memcpy(host_out, ctx->h_scratch, bytes);
     return TGPU_OK;
+}
+
+int tg_read_i64(tgpu_ctx* ctx, const void* d_ptr, int64_t* out) { return tg_read(ctx, d_ptr, 8, out); }
+
+// ------------------------------------------------------------------------------------------------
+// utility kernels
+// ------------------------------------------------------------------------------------------------
+// Java boolean[] valueIsNull (1 = NULL) -> Arrow validity bitmap (1 = valid); one thread packs 8 rows
+__global__ void tg_pack_nullmap_kernel(const uint8_t* __restrict__ is_null, int64_t n, uint8_t* __restrict__ bitmap, unsigned int* __restrict__ any)
+{
+    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t nbytes = (n + 7) >> 3;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    unsigned int seen = 0;
+    for (; b < nbytes; b += stride) {
+        unsigned int v = 0;
+        int64_t base = b << 3;
+#pragma unroll
+        for (int k = 0; k < 8; k++) {
+            int64_t i = base + k;
+            if (i < n) { if (is_null[i] == 0) v |= 1u << k; else seen = 1; }
+        }
+        bitmap[b] = (uint8_t)v;
+    }
+    if (seen && any) atomicOr(any, 1u);
+}
+
+int tg_pack_nullmap(tgpu_ctx* ctx, const uint8_t* is_null, int64_t n, uint8_t* bitmap, unsigned int* d_any)
+{
+    TG_LAUNCH(ctx, tg_pack_nullmap_kernel, tg_grid(ctx, (n + 7) / 8, 256, 8), 256, 0, is_null, n, bitmap, d_any);
+    return TGPU_OK;
+}
+
+__global__ void tg_iota_kernel(int32_t* out, int64_t n, int32_t first)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) out[i] = first + (int32_t)i;
+}
+
+int tg_iota(tgpu_ctx* ctx, int32_t* out, int64_t n, int32_t first)
+{
+    TG_LAUNCH(ctx, tg_iota_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, out, n, first);
+    return TGPU_OK;
+}
+
+__global__ void tg_add_i32_kernel(const int32_t* __restrict__ in, int64_t n, int32_t delta, int32_t* __restrict__ out)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) out[i] = in[i] + delta;
+}
+
+int tg_add_i32(tgpu_ctx* ctx, const int32_t* in, int64_t n, int32_t delta, int32_t* out)
+{
+    TG_LAUNCH(ctx, tg_add_i32_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, in, n, delta, out);
+    return TGPU_OK;
+}
+
+__global__ void tg_fill16_kernel(int4* out, int64_t n, int4 value)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) out[i] = value;
+}
+
+int tg_fill16(tgpu_ctx* ctx, int4* out, int64_t n, int4 value)
+{
+    TG_LAUNCH(ctx, tg_fill16_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, out, n, value);
+    return TGPU_OK;
+}
+
+int tg_flagged_positions(tgpu_ctx* ctx, uint8_t* flags, int64_t n, DevBuf* positions, long long* d_count)
+{
+    TG_TRY(positions->alloc(ctx, (size_t)n * 4));
+    return tg_select_flagged(ctx, thrust::counting_iterator<int32_t>(0), flags, positions->as<int32_t>(), d_count, (int)n);
 }
 
 // ------------------------------------------------------------------------------------------------
 // ingestion kernels
 // ------------------------------------------------------------------------------------------------
-// Java boolean[] valueIsNull (1 = NULL) -> Arrow validity bitmap (1 = valid); one thread packs 8 rows
-__global__ void tg_pack_bytemap_kernel(const uint8_t* __restrict__ is_null, int64_t n, uint8_t* __restrict__ bitmap)
-{
-    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t nbytes = (n + 7) >> 3;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; b < nbytes; b += stride) {
-        uint32_t v = 0;
-        int64_t base = b << 3;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            int64_t i = base + k;
-            if (i < n && is_null[i] == 0) v |= 1u << k;
-        }
-        bitmap[b] = (uint8_t)v;
-    }
-}
-
 // fixed-width gather: out[i] = src[idx[i]] (idx == nullptr -> broadcast of row 0); idx < 0 -> NULL row
 template <typename T>
 __global__ void tg_gather_fixed_kernel(const T* __restrict__ src, const int32_t* __restrict__ idx, int64_t n, T* __restrict__ out)
@@ -348,15 +407,9 @@ int tg_gather_column(tgpu_ctx* ctx, const DevColumn& src, const int32_t* d_idx, 
         DevBuf len;
         TG_TRY(len.alloc(ctx, (size_t)(n + 1) * 4));
         TG_LAUNCH(ctx, tg_utf8_lengths_kernel, grid, threads, 0, src.offsets, d_idx, n, len.as<int32_t>());
-        size_t tmp_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, len.as<int32_t>(), r.own_offsets->as<int32_t>(), n + 1, ctx->stream);
-        DevBuf tmp;
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, len.as<int32_t>(), r.own_offsets->as<int32_t>(), n + 1, ctx->stream));
+        TG_TRY(tg_exclusive_sum(ctx, len.as<int32_t>(), r.own_offsets->as<int32_t>(), n + 1));
         int32_t total = 0;
-        TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, r.own_offsets->as<int32_t>() + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        total = *(int32_t*)ctx->h_scratch;
+        TG_TRY(tg_read(ctx, r.own_offsets->as<int32_t>() + n, 4, &total));
         TG_TRY(alloc_shared(ctx, (size_t)total, &r.own_data));
         TG_LAUNCH(ctx, tg_utf8_copy_kernel, grid, threads, 0, (const uint8_t*)src.data, src.offsets, d_idx, n,
                   r.own_offsets->as<int32_t>(), r.own_data->as<uint8_t>());
@@ -381,13 +434,6 @@ int tg_gather_column(tgpu_ctx* ctx, const DevColumn& src, const int32_t* d_idx, 
     return TGPU_OK;
 }
 
-__global__ void tg_iota_kernel(int32_t* out, int64_t n, int32_t first)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) out[i] = first + (int32_t)i;
-}
-
 int tg_slice_column(tgpu_ctx* ctx, const DevColumn& src, int64_t first, int64_t count, DevColumn* out)
 {
     // byte-aligned fixed-width slices without nulls are plain copies; everything else goes through gather
@@ -404,7 +450,7 @@ int tg_slice_column(tgpu_ctx* ctx, const DevColumn& src, int64_t first, int64_t 
     }
     DevBuf idx;
     TG_TRY(idx.alloc(ctx, (size_t)count * 4));
-    TG_LAUNCH(ctx, tg_iota_kernel, tg_grid(ctx, count, 1024, 8), 256, 0, idx.as<int32_t>(), count, (int32_t)first);
+    TG_TRY(tg_iota(ctx, idx.as<int32_t>(), count, (int32_t)first));
     return tg_gather_column(ctx, src, idx.as<int32_t>(), count, false, out);
 }
 
@@ -431,13 +477,6 @@ __global__ void tg_concat_validity_kernel(ConcatParts parts, int64_t n, uint8_t*
         }
         out[b] = (uint8_t)v;
     }
-}
-
-__global__ void tg_rebase_offsets_kernel(const int32_t* __restrict__ src, int64_t count, int32_t delta, int32_t* __restrict__ dst)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < count; i += stride) dst[i] = src[i] + delta;
 }
 
 int tg_concat_columns(tgpu_ctx* ctx, const std::vector<const DevColumn*>& parts, DevColumn* out)
@@ -474,8 +513,7 @@ int tg_concat_columns(tgpu_ctx* ctx, const std::vector<const DevColumn*>& parts,
         for (size_t c = 0; c < parts.size(); c++) {
             int64_t len = parts[c]->length;
             if (len == 0) continue;
-            TG_LAUNCH(ctx, tg_rebase_offsets_kernel, tg_grid(ctx, len + 1, 1024, 8), 256, 0, parts[c]->offsets, len + 1, (int32_t)(byte - first[c]),
-                      r.own_offsets->as<int32_t>() + row);
+            TG_TRY(tg_add_i32(ctx, parts[c]->offsets, len + 1, (int32_t)(byte - first[c]), r.own_offsets->as<int32_t>() + row));
             if (last[c] > first[c])
                 TG_CUDA(ctx, cudaMemcpyAsync(r.own_data->as<char>() + byte, (const char*)parts[c]->data + first[c], (size_t)(last[c] - first[c]), cudaMemcpyDeviceToDevice, ctx->stream));
             row += len;
@@ -580,7 +618,7 @@ static int ingest_value_column(tgpu_ctx* ctx, const tgpu_column* col, bool devic
             const void* d_raw = nullptr;
             TG_TRY(put_buffer(ctx, col->validity, (size_t)n, device, &raw, &d_raw));
             TG_TRY(alloc_shared(ctx, (size_t)((n + 7) / 8), &r.own_validity));
-            TG_LAUNCH(ctx, tg_pack_bytemap_kernel, tg_grid(ctx, (n + 7) / 8, 256, 8), 256, 0, (const uint8_t*)d_raw, n, r.own_validity->as<uint8_t>());
+            TG_TRY(tg_pack_nullmap(ctx, (const uint8_t*)d_raw, n, r.own_validity->as<uint8_t>()));
             r.validity = r.own_validity->as<uint8_t>();
         }
         else {

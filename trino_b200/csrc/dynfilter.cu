@@ -11,9 +11,6 @@
 // rows that reached it and the rows that passed it (the profiler's two counters) and writes a selection flag; the selected rows are
 // compacted with a stable select + per-column gather (output order = input order).  A Domain is `null allowed` + a value set: ALL,
 // NONE, one inclusive range, or a sorted list of discrete values (binary search).
-#include <cub/cub.cuh>
-#include <thrust/iterator/counting_iterator.h>
-
 #include <algorithm>
 
 #include "common.cuh"
@@ -163,18 +160,13 @@ struct DynFilterOp : tgpu_op {
             dd.d[i].values = domains[i].d_values.as<long long>();
             if (!ineffective[i]) dd.active |= 1u << i;
         }
-        DevBuf flags, counters, sel, tmp;
+        DevBuf flags, counters, sel;
         TG_TRY(flags.alloc(ctx, (size_t)n));
         TG_TRY(counters.alloc(ctx, 2 * DF_MAX * 8 + 8));
         TG_CUDA(ctx, cudaMemsetAsync(counters.p, 0, 2 * DF_MAX * 8 + 8, ctx->stream));
         TG_LAUNCH(ctx, df_flags_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, dd, n, flags.as<uint8_t>(), counters.as<unsigned long long>());
-        TG_TRY(sel.alloc(ctx, (size_t)n * 4));
         long long* d_count = (long long*)(counters.as<unsigned long long>() + 2 * DF_MAX);
-        size_t tmp_bytes = 0;
-        thrust::counting_iterator<int32_t> iota(0);
-        cub::DeviceSelect::Flagged(nullptr, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream));
+        TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, d_count));
         std::vector<unsigned long long> h((size_t)2 * DF_MAX + 1);
         TG_CUDA(ctx, cudaMemcpyAsync(h.data(), counters.p, h.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
         TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

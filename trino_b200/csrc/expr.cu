@@ -4,9 +4,6 @@
 // the filter to SelectedPositions, then every projection over the selected positions
 // (ProjectSelectedPositions.processBatch :302-336); FilterAndProjectOperator
 // (M/operator/FilterAndProjectOperator.java:60-95) wraps it.  Output rows keep input order.
-#include <cub/cub.cuh>
-#include <thrust/iterator/counting_iterator.h>
-
 #include "expr.cuh"
 #include "jit.cuh"
 
@@ -313,7 +310,7 @@ struct FilterProjectOp : tgpu_op {
                 if (o->kind == TGPU_OPND_COLUMN && (in.cols[o->index].elem_size() == 0 || in.cols[o->index].elem_size() == 16 || in.cols[o->index].type == TGPU_FLOAT32))
                     return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "expressions over variable-width / 128-bit / REAL channel %d are not supported on the GPU path", o->index);
         }
-        unsigned int* d_err = (unsigned int*)(ctx->d_scratch + 2);
+        unsigned int* d_err = ctx->d_scratch->fp_flags;
         unsigned int* d_anynull = d_err + 1;
         TG_CUDA(ctx, cudaMemsetAsync(d_err, 0, 8, ctx->stream));
         const DProgram* dp = d_prog.as<DProgram>();
@@ -332,9 +329,8 @@ struct FilterProjectOp : tgpu_op {
             }
         }
         if (host_prog.filter_temp >= 0 && !jit_project_chunks) {
-            DevBuf flags, tmp;
+            DevBuf flags;
             TG_TRY(flags.alloc(ctx, (size_t)n));
-            TG_TRY(sel.alloc(ctx, (size_t)n * 4));
             TG_TRY(jit_prepare(in));
             if (jit_filter) {
                 long long n_arg = n;
@@ -343,12 +339,8 @@ struct FilterProjectOp : tgpu_op {
                 TG_TRY(jit_launch(ctx, jit_filter, tg_grid(ctx, n, FP_THREADS, jit_blocks_per_sm(jit_filter, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
             else TG_LAUNCH(ctx, fp_filter_kernel, grid, FP_THREADS, 0, dp, cols, n, flags.as<uint8_t>(), d_err);
-            long long* d_count = (long long*)(ctx->d_scratch + 4);
-            size_t tmp_bytes = 0;
-            thrust::counting_iterator<int32_t> iota(0);
-            cub::DeviceSelect::Flagged(nullptr, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream);
-            TG_TRY(tmp.alloc(ctx, tmp_bytes));
-            TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream));
+            long long* d_count = &ctx->d_scratch->fp_count;
+            TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, d_count));
             TG_TRY(tg_read_i64(ctx, d_count, &m));
             int64_t errw = 0;
             TG_TRY(tg_read_i64(ctx, d_err, &errw));
@@ -360,10 +352,7 @@ struct FilterProjectOp : tgpu_op {
         DevPage outp;
         outp.rows = m;
         outp.cols.resize(projections.size());
-        OutCols oc;
-        memset(&oc, 0, sizeof(oc));
-        std::vector<std::shared_ptr<DevBuf>> nullmaps;
-        std::vector<int> computed_at;
+        ComputedCols cc;
         for (size_t pi = 0; pi < projections.size(); pi++) {
             const tgpu_projection& pr = projections[pi];
             if (pr.kind == 0) {
@@ -371,51 +360,73 @@ struct FilterProjectOp : tgpu_op {
                 if (!d_sel) outp.cols[pi] = in.cols[pr.index];       // InputPageProjection on all positions: the block itself
                 else TG_TRY(tg_gather_column(ctx, in.cols[pr.index], d_sel, m, false, &outp.cols[pi]));
             }
-            else {
-                DevColumn& c = outp.cols[pi];
-                c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : TGPU_INT64;
-                c.length = m;
-                c.own_data = std::make_shared<DevBuf>();
-                TG_TRY(c.own_data->alloc(ctx, (size_t)m * c.elem_size()));
-                c.data = c.own_data->p;
-                auto nm = std::make_shared<DevBuf>();
-                TG_TRY(nm->alloc(ctx, (size_t)m));
-                int k = oc.count++;
-                oc.temp[k] = pr.index;
-                oc.vtype[k] = pr.vtype;
-                oc.data[k] = c.own_data->p;
-                oc.nullmap[k] = nm->as<uint8_t>();
-                nullmaps.push_back(nm);
-                computed_at.push_back((int)pi);
-            }
+            else TG_TRY(add_computed(pr, m, (int)pi, &outp, &cc));
         }
-        if (oc.count > 0) {
+        if (cc.oc.count > 0) {
             int pgrid = tg_grid(ctx, m, FP_THREADS, 8);
             TG_TRY(jit_prepare(in));
             if (jit_project) {
                 long long m_arg = m;
-                void* params[6] = {&cols, &d_sel, &m_arg, &oc, &d_err, &d_anynull};
+                void* params[6] = {&cols, &d_sel, &m_arg, &cc.oc, &d_err, &d_anynull};
                 TG_TRY(jit_launch(ctx, jit_project, tg_grid(ctx, m, FP_THREADS, jit_blocks_per_sm(jit_project, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
-            else TG_LAUNCH(ctx, fp_project_kernel, pgrid, FP_THREADS, 0, dp, cols, d_sel, m, oc, d_err, d_anynull);
-            int64_t word = 0;
-            TG_TRY(tg_read_i64(ctx, d_err, &word));
-            TG_TRY(raise(word & 0xFFFFFFFFLL));
-            uint32_t any_null = (uint32_t)((uint64_t)word >> 32);
-            for (int k = 0; k < oc.count; k++) {
-                if (!((any_null >> k) & 1)) continue;
-                DevColumn& c = outp.cols[computed_at[k]];
-                c.own_validity = std::make_shared<DevBuf>();
-                TG_TRY(c.own_validity->alloc(ctx, (size_t)((m + 7) / 8)));
-                TG_TRY(pack_nullmap(nullmaps[k]->as<uint8_t>(), m, c.own_validity->as<uint8_t>()));
-                c.validity = c.own_validity->as<uint8_t>();
-            }
+            else TG_LAUNCH(ctx, fp_project_kernel, pgrid, FP_THREADS, 0, dp, cols, d_sel, m, cc.oc, d_err, d_anynull);
+            TG_TRY(finish_computed(cc, d_err, &outp));
         }
         pending.push_back(tg_make_owned_page(std::move(outp)));
         return TGPU_OK;
     }
 
-    int pack_nullmap(const uint8_t* nullmap, int64_t m, uint8_t* bitmap);
+    // computed projection columns of one output page: their buffers as the project kernel sees them, and where they go
+    struct ComputedCols {
+        OutCols oc;
+        std::vector<std::shared_ptr<DevBuf>> nullmaps;   // one byte per row, 1 = NULL
+        std::vector<int> at;                             // output column of each computed column
+        ComputedCols() { memset(&oc, 0, sizeof(oc)); }
+    };
+
+    // allocate output column `pi` (m rows) of computed projection `pr` and its byte null map
+    int add_computed(const tgpu_projection& pr, int64_t m, int pi, DevPage* outp, ComputedCols* cc)
+    {
+        DevColumn& c = outp->cols[pi];
+        c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : TGPU_INT64;
+        c.length = m;
+        c.own_data = std::make_shared<DevBuf>();
+        TG_TRY(c.own_data->alloc(ctx, (size_t)m * c.elem_size()));
+        c.data = c.own_data->p;
+        auto nm = std::make_shared<DevBuf>();
+        TG_TRY(nm->alloc(ctx, (size_t)m));
+        int k = cc->oc.count++;
+        cc->oc.temp[k] = pr.index;
+        cc->oc.vtype[k] = pr.vtype;
+        cc->oc.data[k] = c.own_data->p;
+        cc->oc.nullmap[k] = nm->as<uint8_t>();
+        cc->nullmaps.push_back(std::move(nm));
+        cc->at.push_back(pi);
+        return TGPU_OK;
+    }
+
+    // after the project kernel: raise its error bits, then give validity to the computed columns that hold a NULL
+    int finish_computed(const ComputedCols& cc, unsigned int* d_err, DevPage* outp)
+    {
+        int64_t word = 0;
+        TG_TRY(tg_read_i64(ctx, d_err, &word));
+        TG_TRY(raise(word & 0xFFFFFFFFLL));
+        uint32_t any_null = (uint32_t)((uint64_t)word >> 32);
+        for (int k = 0; k < cc.oc.count; k++)
+            if ((any_null >> k) & 1) TG_TRY(attach_validity(cc.nullmaps[k]->as<uint8_t>(), &outp->cols[cc.at[k]]));
+        return TGPU_OK;
+    }
+
+    // pack the byte null map of c's rows into its validity bitmap
+    int attach_validity(const uint8_t* nullmap, DevColumn* c)
+    {
+        c->own_validity = std::make_shared<DevBuf>();
+        TG_TRY(c->own_validity->alloc(ctx, (size_t)((c->length + 7) / 8)));
+        TG_TRY(tg_pack_nullmap(ctx, nullmap, c->length, c->own_validity->as<uint8_t>()));
+        c->validity = c->own_validity->as<uint8_t>();
+        return TGPU_OK;
+    }
 
     // chunked two-pass form: handled = false (and *m_out = n) when every row is selected
     int add_input_chunked(const DevPage& in, const DColumns& cols, int64_t n, unsigned int* d_err, unsigned int* d_anynull, bool* handled, int64_t* m_out)
@@ -451,19 +462,19 @@ struct FilterProjectOp : tgpu_op {
         DevPage outp;
         outp.rows = m;
         outp.cols.resize(projections.size());
-        OutCols oc;
-        memset(&oc, 0, sizeof(oc));
-        std::vector<std::shared_ptr<DevBuf>> nullmaps, pass_nullmaps;
-        std::vector<int> computed_at, pass_at;
+        ComputedCols cc;
+        OutCols& oc = cc.oc;
+        std::vector<std::shared_ptr<DevBuf>> pass_nullmaps;
+        std::vector<int> pass_at;
         for (size_t pi = 0; pi < projections.size(); pi++) {
             const tgpu_projection& pr = projections[pi];
-            DevColumn& c = outp.cols[pi];
-            c.length = m;
-            c.own_data = std::make_shared<DevBuf>();
             if (pr.kind == 0) {
                 if (pr.index < 0 || pr.index >= (int32_t)in.cols.size()) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "projection channel out of range");
                 const DevColumn& src = in.cols[pr.index];
+                DevColumn& c = outp.cols[pi];
                 c.type = src.type;
+                c.length = m;
+                c.own_data = std::make_shared<DevBuf>();
                 TG_TRY(c.own_data->alloc(ctx, (size_t)m * src.elem_size()));
                 c.data = c.own_data->p;
                 int k = oc.pass_count++;
@@ -477,20 +488,7 @@ struct FilterProjectOp : tgpu_op {
                 pass_nullmaps.push_back(nm);
                 pass_at.push_back((int)pi);
             }
-            else {
-                c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : TGPU_INT64;
-                TG_TRY(c.own_data->alloc(ctx, (size_t)m * c.elem_size()));
-                c.data = c.own_data->p;
-                auto nm = std::make_shared<DevBuf>();
-                TG_TRY(nm->alloc(ctx, (size_t)m));
-                int k = oc.count++;
-                oc.temp[k] = pr.index;
-                oc.vtype[k] = pr.vtype;
-                oc.data[k] = c.own_data->p;
-                oc.nullmap[k] = nm->as<uint8_t>();
-                nullmaps.push_back(nm);
-                computed_at.push_back((int)pi);
-            }
+            else TG_TRY(add_computed(pr, m, (int)pi, &outp, &cc));
         }
         {
             DColumns c = cols;
@@ -499,26 +497,9 @@ struct FilterProjectOp : tgpu_op {
             void* params[8] = {&c, &f_arg, &n_arg, &chunk, &off_arg, &oc, &d_err, &d_anynull};
             TG_TRY(jit_launch(ctx, jit_project_chunks, chunks, FPC_T, 0, params));
         }
-        int64_t word = 0;
-        TG_TRY(tg_read_i64(ctx, d_err, &word));
-        TG_TRY(raise(word & 0xFFFFFFFFLL));
-        uint32_t any_null = (uint32_t)((uint64_t)word >> 32);
-        for (int k = 0; k < oc.count; k++) {
-            if (!((any_null >> k) & 1)) continue;
-            DevColumn& c = outp.cols[computed_at[k]];
-            c.own_validity = std::make_shared<DevBuf>();
-            TG_TRY(c.own_validity->alloc(ctx, (size_t)((m + 7) / 8)));
-            TG_TRY(pack_nullmap(nullmaps[k]->as<uint8_t>(), m, c.own_validity->as<uint8_t>()));
-            c.validity = c.own_validity->as<uint8_t>();
-        }
-        for (int k = 0; k < oc.pass_count; k++) {
-            if (!pass_nullmaps[k]) continue;
-            DevColumn& c = outp.cols[pass_at[k]];
-            c.own_validity = std::make_shared<DevBuf>();
-            TG_TRY(c.own_validity->alloc(ctx, (size_t)((m + 7) / 8)));
-            TG_TRY(pack_nullmap(pass_nullmaps[k]->as<uint8_t>(), m, c.own_validity->as<uint8_t>()));
-            c.validity = c.own_validity->as<uint8_t>();
-        }
+        TG_TRY(finish_computed(cc, d_err, &outp));
+        for (int k = 0; k < oc.pass_count; k++)
+            if (pass_nullmaps[k]) TG_TRY(attach_validity(pass_nullmaps[k]->as<uint8_t>(), &outp.cols[pass_at[k]]));
         pending.push_back(tg_make_owned_page(std::move(outp)));
         return TGPU_OK;
     }
@@ -578,29 +559,6 @@ struct FilterProjectOp : tgpu_op {
     int finish() override { finishing = true; return TGPU_OK; }
     bool is_finished() override { return finishing && next_out >= pending.size(); }
 };
-
-__global__ void fp_pack_nullmap_kernel(const uint8_t* __restrict__ is_null, int64_t n, uint8_t* __restrict__ bitmap)
-{
-    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t nbytes = (n + 7) >> 3;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; b < nbytes; b += stride) {
-        uint32_t v = 0;
-        int64_t base = b << 3;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            int64_t i = base + k;
-            if (i < n && is_null[i] == 0) v |= 1u << k;
-        }
-        bitmap[b] = (uint8_t)v;
-    }
-}
-
-int FilterProjectOp::pack_nullmap(const uint8_t* nullmap, int64_t m, uint8_t* bitmap)
-{
-    TG_LAUNCH(ctx, fp_pack_nullmap_kernel, tg_grid(ctx, (m + 7) / 8, 256, 8), 256, 0, nullmap, m, bitmap);
-    return TGPU_OK;
-}
 
 }  // namespace
 

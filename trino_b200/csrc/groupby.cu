@@ -24,9 +24,6 @@
 //                then accumulators are updated with L2 atomics (RED.ADD.F64 / atomicAdd / atomicMin/Max).
 // Keys are packed exactly into one 64-bit word (single key of any fixed width, or several narrow keys with
 // one null bit each, <= 63 bits); other key shapes return NOT_SUPPORTED so the caller keeps the Java operator.
-#include <cub/cub.cuh>
-#include <thrust/iterator/counting_iterator.h>
-
 #include <algorithm>
 #include <map>
 
@@ -430,14 +427,6 @@ struct GSpecial {
     int gid[2];
     int first_row[2];
 };
-
-__global__ void g_table_init_kernel(int4* table, int64_t slots)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    const int4 empty = make_int4(0, (int)0x80000000, -1, 0x7FFFFFFF);
-    for (; i < slots; i += stride) table[i] = empty;
-}
 
 // K1: find or provisionally insert the key of every row.  slot_of_row: slot index, or -2-special.
 // `budget` new slots may be claimed (reserve-then-claim keeps the load factor bounded); exceeding it sets *overflow.
@@ -845,13 +834,6 @@ __global__ void __launch_bounds__(256) gf_slice_ids_kernel(AggPlan plan, DColumn
     if (threadIdx.x < 64 && sh[threadIdx.x]) atomicAdd(&counts[threadIdx.x], sh[threadIdx.x]);
 }
 
-__global__ void gf_iota_kernel(int* __restrict__ out, int64_t n)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) out[i] = (int)i;
-}
-
 // per-chunk histogram form of gf_slice_ids_kernel for the multi-split scatter (chunks as in multisplit.cuh, CTA granularity)
 __global__ void __launch_bounds__(XT) gf_slice_hist_kernel(AggPlan plan, DColumns cols, int64_t n, int64_t chunk, int64_t cap, int shift, int S,
                                                           uint8_t* __restrict__ ids, unsigned int* __restrict__ hist /* [chunks][S] */)
@@ -1250,28 +1232,9 @@ __global__ void agg_key_output_kernel(const long long* __restrict__ keyvals, con
     }
 }
 
-__global__ void nullmap_pack_kernel(const unsigned char* __restrict__ is_null, int64_t n, unsigned char* __restrict__ bitmap, unsigned int* __restrict__ any)
-{
-    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t nbytes = (n + 7) >> 3;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    unsigned int seen = 0;
-    for (; b < nbytes; b += stride) {
-        unsigned int v = 0;
-        int64_t base = b << 3;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            int64_t i = base + k;
-            if (i < n) { if (is_null[i] == 0) v |= 1u << k; else seen = 1; }
-        }
-        bitmap[b] = (unsigned char)v;
-    }
-    if (seen && any) atomicOr(any, 1u);
-}
-
 // SkipAggregationBuilder.buildOutputPage (M/operator/aggregation/partial/SkipAggregationBuilder.java:103-131): every row is its own
 // group, so the intermediate state of an aggregate is a function of that one row - count: 0/1, sum/min/max: the value or NULL,
-// avg: (0/1, value).  One thread per row, all aggregates in one pass; null bytes are packed into bitmaps by nullmap_pack_kernel.
+// avg: (0/1, value).  One thread per row, all aggregates in one pass; null bytes are packed into bitmaps by tg_pack_nullmap.
 #define SKIP_MAX_FNS 24
 struct SkipFn {
     int32_t function, in_ch, mask_ch, in_is_double;
@@ -2107,8 +2070,8 @@ struct AggOp : tgpu_op {
             TG_TRY(blk_ps.alloc(ctx, (size_t)grid * (L + 2) * 4));
             s_grid = grid;
         }
-        int* d_overflow = (int*)(ctx->d_scratch + 6);
-        unsigned int* d_err = (unsigned int*)(ctx->d_scratch + 6) + 1;
+        int* d_overflow = ctx->d_scratch->agg_small_flags;
+        unsigned int* d_err = (unsigned int*)d_overflow + 1;
         TG_CUDA(ctx, cudaMemsetAsync(d_overflow, 0, 8, ctx->stream));
         SmallOut so;
         so.blk_keys = blk_keys.as<unsigned long long>();
@@ -2191,7 +2154,7 @@ struct AggOp : tgpu_op {
     {
         DevBuf nt;
         TG_TRY(nt.alloc(ctx, (size_t)slots * sizeof(GSlot)));
-        TG_LAUNCH(ctx, g_table_init_kernel, tg_grid(ctx, slots, 1024, 8), 256, 0, nt.as<int4>(), slots);
+        TG_TRY(tg_fill16(ctx, nt.as<int4>(), slots, make_int4(0, (int)0x80000000, -1, 0x7FFFFFFF)));   // empty slot
         if (g_slots > 0)
             TG_LAUNCH(ctx, g_rehash_kernel, tg_grid(ctx, g_slots, 1024, 8), 256, 0, g_table.as<GSlot>(), g_slots, nt.as<GSlot>(), (unsigned long long)slots - 1);
         g_table = std::move(nt);
@@ -2251,13 +2214,13 @@ struct AggOp : tgpu_op {
     {
         int64_t n = in.rows;
         if (n > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "page has more than 2^31-1 positions");
-        DevBuf slot_of_row, flags, rank, tmp;
+        DevBuf slot_of_row, flags, rank;
         TG_TRY(slot_of_row.alloc(ctx, (size_t)n * 4));
         TG_TRY(flags.alloc(ctx, (size_t)n + 1));
         TG_TRY(rank.alloc(ctx, (size_t)(n + 1) * 4));
-        int* d_tickets = (int*)(ctx->d_scratch + 8);
+        int* d_tickets = ctx->d_scratch->agg_tickets;
         int* d_overflow = d_tickets + 1;
-        int* d_retry_count = (int*)(ctx->d_scratch + 18);
+        int* d_retry_count = ctx->d_scratch->agg_retry_count;
         int grid = tg_grid(ctx, n, 256, 8);
         DevBuf attempt, retry_a, retry_b;
         if (plan.key_hashed) TG_TRY(attempt.alloc(ctx, (size_t)n));
@@ -2301,13 +2264,9 @@ struct AggOp : tgpu_op {
             TG_LAUNCH(ctx, g_reset_provisional_kernel, 1, 32, 0, g_table.as<GSlot>(), (int64_t)0, g_special.as<GSpecial>());
         }
         TG_LAUNCH(ctx, g_flag_kernel, grid, 256, 0, n, g_table.as<GSlot>(), g_special.as<GSpecial>(), slot_of_row.as<int>(), flags.as<unsigned char>());
-        size_t tmp_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flags.as<unsigned char>(), rank.as<int>(), n + 1, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, flags.as<unsigned char>(), rank.as<int>(), n + 1, ctx->stream));
-        TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, rank.as<int>() + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        int32_t total_new = *(int32_t*)ctx->h_scratch;
+        TG_TRY(tg_exclusive_sum(ctx, flags.as<unsigned char>(), rank.as<int>(), n + 1));
+        int32_t total_new = 0;
+        TG_TRY(tg_read(ctx, rank.as<int>() + n, 4, &total_new));
         if (group_count + total_new > st_cap) {
             int64_t cap = st_cap;
             while (cap < group_count + total_new) cap *= 2;
@@ -2532,21 +2491,15 @@ struct AggOp : tgpu_op {
         TG_TRY(xchg_launch_scatter(ctx, geom, ids.as<uint8_t>(), n, S, block_off.as<long long>(), xc, nullptr, 0, nullptr, !getenv("TGPU_AGG_STABLE_SCATTER")));
         // the slice-ordered page: same channel numbers, data and validity of the channels the plan reads replaced by the copies
         DColumns pcols = cols;
-        std::vector<DevColumn> packed_keep;
+        std::vector<DevBuf> packed_keep;
         const int* stamp_rows = nullptr;
         for (auto& lane : lanes) {
             if (lane.elem == XCHG_ROW_NUMBER) { stamp_rows = lane.buf.as<int>(); continue; }
             if (!lane.nulls) { pcols.cols[lane.col].data = lane.buf.p; continue; }
-            tgpu_column bm;
-            memset(&bm, 0, sizeof(bm));
-            bm.type = TGPU_INT8;
-            bm.flags = TGPU_COL_NULLS_BYTEMAP;
-            bm.length = n;
-            bm.data = lane.buf.p;
-            bm.validity = lane.buf.as<uint8_t>();
-            DevColumn packed;
-            TG_TRY(tg_ingest_column(ctx, &bm, true, &packed));
-            pcols.cols[lane.col].validity = packed.validity;
+            DevBuf packed;
+            TG_TRY(packed.alloc(ctx, (size_t)((n + 7) / 8)));
+            TG_TRY(tg_pack_nullmap(ctx, lane.buf.as<uint8_t>(), n, packed.as<uint8_t>()));
+            pcols.cols[lane.col].validity = packed.as<uint8_t>();
             packed_keep.push_back(std::move(packed));
         }
         // ONE launch over the slice-ordered copy: a grid-stride pass keeps every CTA in the same neighbourhood of the row array, i.e. in
@@ -2583,24 +2536,18 @@ struct AggOp : tgpu_op {
                     return TGPU_OK;
                 }
             }
-            DevBuf ids, ids_sorted, rows_in, rows_sorted, tmp;
+            DevBuf ids, ids_sorted, rows_in, rows_sorted;
             TG_TRY(ids.alloc(ctx, (size_t)n));
             TG_TRY(ids_sorted.alloc(ctx, (size_t)n));
             TG_TRY(rows_in.alloc(ctx, (size_t)n * 4));
             TG_TRY(rows_sorted.alloc(ctx, (size_t)n * 4));
-            unsigned int* d_counts = (unsigned int*)(ctx->d_scratch + 32);   // 64 counters
+            unsigned int* d_counts = ctx->d_scratch->agg_slice_counts;
             TG_CUDA(ctx, cudaMemsetAsync(d_counts, 0, 64 * 4, ctx->stream));
             TG_LAUNCH(ctx, gf_slice_ids_kernel, tg_grid(ctx, n, 256, 8), 256, 0, plan, cols, n, f_cap, log_cap - log_slices, ids.as<uint8_t>(), d_counts);
-            TG_LAUNCH(ctx, gf_iota_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, rows_in.as<int>(), n);
-            size_t tmp_bytes = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ids.as<uint8_t>(), ids_sorted.as<uint8_t>(), rows_in.as<int>(), rows_sorted.as<int>(), (int)n, 0, log_slices, ctx->stream);
-            TG_TRY(tmp.alloc(ctx, tmp_bytes));
-            TG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, ids.as<uint8_t>(), ids_sorted.as<uint8_t>(), rows_in.as<int>(), rows_sorted.as<int>(), (int)n, 0,
-                                                         log_slices, ctx->stream));
+            TG_TRY(tg_iota(ctx, rows_in.as<int>(), n));
+            TG_TRY(tg_sort_pairs(ctx, ids.as<uint8_t>(), ids_sorted.as<uint8_t>(), rows_in.as<int>(), rows_sorted.as<int>(), (int)n, 0, log_slices));
             unsigned int counts[64];
-            TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_counts, 64 * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            memcpy(counts, ctx->h_scratch, sizeof(counts));
+            TG_TRY(tg_read(ctx, d_counts, sizeof(counts), counts));
             int64_t off = 0;
             for (int q = 0; q < S; q++) {
                 if (counts[q]) TG_TRY(run_fused_rows(cols, rows_sorted.as<int>() + off, counts[q]));
@@ -2618,29 +2565,21 @@ struct AggOp : tgpu_op {
     int gf_finalize()
     {
         int64_t total = f_cap + 2;
-        DevBuf flags, slots, tmp;
+        DevBuf flags, slots;
         TG_TRY(flags.alloc(ctx, (size_t)total));
-        TG_TRY(slots.alloc(ctx, (size_t)total * 4));
         TG_LAUNCH(ctx, gf_used_flags_kernel, tg_grid(ctx, total, 1024, 8), 256, 0, f_recs.as<unsigned long long>(), total, gf_words(), flags.as<unsigned char>());
-        long long* d_count = (long long*)(ctx->d_scratch + 22);
-        size_t tmp_bytes = 0;
-        thrust::counting_iterator<int> iota(0);
-        cub::DeviceSelect::Flagged(nullptr, tmp_bytes, iota, flags.as<unsigned char>(), slots.as<int>(), d_count, (int)total, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, iota, flags.as<unsigned char>(), slots.as<int>(), d_count, (int)total, ctx->stream));
+        long long* d_count = &ctx->d_scratch->agg_finalize_count;
+        TG_TRY(tg_flagged_positions(ctx, flags.as<unsigned char>(), total, &slots, d_count));
         int64_t G = 0;
         TG_TRY(tg_read_i64(ctx, d_count, &G));
         group_count = G;
         if (G == 0) return TGPU_OK;
-        DevBuf k_in, k_out, s_out, tmp2;
+        DevBuf k_in, k_out, s_out;
         TG_TRY(k_in.alloc(ctx, (size_t)G * 8));
         TG_TRY(k_out.alloc(ctx, (size_t)G * 8));
         TG_TRY(s_out.alloc(ctx, (size_t)G * 4));
         TG_LAUNCH(ctx, gf_sort_keys_kernel, tg_grid(ctx, G, 1024, 8), 256, 0, f_recs.as<unsigned long long>(), gf_words(), slots.as<int>(), G, k_in.as<unsigned long long>());
-        tmp_bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k_in.as<unsigned long long>(), k_out.as<unsigned long long>(), slots.as<int>(), s_out.as<int>(), (int)G, 0, 64, ctx->stream);
-        TG_TRY(tmp2.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp2.p, tmp_bytes, k_in.as<unsigned long long>(), k_out.as<unsigned long long>(), slots.as<int>(), s_out.as<int>(), (int)G, 0, 64, ctx->stream));
+        TG_TRY(tg_sort_pairs(ctx, k_in.as<unsigned long long>(), k_out.as<unsigned long long>(), slots.as<int>(), s_out.as<int>(), (int)G, 0, 64));
         if (G > st_cap) {
             int64_t keep = group_count;
             group_count = 0;            // nothing to carry over: the dense arrays are rebuilt from the slots
@@ -2883,8 +2822,7 @@ struct AggOp : tgpu_op {
                     if (nm.first == (size_t)-1) continue;
                     auto bm = std::make_shared<DevBuf>();
                     TG_TRY(bm->alloc(ctx, (size_t)((n + 7) / 8)));
-                    TG_LAUNCH(ctx, nullmap_pack_kernel, tg_grid(ctx, (n + 7) / 8, 256, 8), 256, 0, nm.second->as<unsigned char>(), n, bm->as<unsigned char>(),
-                              (unsigned int*)nullptr);
+                    TG_TRY(tg_pack_nullmap(ctx, nm.second->as<uint8_t>(), n, bm->as<uint8_t>()));
                     outp.cols[nm.first].own_validity = bm;
                     outp.cols[nm.first].validity = bm->as<uint8_t>();
                 }
@@ -2949,7 +2887,7 @@ struct AggOp : tgpu_op {
         int64_t G = group_count;
         DevPage outp;
         outp.rows = G;
-        unsigned int* d_err = (unsigned int*)(ctx->d_scratch + 10);
+        unsigned int* d_err = ctx->d_scratch->agg_output_flags;
         unsigned int* d_any = d_err + 2;    // two words of per-column null flags
         TG_CUDA(ctx, cudaMemsetAsync(d_err, 0, 16, ctx->stream));
         int grid = tg_grid(ctx, G, 256, 8);
@@ -3081,8 +3019,7 @@ struct AggOp : tgpu_op {
         for (size_t c = 0; c < outp.cols.size(); c++) {
             bitmaps[c] = std::make_shared<DevBuf>();
             TG_TRY(bitmaps[c]->alloc(ctx, (size_t)((G + 7) / 8)));
-            TG_LAUNCH(ctx, nullmap_pack_kernel, tg_grid(ctx, (G + 7) / 8, 256, 8), 256, 0, nullmaps[c]->as<unsigned char>(), G,
-                      bitmaps[c]->as<unsigned char>(), anyflags.as<unsigned int>() + c);
+            TG_TRY(tg_pack_nullmap(ctx, nullmaps[c]->as<uint8_t>(), G, bitmaps[c]->as<uint8_t>(), anyflags.as<unsigned int>() + c));
         }
         std::vector<unsigned int> h_any(outp.cols.size());
         TG_CUDA(ctx, cudaMemcpyAsync(h_any.data(), anyflags.p, outp.cols.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));

@@ -21,9 +21,6 @@
 #include <algorithm>
 #include <mutex>
 
-#include <cub/cub.cuh>
-#include <thrust/iterator/counting_iterator.h>
-
 #include "rowkeys.cuh"
 
 namespace {
@@ -89,14 +86,6 @@ __device__ __forceinline__ bool join_key(const ColRef& c, int kind, int64_t i, u
     }
     *out = (unsigned long long)v;
     return true;
-}
-
-__global__ void join_table_init_kernel(int4* table, int64_t slots)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    const int4 empty = make_int4(0, (int)0x80000000, -1, 0);
-    for (; i < slots; i += stride) table[i] = empty;
 }
 
 // one thread per build row: claim/find the key's slot, head = max(row).  *dup_flag is set when a key repeats.
@@ -1354,7 +1343,7 @@ struct JoinBuildOp : tgpu_op {
             const int64_t base_cap = cap;
             unsigned long long span = 0, kmin = 0;
             if (hash_mode == 2) {
-                long long* d_range = (long long*)(ctx->d_scratch + 24);
+                long long* d_range = ctx->d_scratch->join_key_range;
                 long long init_range[2] = {INT64_MAX, INT64_MIN};
                 TG_CUDA(ctx, cudaMemcpyAsync(d_range, init_range, sizeof(init_range), cudaMemcpyHostToDevice, ctx->stream));
                 TG_LAUNCH(ctx, join_key_range_kernel, tg_grid(ctx, rows, 1024, 8), 256, 0, tg_colref(bkey), rows, d_range);
@@ -1367,8 +1356,8 @@ struct JoinBuildOp : tgpu_op {
                     kmin = (unsigned long long)h_range[0];
                 }
             }
-            int* d_flags = (int*)ctx->d_scratch;   // [0] special_head, [1] dup flag, [2] rows off their home line, [3] rows more than 8 lines off
-            unsigned int* d_gave_up = (unsigned int*)(ctx->d_scratch + 22);   // rows a trial geometry could not place within its bound
+            int* d_flags = ctx->d_scratch->join_build_flags;
+            unsigned int* d_gave_up = ctx->d_scratch->join_gave_up;
             // attempt 0: dense mode 2; attempt 1: roomy mode 2; attempt 2: mode 1 (or whatever the environment pinned)
             for (int attempt = (hash_mode == 2 && !env_shift && !getenv("TGPU_JOIN_NO_DENSE")) ? 0 : 1; ; attempt++) {
                 if (hash_mode == 2 && attempt >= 2) hash_mode = 1;
@@ -1389,7 +1378,7 @@ struct JoinBuildOp : tgpu_op {
                 }
                 lk->geo.mode = hash_mode;
                 TG_TRY(lk->table.alloc(ctx, (size_t)cap * sizeof(JoinSlot)));
-                TG_LAUNCH(ctx, join_table_init_kernel, tg_grid(ctx, cap, 1024, 8), 256, 0, lk->table.as<int4>(), cap);
+                TG_TRY(tg_fill16(ctx, lk->table.as<int4>(), cap, make_int4(0, (int)0x80000000, -1, 0)));   // empty slot
                 int init[4] = {-1, 0, 0, 0};
                 TG_CUDA(ctx, cudaMemcpyAsync(d_flags, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
                 TG_CUDA(ctx, cudaMemsetAsync(d_gave_up, 0, 8, ctx->stream));
@@ -1435,7 +1424,7 @@ struct JoinBuildOp : tgpu_op {
                 TG_TRY(build_table());
                 lk->attempts = round + 1;
                 if (rows == 0) break;
-                int* d_moved = (int*)(ctx->d_scratch + 16);
+                int* d_moved = ctx->d_scratch->join_moved;
                 TG_CUDA(ctx, cudaMemsetAsync(d_moved, 0, 8, ctx->stream));
                 const DevColumn& fp = lk->store.cols[0];
                 TG_LAUNCH(ctx, join_verify_build_kernel, tg_grid(ctx, rows, 256, 8), 256, 0, key_cols_of(lk->build_keys), (const long long*)fp.data, fp.validity, rows,
@@ -1448,15 +1437,12 @@ struct JoinBuildOp : tgpu_op {
         if (lk->has_dups) {
             // ArrayPositionLinks: chains in descending row order
             const DevColumn& key = lk->store.cols[0];
-            DevBuf keys_in, keys_out, tmp;
+            DevBuf keys_in, keys_out;
             TG_TRY(keys_in.alloc(ctx, (size_t)rows * 8));
             TG_TRY(keys_out.alloc(ctx, (size_t)rows * 8));
             TG_LAUNCH(ctx, join_slot_of_row_kernel, tg_grid(ctx, rows, 256, 8), 256, 0, tg_colref(key), key_kind_of(key.type), rows,
                       lk->table.as<JoinSlot>(), lk->geo, (unsigned long long)cap, keys_in.as<unsigned long long>());
-            size_t tmp_bytes = 0;
-            cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, keys_in.as<unsigned long long>(), keys_out.as<unsigned long long>(), (int)rows, 0, 64, ctx->stream);
-            TG_TRY(tmp.alloc(ctx, tmp_bytes));
-            TG_CUDA(ctx, cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, keys_in.as<unsigned long long>(), keys_out.as<unsigned long long>(), (int)rows, 0, 64, ctx->stream));
+            TG_TRY(tg_sort_keys(ctx, keys_in.as<unsigned long long>(), keys_out.as<unsigned long long>(), (int)rows, 0, 64));
             TG_TRY(lk->links.alloc(ctx, (size_t)rows * 4));
             TG_LAUNCH(ctx, join_links_kernel, tg_grid(ctx, rows, 256, 8), 256, 0, keys_out.as<unsigned long long>(), rows, lk->links.as<int>());
             TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1681,16 +1667,10 @@ struct JoinProbeOp : tgpu_op {
         else {
             if (matches == 0) return TGPU_OK;
             // compact the matched rows (stable): selection list, then sequential-read gathers
-            DevBuf flags, sel, tmp;
+            DevBuf flags, sel;
             TG_TRY(flags.alloc(ctx, (size_t)n));
-            TG_TRY(sel.alloc(ctx, (size_t)n * 4));
             TG_LAUNCH(ctx, join_match_flags_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, jp->as<int>(), n, flags.as<uint8_t>());
-            long long* d_count = (long long*)(ctx->d_scratch + 14);
-            size_t tmp_bytes = 0;
-            thrust::counting_iterator<int32_t> iota(0);
-            cub::DeviceSelect::Flagged(nullptr, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream);
-            TG_TRY(tmp.alloc(ctx, tmp_bytes));
-            TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream));
+            TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, &ctx->d_scratch->join_probe_count));
             outp.rows = matches;
             for (int32_t ch : output_channels) {
                 DevColumn c;
@@ -1748,15 +1728,12 @@ struct JoinProbeOp : tgpu_op {
         bool outer = join_type == TGPU_JOIN_PROBE_OUTER || join_type == TGPU_JOIN_FULL_OUTER;
         const int* links = lookup->has_dups ? lookup->links.as<int>() : nullptr;
         // match counts -> exclusive scan -> output offsets
-        DevBuf counts, offsets, tmp;
+        DevBuf counts, offsets;
         TG_TRY(counts.alloc(ctx, (size_t)(n + 1) * 4));
         TG_TRY(offsets.alloc(ctx, (size_t)(n + 1) * 8));
         int grid = tg_grid(ctx, n, 256 * 4, 8);
         TG_LAUNCH(ctx, join_count_kernel, grid, 256, 0, jp->as<int>(), n, links, single_match, outer ? 1 : 0, counts.as<int>());
-        size_t tmp_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, counts.as<int>(), offsets.as<long long>(), n + 1, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, counts.as<int>(), offsets.as<long long>(), n + 1, ctx->stream));
+        TG_TRY(tg_exclusive_sum(ctx, counts.as<int>(), offsets.as<long long>(), n + 1));
         int64_t total = 0;
         TG_TRY(tg_read_i64(ctx, offsets.as<long long>() + n, &total));
         if (total == 0) return TGPU_OK;
@@ -1828,17 +1805,12 @@ struct JoinOuterOp : tgpu_op {
         done = true;
         const int64_t n = lookup->positions;
         if (n == 0) return TGPU_OK;
-        DevBuf flags, sel, tmp;
+        DevBuf flags, sel;
         TG_TRY(flags.alloc(ctx, (size_t)n));
-        TG_TRY(sel.alloc(ctx, (size_t)n * 4));
         if (lookup->visited.p) TG_LAUNCH(ctx, join_unvisited_flags_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, lookup->visited.as<uint8_t>(), n, flags.as<uint8_t>());
         else TG_CUDA(ctx, cudaMemsetAsync(flags.p, 1, (size_t)n, ctx->stream));     // no tracking probe ever ran: every row is unvisited
-        long long* d_count = (long long*)(ctx->d_scratch + 14);
-        size_t tmp_bytes = 0;
-        thrust::counting_iterator<int32_t> iota(0);
-        cub::DeviceSelect::Flagged(nullptr, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, iota, flags.as<uint8_t>(), sel.as<int32_t>(), d_count, (int)n, ctx->stream));
+        long long* d_count = &ctx->d_scratch->join_outer_count;
+        TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, d_count));
         int64_t m = 0;
         TG_TRY(tg_read_i64(ctx, d_count, &m));
         if (m == 0) return TGPU_OK;

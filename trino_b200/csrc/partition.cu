@@ -15,7 +15,6 @@
 // Device path: one kernel computes row hash -> partition id, a stable radix sort of (partition, row) pairs
 // yields the per-partition position lists, and one gather per column writes partition-contiguous buffers —
 // which are exactly the send buffers of the all-to-all.
-#include <cub/cub.cuh>
 #include <dlfcn.h>
 
 #include <chrono>
@@ -91,21 +90,6 @@ __global__ void partition_rowwise_kernel(const int32_t* __restrict__ ids, int64_
     }
     counts[p] = c;
 }
-
-__global__ void iota32_kernel(int32_t* out, int64_t n)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) out[i] = (int32_t)i;
-}
-
-__global__ void shift_rows_kernel(const int32_t* __restrict__ in, int64_t n, int32_t delta, int32_t* __restrict__ out)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) out[i] = in[i] + delta;
-}
-
 
 // type hash of the single position of a HOST column (the value of a partition constant); same functions as the device's type_hash
 int host_type_hash(tgpu_ctx* ctx, const tgpu_column& c, uint64_t* out)
@@ -184,18 +168,15 @@ struct PartitionOp : tgpu_op {
     // stable sort of rows by partition id: sorted row list + P+2 boundaries (bounds[P]..bounds[P+1] = NULL-channel rows)
     int sort_rows(const int32_t* d_ids, int64_t n, DevBuf* sorted_rows, DevBuf* bounds)
     {
-        DevBuf rows_in, ids_out, tmp;
+        DevBuf rows_in, ids_out;
         TG_TRY(rows_in.alloc(ctx, (size_t)n * 4));
         TG_TRY(ids_out.alloc(ctx, (size_t)n * 4));
         TG_TRY(sorted_rows->alloc(ctx, (size_t)n * 4));
         TG_TRY(bounds->alloc(ctx, (size_t)(partition_count + 2) * 8));
-        TG_LAUNCH(ctx, iota32_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, rows_in.as<int32_t>(), n);
+        TG_TRY(tg_iota(ctx, rows_in.as<int32_t>(), n));
         int bits = 1;
         while ((1 << bits) <= partition_count) bits++;
-        size_t tmp_bytes = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_ids, ids_out.as<int32_t>(), rows_in.as<int32_t>(), sorted_rows->as<int32_t>(), (int)n, 0, bits, ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, d_ids, ids_out.as<int32_t>(), rows_in.as<int32_t>(), sorted_rows->as<int32_t>(), (int)n, 0, bits, ctx->stream));
+        TG_TRY(tg_sort_pairs(ctx, d_ids, ids_out.as<int32_t>(), rows_in.as<int32_t>(), sorted_rows->as<int32_t>(), (int)n, 0, bits));
         int nb = partition_count + 2;
         TG_LAUNCH(ctx, partition_bounds_kernel, (nb + 127) / 128, 128, 0, ids_out.as<int32_t>(), n, nb, bounds->as<long long>());
         return TGPU_OK;
@@ -273,7 +254,7 @@ struct PartitionOp : tgpu_op {
         const int32_t* rows_ptr = sorted_rows.as<int32_t>();
         if (start_row) {
             TG_TRY(shifted.alloc(ctx, (size_t)(n - start_row) * 4));
-            TG_LAUNCH(ctx, shift_rows_kernel, tg_grid(ctx, n - start_row, 1024, 8), 256, 0, sorted_rows.as<int32_t>(), n - start_row, start_row, shifted.as<int32_t>());
+            TG_TRY(tg_add_i32(ctx, sorted_rows.as<int32_t>(), n - start_row, start_row, shifted.as<int32_t>()));
             rows_ptr = shifted.as<int32_t>();
         }
         dim3 grid((unsigned)std::max<int64_t>(1, std::min<int64_t>(tg_div_up(total / P + 1, 256), ctx->sm_count)), (unsigned)P);

@@ -16,7 +16,6 @@
 // data-parallel pieces per column — the NULL bit transform (Arrow LSB-first validity <-> MSB-first is-NULL bits: one byte in, one
 // byte out) and the NULL compaction / expansion of the values (ordered stream compaction, CUB) — and every piece is copied
 // straight between its place in the pinned stream and the device with cudaMemcpyAsync.  Small fields are written by the host.
-#include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
 
@@ -108,21 +107,16 @@ int valid_ranks(tgpu_ctx* ctx, const uint8_t* validity, int64_t n, DevBuf* rank,
     TG_TRY(rank->alloc(ctx, (size_t)(n + 1) * 4));
     thrust::counting_iterator<int64_t> idx(0);
     auto flags = thrust::make_transform_iterator(idx, ValidAt{validity});
-    size_t tmp_bytes = 0;
-    DevBuf tmp;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, flags, rank->as<int>(), (int)(n + 1), ctx->stream);
-    TG_TRY(tmp.alloc(ctx, tmp_bytes));
     // n + 1 outputs: rank[n] = number of valid positions (the iterator is read one past the end: validity buffers are padded to
     // whole bytes and position n of the last byte is a defined bit; when n is a multiple of 8 the scan is split instead)
     if (n % 8 != 0) {
-        TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, flags, rank->as<int>(), (int)(n + 1), ctx->stream));
+        TG_TRY(tg_exclusive_sum(ctx, flags, rank->as<int>(), (int)(n + 1)));
         int32_t total = 0;
-        TG_CUDA(ctx, cudaMemcpyAsync(&total, rank->as<int>() + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        TG_TRY(tg_read(ctx, rank->as<int>() + n, 4, &total));
         *valid_count = total;
         return TGPU_OK;
     }
-    TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, flags, rank->as<int>(), (int)n, ctx->stream));
+    TG_TRY(tg_exclusive_sum(ctx, flags, rank->as<int>(), (int)n));
     int32_t last_rank = 0;
     uint8_t last_byte = 0;
     if (n > 0) {
@@ -211,26 +205,21 @@ extern "C" int tgpu_page_serialize(tgpu_ctx* ctx, const tgpu_page* page, uint8_t
                 TG_TRY(need(4 + valid * es));
                 put_i32(out + pos, (int32_t)valid);
                 pos += 4;
-                DevBuf compact, tmp;
+                DevBuf compact;
                 TG_TRY(compact.alloc(ctx, (size_t)std::max<int64_t>(valid, 1) * es));
-                long long* d_count = (long long*)(ctx->d_scratch + 40);
+                long long* d_count = &ctx->d_scratch->serde_count;
                 thrust::counting_iterator<int64_t> idx(0);
                 auto flags = thrust::make_transform_iterator(idx, ValidAt{col.validity});
-                size_t tmp_bytes = 0;
-#define SERDE_SELECT(T)                                                                                                                       \
-    cub::DeviceSelect::Flagged(nullptr, tmp_bytes, (const T*)col.data, flags, compact.as<T>(), d_count, (int)n, ctx->stream);                \
-    TG_TRY(tmp.alloc(ctx, tmp_bytes));                                                                                                        \
-    TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, (const T*)col.data, flags, compact.as<T>(), d_count, (int)n, ctx->stream));
-                if (es == 16) { SERDE_SELECT(longlong2) }
-                else if (es == 8) { SERDE_SELECT(long long) }
-                else if (es == 4) { SERDE_SELECT(int) }
-                else if (es == 2) { SERDE_SELECT(short) }
-                else { SERDE_SELECT(signed char) }
+#define SERDE_SELECT(T) TG_TRY(tg_select_flagged(ctx, (const T*)col.data, flags, compact.as<T>(), d_count, (int)n))
+                if (es == 16) SERDE_SELECT(longlong2);
+                else if (es == 8) SERDE_SELECT(long long);
+                else if (es == 4) SERDE_SELECT(int);
+                else if (es == 2) SERDE_SELECT(short);
+                else SERDE_SELECT(signed char);
 #undef SERDE_SELECT
                 if (valid) TG_CUDA(ctx, cudaMemcpyAsync(out + pos, compact.p, (size_t)valid * es, cudaMemcpyDeviceToHost, ctx->stream));
                 pos += valid * es;
                 keep.push_back(std::move(compact));
-                keep.push_back(std::move(tmp));
             }
         }
         else {
@@ -240,19 +229,15 @@ extern "C" int tgpu_page_serialize(tgpu_ctx* ctx, const tgpu_page* page, uint8_t
             pos += 4;
             int32_t first = 0, last = 0;
             if (n > 0) {
-                DevBuf ends, compact, tmp;
+                DevBuf ends, compact;
                 TG_TRY(ends.alloc(ctx, (size_t)n * 4));
                 TG_LAUNCH(ctx, serde_end_offsets_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, col.offsets, n, ends.as<int32_t>());
                 const int32_t* src = ends.as<int32_t>();
                 if (has_nulls) {
                     TG_TRY(compact.alloc(ctx, (size_t)std::max<int64_t>(valid, 1) * 4));
-                    long long* d_count = (long long*)(ctx->d_scratch + 40);
                     thrust::counting_iterator<int64_t> idx(0);
                     auto flags = thrust::make_transform_iterator(idx, ValidAt{col.validity});
-                    size_t tmp_bytes = 0;
-                    cub::DeviceSelect::Flagged(nullptr, tmp_bytes, ends.as<int32_t>(), flags, compact.as<int32_t>(), d_count, (int)n, ctx->stream);
-                    TG_TRY(tmp.alloc(ctx, tmp_bytes));
-                    TG_CUDA(ctx, cub::DeviceSelect::Flagged(tmp.p, tmp_bytes, ends.as<int32_t>(), flags, compact.as<int32_t>(), d_count, (int)n, ctx->stream));
+                    TG_TRY(tg_select_flagged(ctx, ends.as<int32_t>(), flags, compact.as<int32_t>(), &ctx->d_scratch->serde_count, (int)n));
                     src = compact.as<int32_t>();
                 }
                 if (valid) TG_CUDA(ctx, cudaMemcpyAsync(out + pos, src, (size_t)valid * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -261,7 +246,6 @@ extern "C" int tgpu_page_serialize(tgpu_ctx* ctx, const tgpu_page* page, uint8_t
                 TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
                 keep.push_back(std::move(ends));
                 keep.push_back(std::move(compact));
-                keep.push_back(std::move(tmp));
             }
             pos += valid * 4;
             const int64_t payload = (int64_t)last - first;

@@ -15,8 +15,6 @@
 //     whose bytes differ - two strings sharing a 64-bit hash - moves on to attempt + 1, a different hash function of the same
 //     bytes: chaining by rehash, never a query failure.
 #pragma once
-#include <cub/cub.cuh>
-
 #include "common.cuh"
 
 namespace tg {
@@ -410,7 +408,7 @@ struct StringDict {
         DevBuf slot_of_row, attempt, retry_a, retry_b;
         TG_TRY(slot_of_row.alloc(ctx, (size_t)n * 4));
         TG_TRY(attempt.alloc(ctx, (size_t)n));
-        int* d_cnt = (int*)(ctx->d_scratch + 48);            // [0] claims / retry count / new strings, [1] overflow, [2..3] new bytes
+        int* d_cnt = ctx->d_scratch->strdict_counts;
         const int32_t* offs = col.offsets;
         const uint8_t* data = (const uint8_t*)col.data;
         const int grid = tg_grid(ctx, n, 256, 8);
@@ -426,18 +424,14 @@ struct StringDict {
                 const int64_t budget = cap / 2 - count;
                 TG_LAUNCH(ctx, sd_insert_kernel, tg_grid(ctx, todo, 256, 8), 256, 0, offs, data, col.validity, rows, todo, attempt.as<uint8_t>(), table.as<StrSlot>(),
                           (unsigned long long)cap - 1, slot_of_row.as<int>(), d_cnt, (int)std::min<int64_t>(std::max<int64_t>(budget, 0), INT32_MAX));
-                TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
-                TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-                memcpy(h, ctx->h_scratch, 8);
+                TG_TRY(tg_read(ctx, d_cnt, 8, h));
                 if (h[1]) { overflow = true; break; }
                 DevBuf& retry = (round & 1) ? retry_b : retry_a;
                 TG_TRY(retry.alloc(ctx, (size_t)todo * 4));
                 TG_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 4, ctx->stream));
                 TG_LAUNCH(ctx, sd_verify_kernel, tg_grid(ctx, todo, 256, 8), 256, 0, offs, data, rows, todo, attempt.as<uint8_t>(), table.as<StrSlot>(), slot_of_row.as<int>(),
                           bytes.as<uint8_t>(), start.as<long long>(), len.as<int>(), retry.as<int>(), d_cnt);
-                TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_cnt, 4, cudaMemcpyDeviceToHost, ctx->stream));
-                TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-                memcpy(h, ctx->h_scratch, 4);
+                TG_TRY(tg_read(ctx, d_cnt, 4, h));
                 if (h[0] == 0) break;
                 rows = retry.as<int>();
                 todo = h[0];
@@ -450,9 +444,7 @@ struct StringDict {
         // new strings: count, make room, append
         TG_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
         TG_LAUNCH(ctx, sd_count_new_kernel, grid, 256, 0, offs, n, table.as<StrSlot>(), slot_of_row.as<int>(), d_cnt, (unsigned long long*)(d_cnt + 2));
-        TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, d_cnt, 16, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        memcpy(h, ctx->h_scratch, 16);
+        TG_TRY(tg_read(ctx, d_cnt, 16, h));
         const int64_t fresh = h[0];
         long long fresh_bytes = 0;
         memcpy(&fresh_bytes, h + 2, 8);
@@ -496,16 +488,12 @@ struct StringDict {
         c.length = n;
         c.own_offsets = std::make_shared<DevBuf>();
         TG_TRY(c.own_offsets->alloc(ctx, (size_t)(n + 1) * 4));
-        DevBuf lens, tmp;
+        DevBuf lens;
         TG_TRY(lens.alloc(ctx, (size_t)(n + 1) * 4));
         TG_LAUNCH(ctx, sd_lens_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, d_ids, d_is_null, n, len.as<int>(), lens.as<int32_t>());
-        size_t tmp_bytes = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, lens.as<int32_t>(), c.own_offsets->as<int32_t>(), (int)(n + 1), ctx->stream);
-        TG_TRY(tmp.alloc(ctx, tmp_bytes));
-        TG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, lens.as<int32_t>(), c.own_offsets->as<int32_t>(), (int)(n + 1), ctx->stream));
-        TG_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch, c.own_offsets->as<int32_t>() + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        const int32_t total = *(int32_t*)ctx->h_scratch;
+        TG_TRY(tg_exclusive_sum(ctx, lens.as<int32_t>(), c.own_offsets->as<int32_t>(), (int)(n + 1)));
+        int32_t total = 0;
+        TG_TRY(tg_read(ctx, c.own_offsets->as<int32_t>() + n, 4, &total));
         if (total < 0) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "variable-width key column of one output page exceeds 2 GB");
         c.own_data = std::make_shared<DevBuf>();
         TG_TRY(c.own_data->alloc(ctx, (size_t)std::max<int32_t>(total, 1)));
