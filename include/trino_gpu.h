@@ -45,7 +45,8 @@ typedef enum tgpu_status {
     TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE = -4, /* NUMERIC_VALUE_OUT_OF_RANGE (M/type/BigintOperators.java:52-84) */
     TGPU_ERR_DIVISION_BY_ZERO = -5,       /* DIVISION_BY_ZERO (M/type/BigintOperators.java:96-106) */
     TGPU_ERR_NOT_SUPPORTED = -6,          /* NOT_SUPPORTED: caller keeps the Java operator */
-    TGPU_ERR_ILLEGAL_STATE = -7           /* IllegalStateException / checkState (protocol misuse) */
+    TGPU_ERR_ILLEGAL_STATE = -7,          /* IllegalStateException / checkState (protocol misuse) */
+    TGPU_ERR_INVALID_CAST_ARGUMENT = -8   /* INVALID_CAST_ARGUMENT (M/type/DoubleOperators.java:159-167: CAST(DOUBLE AS BIGINT) of NaN, +-Infinity, |x| >= 2^63) */
 } tgpu_status;
 
 /* ------------------------------------------------------------------ columnar data model

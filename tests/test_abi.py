@@ -98,6 +98,7 @@ def test_status_names_are_trino_error_codes():
     assert lib.tgpu_status_name(abi.ERR_INSUFFICIENT_RESOURCES) == b"GENERIC_INSUFFICIENT_RESOURCES"
     assert lib.tgpu_status_name(abi.ERR_NUMERIC_VALUE_OUT_OF_RANGE) == b"NUMERIC_VALUE_OUT_OF_RANGE"
     assert lib.tgpu_status_name(abi.ERR_DIVISION_BY_ZERO) == b"DIVISION_BY_ZERO"
+    assert lib.tgpu_status_name(abi.ERR_INVALID_CAST_ARGUMENT) == b"INVALID_CAST_ARGUMENT"
 
 
 def test_no_cpu_fallback_without_device():

@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libtrino_gpu.so")
 # ---- enums (include/trino_gpu.h)
 TGPU_OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_INSUFFICIENT_RESOURCES, ERR_NUMERIC_VALUE_OUT_OF_RANGE = -1, -2, -3, -4
-ERR_DIVISION_BY_ZERO, ERR_NOT_SUPPORTED, ERR_ILLEGAL_STATE = -5, -6, -7
+ERR_DIVISION_BY_ZERO, ERR_NOT_SUPPORTED, ERR_ILLEGAL_STATE, ERR_INVALID_CAST_ARGUMENT = -5, -6, -7, -8
 
 INT64, INT32, INT16, INT8, FLOAT64, UTF8, DICT32, RLE, INT128, FLOAT32 = 1, 2, 3, 4, 5, 7, 8, 9, 10, 11
 COL_NULLS_BYTEMAP = 1

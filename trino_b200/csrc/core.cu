@@ -40,6 +40,7 @@ extern "C" const char* tgpu_status_name(int status)
         case TGPU_ERR_DIVISION_BY_ZERO: return "DIVISION_BY_ZERO";
         case TGPU_ERR_NOT_SUPPORTED: return "NOT_SUPPORTED";
         case TGPU_ERR_ILLEGAL_STATE: return "ILLEGAL_STATE";
+        case TGPU_ERR_INVALID_CAST_ARGUMENT: return "INVALID_CAST_ARGUMENT";
         default: return "UNKNOWN";
     }
 }

@@ -42,7 +42,7 @@ enum {
     TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_IN = 40
 };
 enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2 };
-enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2 };
+enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4 };
 
 enum AccKind {
     ACC_ROWS = 0, ACC_NONNULL = 1, ACC_SUM_F64 = 2, ACC_SUM_I64_LO = 3, ACC_SUM_I64_HI = 4,
@@ -239,8 +239,8 @@ __device__ __forceinline__ Value vm_apply(int op, int vtype, Value a, Value b, V
             rn = a.is_null;
             if (rn) break;
             double x = __longlong_as_double(a.bits);
-            // DoubleMath.roundToLong(x, HALF_UP): NaN / out of range is an error
-            if (!(x >= -9.2233720368547758e18 && x < 9.2233720368547758e18)) *err |= TG_ERR_BIT_OVERFLOW;
+            // DoubleMath.roundToLong(x, HALF_UP): NaN / out of range is INVALID_CAST_ARGUMENT (M/type/DoubleOperators.java:159-167)
+            if (!(x >= -9.2233720368547758e18 && x < 9.2233720368547758e18)) *err |= TG_ERR_BIT_INVALID_CAST;
             else r = llround(x);
             break;
         }
@@ -249,6 +249,35 @@ __device__ __forceinline__ Value vm_apply(int op, int vtype, Value a, Value b, V
     res.bits = r;
     res.is_null = rn;
     return res;
+}
+
+// The error the result of one instruction carries (one TG_ERR_BIT_* or 0): the first error, in the reference's evaluation order,
+// of the operands it evaluates, otherwise its own (`own`, what vm_apply raised).  ea / eb / ec are the errors the operands carry
+// (a column or constant never carries one).  Only the errors carried by the filter and by the outputs are raised, so an operand
+// the reference never evaluates raises nothing:
+//   AND / OR: the left operand's error; none when the left operand is FALSE / TRUE (AndCodeGenerator.java:56-75,
+//             OrCodeGenerator.java:69-70); otherwise the right operand's
+//   BETWEEN:  the value's error; none when the value is NULL; min's; none when min <= value is FALSE; max's
+//             (BetweenCodeGenerator.java:62-80)
+//   calls:    the operands' errors in order, stopping at the first NULL operand (BytecodeUtils.java:303-306), then their own
+//   IS [NOT] NULL, MOV: the operand's
+__device__ __forceinline__ uint32_t vm_error(int op, int vtype, Value a, uint32_t ea, Value b, uint32_t eb, Value c, uint32_t ec, uint32_t own)
+{
+    if (ea) return ea;
+    switch (op) {
+        case TGD_EX_AND: return (!a.is_null && a.bits == 0) ? 0 : eb;
+        case TGD_EX_OR: return (!a.is_null && a.bits != 0) ? 0 : eb;
+        case TGD_EX_BETWEEN:
+            if (a.is_null) return 0;
+            if (eb) return eb;
+            if (!b.is_null && !vm_cmp(TGD_EX_LE, vtype, b.bits, a.bits)) return 0;
+            return ec;
+        case TGD_EX_ADD: case TGD_EX_SUB: case TGD_EX_MUL: case TGD_EX_DIV: case TGD_EX_MOD:
+        case TGD_EX_EQ: case TGD_EX_NE: case TGD_EX_LT: case TGD_EX_LE: case TGD_EX_GT: case TGD_EX_GE:
+            if (a.is_null) return 0;
+            return eb ? eb : own;
+        default: return own;   // one operand
+    }
 }
 
 // ---- accumulators -------------------------------------------------------------------------------------

@@ -89,8 +89,10 @@ __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* _
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t err = 0;
     for (; i < n; i += stride) {
-        uint32_t nb = vm_run(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &err);
+        uint32_t te = 0;
+        uint32_t nb = vm_run(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te);
         int ft = prog->filter_temp;
+        err |= vm_temp_error(te, ft);
         bool sel = !((nb >> ft) & 1) && temps[ft * FP_THREADS + threadIdx.x] != 0;
         flags[i] = sel ? 1 : 0;
     }
@@ -104,14 +106,15 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    uint32_t err = 0, ignored = 0, nulls_seen = 0;
+    uint32_t err = 0, nulls_seen = 0;
     for (; j < m; j += stride) {
         int64_t row = sel ? sel[j] : j;
         int64_t* t = temps + threadIdx.x;
-        uint32_t nb = vm_run(prog, 0, prog->num_filter_insns, cols, row, t, FP_THREADS, 0, &ignored);
-        nb = vm_run(prog, prog->num_filter_insns, prog->num_insns, cols, row, t, FP_THREADS, nb, &err);
+        uint32_t te = 0;
+        uint32_t nb = vm_run(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te);
         for (int c = 0; c < out.count; c++) {
             int tp = out.temp[c];
+            err |= vm_temp_error(te, tp);
             bool isn = (nb >> tp) & 1;
             int64_t v = isn ? 0 : t[tp * FP_THREADS];
             if (out.vtype[c] == TGPU_V_BOOLEAN) ((int8_t*)out.data[c])[j] = (int8_t)v;
@@ -148,7 +151,13 @@ static std::string fp_operand(const DOperand& o)
     return buf;
 }
 
-static void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last, const char* err)
+// the error operand o carries (see vm_error): a temp's, never a column's or a constant's
+static std::string fp_operand_error(const DOperand& o)
+{
+    return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : "0u";
+}
+
+static void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
 {
     for (int i = first; i < last; i++) {
         const DInsn& in = prog.insns[i];
@@ -160,11 +169,14 @@ static void fp_emit_insns(std::string& s, const DProgram& prog, int first, int l
                 if (in.vtype == TGPU_V_DOUBLE) fp_appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
                 else fp_appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
             }
-            fp_appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; }\n", in.dst, in.dst);
+            fp_appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, fp_operand_error(in.a).c_str());
         }
         else {
-            fp_appendf(s, "    { Value x = vm_apply(%d, %d, %s, %s, %s, %s); t%d = x.bits; tn%d = x.is_null; }\n", in.op, in.vtype, fp_operand(in.a).c_str(),
-                       fp_operand(in.b).c_str(), fp_operand(in.c).c_str(), err, in.dst, in.dst);
+            // operands are read into locals first: dst may be one of them, and vm_error needs their values
+            fp_appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", fp_operand(in.a).c_str(),
+                       fp_operand(in.b).c_str(), fp_operand(in.c).c_str(), in.op, in.vtype);
+            fp_appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
+                       fp_operand_error(in.a).c_str(), fp_operand_error(in.b).c_str(), fp_operand_error(in.c).c_str(), in.dst, in.dst, in.dst);
         }
     }
 }
@@ -186,30 +198,31 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         if ((nullable_mask >> c) & 1) fp_appendf(loads, " const bool c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
         else fp_appendf(loads, " const bool c%dn = false;\n", c);
     }
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    long long t%d = 0; bool tn%d = true;\n", t, t);
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    // value, NULL flag and carried error of the temp behind each computed output column (the only errors a projection raises)
+    std::string output_switch = "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true; unsigned int e = 0;\n      switch (out.temp[c]) {\n";
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(output_switch, "        case %d: v = t%d; isn = tn%d; e = te%d; break;\n", t, t, t, t);
+    output_switch += "      }\n      err |= e;\n      if (isn) v = 0;\n";
     // filter kernel
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_jit(DColumns cols, long long n, unsigned char* flags, unsigned int* err_out) {\n";
     s += "  unsigned int err = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
     s += "  for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += stride) {\n";
     s += loads + temps;
-    fp_emit_insns(s, prog, 0, prog.num_filter_insns, "&err");
-    if (prog.filter_temp >= 0) fp_appendf(s, "    flags[row] = (!tn%d && t%d != 0) ? 1 : 0;\n", prog.filter_temp, prog.filter_temp);
+    fp_emit_insns(s, prog, 0, prog.num_filter_insns);
+    if (prog.filter_temp >= 0) fp_appendf(s, "    err |= te%d;\n    flags[row] = (!tn%d && t%d != 0) ? 1 : 0;\n", prog.filter_temp, prog.filter_temp, prog.filter_temp);
     else s += "    flags[row] = 1;\n";
     s += "  }\n  if (err) atomicOr(err_out, err);\n}\n";
     // projection kernel
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_jit(DColumns cols, const int* sel, long long m, OutCols out, unsigned int* err_out, unsigned int* any_null) {\n";
-    s += "  unsigned int err = 0, ignored = 0, nulls_seen = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
+    s += "  unsigned int err = 0, nulls_seen = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
     s += "  for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < m; j += stride) {\n";
     s += "    const long long row = sel ? sel[j] : j;\n";
     s += loads + temps;
-    fp_emit_insns(s, prog, 0, prog.num_filter_insns, "&ignored");
-    fp_emit_insns(s, prog, prog.num_filter_insns, prog.num_insns, "&err");
-    s += "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true;\n      switch (out.temp[c]) {\n";
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(s, "        case %d: v = t%d; isn = tn%d; break;\n", t, t, t);
-    s += "      }\n      if (isn) v = 0;\n";
+    fp_emit_insns(s, prog, 0, prog.num_insns);
+    s += output_switch;
     s += "      if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
-    s += "  }\n  (void)ignored;\n  if (err) atomicOr(err_out, err);\n  if (nulls_seen) atomicOr(any_null, nulls_seen);\n}\n";
+    s += "  }\n  if (err) atomicOr(err_out, err);\n  if (nulls_seen) atomicOr(any_null, nulls_seen);\n}\n";
     // chunked two-pass form (no selection vector): per-row functors + the two kernels around the bodies of device_lib.cuh
     bool chunkable = prog.filter_temp >= 0;
     for (int ch : pass_channels)
@@ -218,16 +231,13 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     s += "struct FProg {\n";
     s += "  static __device__ __forceinline__ bool filter(const DColumns& cols, long long row, unsigned int* errp) {\n    unsigned int err = 0;\n";
     s += loads + temps;
-    fp_emit_insns(s, prog, 0, prog.num_filter_insns, "&err");
-    fp_appendf(s, "    *errp |= err;\n    return !tn%d && t%d != 0;\n  }\n", prog.filter_temp, prog.filter_temp);
+    fp_emit_insns(s, prog, 0, prog.num_filter_insns);
+    fp_appendf(s, "    err |= te%d;\n    *errp |= err;\n    return !tn%d && t%d != 0;\n  }\n", prog.filter_temp, prog.filter_temp, prog.filter_temp);
     s += "  static __device__ __forceinline__ void row(const DColumns& cols, long long row, long long j, const OutCols& out, unsigned int* errp, unsigned int* nullsp) {\n";
-    s += "    unsigned int err = 0, ignored = 0, nulls_seen = 0;\n";
+    s += "    unsigned int err = 0, nulls_seen = 0;\n";
     s += loads + temps;
-    fp_emit_insns(s, prog, 0, prog.num_filter_insns, "&ignored");
-    fp_emit_insns(s, prog, prog.num_filter_insns, prog.num_insns, "&err");
-    s += "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true;\n      switch (out.temp[c]) {\n";
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(s, "        case %d: v = t%d; isn = tn%d; break;\n", t, t, t);
-    s += "      }\n      if (isn) v = 0;\n";
+    fp_emit_insns(s, prog, 0, prog.num_insns);
+    s += output_switch;
     s += "      if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
     for (size_t k = 0; k < pass_channels.size(); k++) {
@@ -236,7 +246,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         fp_appendf(s, "    ((%s*)out.pass_data[%d])[j] = ((const %s*)cols.cols[%d].data)[row];\n", ty, (int)k, ty, ch);
         if ((nullable_mask >> ch) & 1) fp_appendf(s, "    out.pass_nullmap[%d][j] = tg_valid(cols.cols[%d].validity, row) ? 0 : 1;\n", (int)k, ch);
     }
-    s += "    (void)ignored;\n    *errp |= err;\n    *nullsp |= nulls_seen;\n  }\n};\n";
+    s += "    *errp |= err;\n    *nullsp |= nulls_seen;\n  }\n};\n";
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_chunks_jit(DColumns cols, long long n, long long chunk, unsigned char* flags, "
          "unsigned int* counts, unsigned int* err_out) { fp_filter_chunks_body<FProg>(cols, n, chunk, flags, counts, err_out); }\n";
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_chunks_jit(DColumns cols, const unsigned char* flags, long long n, long long chunk, "
@@ -547,6 +557,7 @@ struct FilterProjectOp : tgpu_op {
     {
         if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
         if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
+        if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
         return TGPU_OK;
     }
 

@@ -6,7 +6,10 @@
 //     (M/sql/gen/columnar/AndFilterEvaluator.java, OrFilterEvaluator.java; filters reject NULL:
 //      M/sql/gen/columnar/ColumnarFilter.java:27-30)
 //   - BIGINT arithmetic is checked (Math.addExact/subtractExact/multiplyExact/negateExact,
-//     M/type/BigintOperators.java:52-110) -> NUMERIC_VALUE_OUT_OF_RANGE / DIVISION_BY_ZERO
+//     M/type/BigintOperators.java:52-110) -> NUMERIC_VALUE_OUT_OF_RANGE / DIVISION_BY_ZERO; CAST(DOUBLE AS BIGINT) out of
+//     range -> INVALID_CAST_ARGUMENT
+//   - an error is raised only where the reference evaluates the operation that raises it: AND / OR short-circuit,
+//     a NULL argument skips the remaining ones (vm_error in device_lib.cuh)
 //   - DOUBLE arithmetic is IEEE-754 binary64 with NO fused multiply-add (M/type/DoubleOperators.java:66-86):
 //     every operation goes through __dadd_rn/__dmul_rn/__ddiv_rn which the compiler never contracts.
 //
@@ -69,15 +72,28 @@ __device__ __forceinline__ Value vm_fetch(const DOperand& o, const DColumns& col
     return v;
 }
 
-// Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
-// [temp][thread] array (stride tstride).  Returns the updated null bitmask; *err accumulates TG_ERR_BIT_*.
-__device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
-                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* err)
+// error carried by operand o: temps carry one (4 bits per temp in `errs`), columns and constants none
+__device__ __forceinline__ uint32_t vm_carried(const DOperand& o, uint32_t errs)
 {
+    return o.kind == TGPU_OPND_TEMP ? (errs >> (4 * o.index)) & 0xFu : 0u;
+}
+
+__device__ __forceinline__ uint32_t vm_temp_error(uint32_t errs, int t) { return (errs >> (4 * t)) & 0xFu; }
+
+// Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
+// [temp][thread] array (stride tstride).  Returns the updated null bitmask; *errs holds the TG_ERR_BIT_* each temp
+// carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.
+__device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
+                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs)
+{
+    uint32_t te = *errs;
     for (int pc = first; pc < last; pc++) {
         const DInsn& in = prog->insns[pc];
         Value a = vm_fetch(in.a, cols, row, temps, tstride, nullbits);
         Value b = vm_fetch(in.b, cols, row, temps, tstride, nullbits);
+        Value c;
+        c.bits = 0; c.is_null = true;
+        uint32_t own = 0, ec = 0;
         int64_t r;
         bool rn;
         if (in.op == TGPU_EX_IN) {
@@ -88,23 +104,27 @@ __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, in
                 int off = prog->in_offset[li], cnt = prog->in_count[li];
                 bool hit = false;
                 for (int k = 0; k < cnt; k++) {
-                    int64_t c = prog->in_values[off + k];
-                    hit |= in.vtype == TGPU_V_DOUBLE ? (__longlong_as_double(a.bits) == __longlong_as_double(c)) : (a.bits == c);
+                    int64_t v = prog->in_values[off + k];
+                    hit |= in.vtype == TGPU_V_DOUBLE ? (__longlong_as_double(a.bits) == __longlong_as_double(v)) : (a.bits == v);
                 }
                 r = hit ? 1 : 0;
             }
         }
         else {
-            Value c;
-            c.bits = 0; c.is_null = true;
-            if (in.op == TGPU_EX_BETWEEN) c = vm_fetch(in.c, cols, row, temps, tstride, nullbits);
-            Value res = vm_apply(in.op, in.vtype, a, b, c, err);
+            if (in.op == TGPU_EX_BETWEEN) {
+                c = vm_fetch(in.c, cols, row, temps, tstride, nullbits);
+                ec = vm_carried(in.c, te);
+            }
+            Value res = vm_apply(in.op, in.vtype, a, b, c, &own);
             r = res.bits;
             rn = res.is_null;
         }
+        uint32_t e = vm_error(in.op, in.vtype, a, vm_carried(in.a, te), b, in.op == TGPU_EX_IN ? 0u : vm_carried(in.b, te), c, ec, own);
         temps[in.dst * tstride] = r;
         nullbits = (nullbits & ~(1u << in.dst)) | ((rn ? 1u : 0u) << in.dst);
+        te = (te & ~(0xFu << (4 * in.dst))) | (e << (4 * in.dst));
     }
+    *errs = te;
     return nullbits;
 }
 

@@ -205,20 +205,29 @@ __global__ void __launch_bounds__(S_THREADS) agg_small_kernel(AggPlan plan, DCol
     __syncthreads();
 
     unsigned long long seen = 0;
-    uint32_t err = 0, ignored = 0;
+    uint32_t err = 0;
+    uint32_t read_errs = 0;      // the 4-bit error fields (vm_run) of the temps the aggregation reads
+    for (int i = 0; i < plan.num_srcs; i++)
+        if (plan.srcs[i].is_temp) read_errs |= 0xFu << (4 * plan.srcs[i].index);
     const long long hi_off = T;   // HI half is the next accumulator: ((s*A + a+1)*T + tid) - ((s*A + a)*T + tid)
     int64_t stride = (int64_t)gridDim.x * T;
     for (int64_t row = (int64_t)blockIdx.x * T + tid; row < n; row += stride) {
         uint32_t nb = 0;
         if (plan.has_pre) {
+            uint32_t te = 0;
             if (prog->filter_temp >= 0) {
-                nb = vm_run(prog, 0, prog->num_filter_insns, cols, row, temps, T, 0, &ignored);
-                err |= ignored;
+                nb = vm_run(prog, 0, prog->num_filter_insns, cols, row, temps, T, 0, &te);
                 int ft = prog->filter_temp;
+                err |= vm_temp_error(te, ft);      // the filter's errors count on every row
                 bool sel = !((nb >> ft) & 1) && temps[ft * T] != 0;
                 if (!sel) continue;
             }
-            nb = vm_run(prog, prog->num_filter_insns, prog->num_insns, cols, row, temps, T, nb, &err);
+            nb = vm_run(prog, prog->num_filter_insns, prog->num_insns, cols, row, temps, T, nb, &te);
+            uint32_t e = te & read_errs;         // a projection raises only when the aggregation reads it
+            e |= e >> 16;
+            e |= e >> 8;
+            e |= e >> 4;
+            err |= e & 0xFu;
         }
         unsigned long long pk = 0;
         int special = pack_key(plan, cols, row, temps, T, nb, &pk);
@@ -1440,11 +1449,15 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++)
         if (used[c]) appendf(s, "    const long long c%d = r.c%d; const bool c%dn = r.c%dn;\n", c, c, c, c);
     if (prog) {
-        for (int t = 0; t < TGPU_MAX_TEMPS; t++) appendf(s, "    long long t%d = 0; bool tn%d = true;\n", t, t);
+        for (int t = 0; t < TGPU_MAX_TEMPS; t++) appendf(s, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+        // the filter's errors count on every row, a projection's only when the aggregation reads it (see vm_error)
+        auto filter_check = [&]() {
+            appendf(s, "    *err |= te%d;\n    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
+        };
+        auto opnd_error = [](const DOperand& o) { return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : std::string("0u"); };
         for (int i = 0; i < prog->num_insns; i++) {
             const DInsn& in = prog->insns[i];
-            if (i == prog->num_filter_insns && prog->filter_temp >= 0)
-                appendf(s, "    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp);
+            if (i == prog->num_filter_insns && prog->filter_temp >= 0) filter_check();
             if (in.op == TGPU_EX_IN) {
                 int li = (int)in.b.imm;
                 appendf(s, "    { Value a = %s; bool hit = false;\n", gen_operand(in.a).c_str());
@@ -1453,15 +1466,19 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
                     if (in.vtype == TGPU_V_DOUBLE) appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
                     else appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
                 }
-                appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; }\n", in.dst, in.dst);
+                appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, opnd_error(in.a).c_str());
             }
             else {
-                appendf(s, "    { Value x = vm_apply(%d, %d, %s, %s, %s, err); t%d = x.bits; tn%d = x.is_null; }\n", in.op, in.vtype,
-                        gen_operand(in.a).c_str(), gen_operand(in.b).c_str(), gen_operand(in.c).c_str(), in.dst, in.dst);
+                // operands are read into locals first: dst may be one of them, and vm_error needs their values
+                appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", gen_operand(in.a).c_str(),
+                        gen_operand(in.b).c_str(), gen_operand(in.c).c_str(), in.op, in.vtype);
+                appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
+                        opnd_error(in.a).c_str(), opnd_error(in.b).c_str(), opnd_error(in.c).c_str(), in.dst, in.dst, in.dst);
             }
         }
-        if (prog->num_filter_insns == prog->num_insns && prog->filter_temp >= 0)
-            appendf(s, "    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp);
+        if (prog->num_filter_insns == prog->num_insns && prog->filter_temp >= 0) filter_check();
+        for (int i = 0; i < plan.num_srcs; i++)
+            if (plan.srcs[i].is_temp) appendf(s, "    *err |= te%d;\n", plan.srcs[i].index);
     }
     for (int i = 0; i < plan.num_srcs; i++) {
         if (plan.srcs[i].is_temp) appendf(s, "    v%d = t%d; vn%d = tn%d;\n", i, plan.srcs[i].index, i, plan.srcs[i].index);
@@ -2146,6 +2163,7 @@ struct AggOp : tgpu_op {
     {
         if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
         if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
+        if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
         return TGPU_OK;
     }
 
