@@ -240,14 +240,33 @@ struct GatherCols {
     void* dst[4];
 };
 
+// Match bitmap of the fused probes: bit i of 32-bit word i / 32 is set when probe row i found its key (Arrow LSB order, so the words
+// are the build columns' validity under PROBE_OUTER).  Every fused kernel gives lane L of a warp row warp_row + L, 32 consecutive,
+// 32-aligned rows: one ballot makes the word, lane 0 stores it and counts its bits.  All 32 lanes must get here.
+__device__ __forceinline__ void store_match_word(unsigned int* __restrict__ match_bits, int64_t warp_row, bool hit, unsigned int* matched)
+{
+    const unsigned int word = __ballot_sync(0xffffffffu, hit);
+    if ((threadIdx.x & 31) == 0) {
+        match_bits[warp_row >> 5] = word;
+        *matched += __popc(word);
+    }
+}
+
+// lane 0 of each warp holds the warp's count: one atomic per warp
+__device__ __forceinline__ void add_match_count(unsigned long long* __restrict__ match_count, unsigned int matched)
+{
+    if ((threadIdx.x & 31) == 0 && matched) atomicAdd(match_count, (unsigned long long)matched);
+}
+
 // Fused probe + build-side gather for the common join shape (no duplicate chains, fixed-width non-null build
 // columns): the chain head is looked up and the build payload of the matching row is fetched while the slot is
 // still in flight in the same thread, so the positions never make a round trip through HBM before the gather and
 // no count/scan pass is needed when every probe row matches (FK -> PK joins).  Misses are counted; the host
-// compacts only when there are any.
+// compacts only when there are any.  Which rows matched goes to the match bitmap (see store_match_word); its words past n are not
+// written, its bits at or past n are 0.  Launched with blockDim.x a multiple of 32, and match_bits 32-row aligned.
 template <int ROWS, bool INT64_NO_NULLS>
 __global__ void __launch_bounds__(256) join_probe_gather_kernel(ColRef key, int kind, int64_t n, const JoinSlot* __restrict__ table, JoinGeom geo,
-                                                                int special_head, int* __restrict__ out, GatherCols g, unsigned long long* __restrict__ match_count)
+                                                                int special_head, unsigned int* __restrict__ match_bits, GatherCols g, unsigned long long* __restrict__ match_count)
 {
     // g.by_slot: payload arrays are indexed by table slot (special key at index mask + 1), else by build row id
     int64_t tile = (int64_t)blockDim.x * ROWS;
@@ -327,40 +346,24 @@ __global__ void __launch_bounds__(256) join_probe_gather_kernel(ColRef key, int 
         }
 #pragma unroll
         for (int j = 0; j < ROWS; j++) {
-            int64_t i = base + (int64_t)j * blockDim.x;
-            if (i >= n) continue;
-            out[i] = res[j];
-            matched += res[j] >= 0;
+            // every lane takes part in the ballot: rows at or past n have res = -1; the warp's first row decides whether its word exists
+            const int64_t warp_row = base - (threadIdx.x & 31) + (int64_t)j * blockDim.x;
+            const unsigned int word = __ballot_sync(0xffffffffu, res[j] >= 0);
+            if ((threadIdx.x & 31) == 0 && warp_row < n) {
+                match_bits[warp_row >> 5] = word;
+                matched += __popc(word);
+            }
         }
     }
-    // one atomic per warp
-    for (int off = 16; off > 0; off >>= 1) matched += __shfl_xor_sync(0xffffffffu, matched, off);
-    if ((threadIdx.x & 31) == 0 && matched) atomicAdd(match_count, (unsigned long long)matched);
+    add_match_count(match_count, matched);
 }
 
-// validity bitmap of the build side of a PROBE_OUTER join: bit i = (jp[i] >= 0)
-__global__ void join_match_validity_kernel(const int* __restrict__ jp, int64_t n, uint8_t* __restrict__ bitmap)
-{
-    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t nbytes = (n + 7) >> 3;
-    int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; b < nbytes; b += stride) {
-        unsigned int v = 0;
-        int64_t base = b << 3;
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-            int64_t i = base + k;
-            if (i < n && jp[i] >= 0) v |= 1u << k;
-        }
-        bitmap[b] = (uint8_t)v;
-    }
-}
-
-__global__ void join_match_flags_kernel(const int* __restrict__ jp, int64_t n, uint8_t* __restrict__ flags)
+// compaction flags of an INNER join page from the match bitmap: flags[i] = bit i
+__global__ void join_match_flags_kernel(const unsigned int* __restrict__ match_bits, int64_t n, uint8_t* __restrict__ flags)
 {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; i < n; i += stride) flags[i] = jp[i] >= 0 ? 1 : 0;
+    for (; i < n; i += stride) flags[i] = (uint8_t)((match_bits[i >> 5] >> (i & 31)) & 1u);
 }
 
 
@@ -457,9 +460,12 @@ static int lean_grid(tgpu_ctx* ctx, K kernel, int64_t tiles)
     return (int)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * per_sm);
 }
 
+// GATHER = false: the join position of every row goes to out[].  GATHER = true: the build payload goes to g.dst and the match bits
+// to match_bits (out is unused)
 template <int MODE, bool GATHER, int MINB = 1>
 __global__ void __launch_bounds__(256, MINB) join_probe_lean_kernel(const long long* __restrict__ keys, int64_t tiles, const int4* __restrict__ table, unsigned int mask,
-                                                              unsigned long long kmin, int shift, int special_head, int* __restrict__ out, GatherCols g, unsigned long long* __restrict__ match_count)
+                                                              unsigned long long kmin, int shift, int special_head, int* __restrict__ out, unsigned int* __restrict__ match_bits,
+                                                              GatherCols g, unsigned long long* __restrict__ match_count)
 {
     // the word behind the match counter holds the layout choice of the page (0 = these 16-byte slots; join_probe_locality_kernel decides)
     if (GATHER && *(const volatile int*)(match_count + 1) != 0) return;
@@ -522,14 +528,11 @@ __global__ void __launch_bounds__(256, MINB) join_probe_lean_kernel(const long l
         }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
-            out[base + j * 256] = res[j];
-            if (GATHER) matched += res[j] >= 0;
+            if (GATHER) store_match_word(match_bits, base + j * 256, res[j] >= 0, &matched);
+            else out[base + j * 256] = res[j];
         }
     }
-    if (GATHER) {
-        for (int off = 16; off > 0; off >>= 1) matched += __shfl_xor_sync(0xffffffffu, matched, off);
-        if ((threadIdx.x & 31) == 0 && matched) atomicAdd(match_count, (unsigned long long)matched);
-    }
+    if (GATHER) add_match_count(match_count, matched);
 }
 
 // ---- TMA-staged probe for order-preserving tables (mode 2) ----------------------------------------------------------------
@@ -576,8 +579,8 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned int 
 
 template <bool GATHER>
 __global__ void __launch_bounds__(256, 6) join_probe_span_kernel(const long long* __restrict__ keys, int64_t tiles, const int4* __restrict__ table, unsigned int mask,
-                                                                unsigned long long kmin, int shift, int special_head, int* __restrict__ out, GatherCols g,
-                                                                unsigned long long* __restrict__ match_count)
+                                                                unsigned long long kmin, int shift, int special_head, int* __restrict__ out,
+                                                                unsigned int* __restrict__ match_bits, GatherCols g, unsigned long long* __restrict__ match_count)
 {
     __shared__ __align__(128) int4 s_slots[SPAN_LINES * 8];
     __shared__ __align__(128) long long s_pay[SPAN_LINES * 8];
@@ -675,21 +678,18 @@ __global__ void __launch_bounds__(256, 6) join_probe_span_kernel(const long long
         }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
-            out[base + j * 256] = res[j];
-            if (GATHER) matched += res[j] >= 0;
+            if (GATHER) store_match_word(match_bits, base + j * 256, res[j] >= 0, &matched);
+            else out[base + j * 256] = res[j];
         }
         __syncthreads();          // everyone is done with the staged span (and s_min / s_max) before the next tile overwrites them
     }
-    if (GATHER) {
-        for (int off = 16; off > 0; off >>= 1) matched += __shfl_xor_sync(0xffffffffu, matched, off);
-        if (lane == 0 && matched) atomicAdd(match_count, (unsigned long long)matched);
-    }
+    if (GATHER) add_match_count(match_count, matched);
 }
 
-// launch of the lean probe kernel for the table's layout mode
+// launch of the lean probe kernel for the table's layout mode (out: positions of the index-only probe; match_bits: of the fused one)
 template <bool GATHER>
-static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const int4* table, int special_head, int* out, const GatherCols& g,
-                       unsigned long long* matches)
+static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const int4* table, int special_head, int* out,
+                       unsigned int* match_bits, const GatherCols& g, unsigned long long* matches)
 {
     const unsigned int mask32 = (unsigned int)geo.mask;
     // 8 CTAs per SM (32 registers): full occupancy is worth more than the registers
@@ -697,19 +697,19 @@ static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
         // TMA-staged table spans (falls back per tile when the keys are not clustered).  Opt-in: with the dense table the lean kernel
         // already streams the table once, and the span kernel pays a block-wide span reduction plus a second dependent DRAM round trip per tile
         auto k = join_probe_span_kernel<GATHER>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, geo.kmin, geo.shift, special_head, out, g, matches);
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, geo.kmin, geo.shift, special_head, out, match_bits, g, matches);
     }
     else if (geo.mode == 2) {
         auto k = join_probe_lean_kernel<2, GATHER, 8>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, geo.kmin, geo.shift, special_head, out, g, matches);
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, geo.kmin, geo.shift, special_head, out, match_bits, g, matches);
     }
     else if (geo.mode == 1) {
         auto k = join_probe_lean_kernel<1, GATHER, 8>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, 0ULL, 0, special_head, out, g, matches);
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, 0ULL, 0, special_head, out, match_bits, g, matches);
     }
     else {
         auto k = join_probe_lean_kernel<0, GATHER, 8>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, 0ULL, 0, special_head, out, g, matches);
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, table, mask32, 0ULL, 0, special_head, out, match_bits, g, matches);
     }
     return TGPU_OK;
 }
@@ -722,13 +722,26 @@ static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
 // On a key-ordered probe page the bytes are the same as slot table + slot-ordered payload arrays, read front to back.
 // Built next to the 16-byte table (which the index-only probe, the duplicate chains and every generic kernel keep using).
 struct __align__(32) WideSlot {
+    static constexpr int CELLS = 2;
     unsigned long long key;
     int head;
     int pad;
     unsigned long long cell[2];
 };
 
-// sm_90 has no 256-bit load: a slot is read as the two 128-bit halves of its 32-byte sector, which costs one DRAM sector all the same.
+// ---- keyed slots: key and the payload of its head row in 16 bytes, for builds with ONE payload column ------------------------------
+// With a single payload column of at most 8 bytes (no NULLs, no duplicate keys) the head row id is never needed: the slot is {key, cell},
+// and one 128-bit load both resolves a probe row and fetches its payload.  On a key-ordered probe page this reads 16 bytes per slot
+// instead of the 16-byte slot plus its slot-ordered payload cell, with no dependent payload load; on a page without key locality it is
+// one random sector per row, like the wide slot.  It replaces the wide table for these builds.  An occupied slot always matches (its key
+// was inserted, so its head is >= 0); the special key INT64_MIN keeps its cell in slot mask + 1, as in the wide table.
+struct __align__(16) KeyedSlot {
+    static constexpr int CELLS = 1;
+    unsigned long long key;
+    unsigned long long cell;
+};
+
+// sm_90 has no 256-bit load: a wide slot is read as the two 128-bit halves of its 32-byte sector, which costs one DRAM sector all the same.
 // LD: 0 = plain read-only loads; 3 = the same with an explicit 64-byte L2 fetch size
 template <int LD>
 __device__ __forceinline__ WideSlot wide_load(const WideSlot* p)
@@ -748,6 +761,39 @@ __device__ __forceinline__ WideSlot wide_load(const WideSlot* p)
     return w;
 }
 
+template <int LD>
+__device__ __forceinline__ KeyedSlot wide_load(const KeyedSlot* p)
+{
+    KeyedSlot w;
+    if (LD == 3) asm("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2];" : "=l"(w.key), "=l"(w.cell) : "l"(p));
+    else asm("ld.global.nc.v2.u64 {%0,%1}, [%2];" : "=l"(w.key), "=l"(w.cell) : "l"(p));
+    return w;
+}
+
+// head row of a slot whose key matched (a keyed slot has none: any non-negative value stands for "matched")
+__device__ __forceinline__ int slot_head(const WideSlot& w) { return w.head; }
+__device__ __forceinline__ int slot_head(const KeyedSlot&) { return 0; }
+__device__ __forceinline__ unsigned long long slot_cell(const WideSlot& w, int c) { return w.cell[c]; }
+__device__ __forceinline__ unsigned long long slot_cell(const KeyedSlot& w, int) { return w.cell; }
+
+__device__ __forceinline__ void put_slot(WideSlot* s, unsigned long long key, int head, unsigned long long c0, unsigned long long c1)
+{
+    WideSlot w;
+    w.key = key;
+    w.head = head;
+    w.pad = 0;
+    w.cell[0] = c0;
+    w.cell[1] = c1;
+    *s = w;
+}
+__device__ __forceinline__ void put_slot(KeyedSlot* s, unsigned long long key, int, unsigned long long c0, unsigned long long)
+{
+    KeyedSlot w;
+    w.key = key;
+    w.cell = c0;
+    *s = w;
+}
+
 __device__ __forceinline__ unsigned long long wide_cell_of(const void* src, int elem, int row)
 {
     switch (elem) {
@@ -758,30 +804,29 @@ __device__ __forceinline__ unsigned long long wide_cell_of(const void* src, int 
     }
 }
 
+// S = WideSlot (cells of up to two columns) or KeyedSlot (one column); slot i < slots mirrors the 16-byte table, slot `slots` holds INT64_MIN's
+template <class S>
 __global__ void join_wide_table_kernel(const JoinSlot* __restrict__ table, int64_t slots, int special_head, const void* __restrict__ src0, int elem0,
-                                       const void* __restrict__ src1, int elem1, WideSlot* __restrict__ wide)
+                                       const void* __restrict__ src1, int elem1, S* __restrict__ wide)
 {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (; i <= slots; i += stride) {
-        WideSlot w;
-        w.key = i < slots ? table[i].key : EMPTY_KEY;
-        w.head = i < slots ? table[i].head : special_head;
-        w.pad = 0;
-        w.cell[0] = w.head >= 0 && src0 ? wide_cell_of(src0, elem0, w.head) : 0ULL;
-        w.cell[1] = w.head >= 0 && src1 ? wide_cell_of(src1, elem1, w.head) : 0ULL;
-        wide[i] = w;
+        const unsigned long long key = i < slots ? table[i].key : EMPTY_KEY;
+        const int head = i < slots ? table[i].head : special_head;
+        put_slot(wide + i, key, head, head >= 0 && src0 ? wide_cell_of(src0, elem0, head) : 0ULL, head >= 0 && src1 ? wide_cell_of(src1, elem1, head) : 0ULL);
     }
 }
 
 // same contract as join_probe_lean_kernel<MODE, true>: whole 1024-row tiles of a BIGINT key without NULLs; ROWS rows of a thread are in
-// flight together (a tile is 4 rows per thread, taken ROWS at a time)
-template <int MODE, int ROWS, int MINB, int LD = 0>
-__global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long long* __restrict__ keys, int64_t tiles, const WideSlot* __restrict__ wide, unsigned int mask,
-                                                                  unsigned long long kmin, int shift, int special_head, int* __restrict__ out, GatherCols g,
-                                                                  unsigned long long* __restrict__ match_count, const int* __restrict__ layout_choice)
+// flight together (a tile is 4 rows per thread, taken ROWS at a time).  S is the slot type of the table (WideSlot or KeyedSlot).
+// With layout_choice set the kernel runs only when join_probe_locality_kernel chose run_on for the page.
+template <int MODE, int ROWS, int MINB, int LD, class S>
+__global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long long* __restrict__ keys, int64_t tiles, const S* __restrict__ wide, unsigned int mask,
+                                                                  unsigned long long kmin, int shift, int special_head, unsigned int* __restrict__ match_bits, GatherCols g,
+                                                                  unsigned long long* __restrict__ match_count, const int* __restrict__ layout_choice, int run_on)
 {
-    if (layout_choice && *layout_choice == 0) return;      // the page goes through the 16-byte slots
+    if (layout_choice && *layout_choice != run_on) return;
     unsigned int matched = 0;
     for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
 #pragma unroll
@@ -789,7 +834,8 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
             const int64_t base = t * 1024 + h * 256 + threadIdx.x;
             unsigned long long k[ROWS];
             unsigned int pos[ROWS];
-            WideSlot w[ROWS];
+            S w[ROWS];
+            bool hit[ROWS];
 #pragma unroll
             for (int j = 0; j < ROWS; j++) k[j] = (unsigned long long)__ldg(keys + base + j * 256);
 #pragma unroll
@@ -801,7 +847,7 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
                 unsigned int p = pos[j];
                 int r = -1;
                 while (true) {
-                    if (w[j].key == k[j]) { r = w[j].head; break; }
+                    if (w[j].key == k[j]) { r = slot_head(w[j]); break; }
                     if (w[j].key == EMPTY_KEY) break;
                     p = lean_next<MODE>(p, (unsigned int)k[j] & 7u, mask);
                     w[j] = wide_load<LD>(wide + p);
@@ -810,15 +856,14 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
                     r = special_head;
                     if (r >= 0) w[j] = wide_load<LD>(wide + (mask + 1u));
                 }
-                if (r < 0) { w[j].cell[0] = 0ULL; w[j].cell[1] = 0ULL; }
-                w[j].head = r;
+                hit[j] = r >= 0;
             }
 #pragma unroll
-            for (int c = 0; c < 2; c++) {
+            for (int c = 0; c < S::CELLS; c++) {
                 if (c >= g.count) break;
 #pragma unroll
                 for (int j = 0; j < ROWS; j++) {
-                    const unsigned long long v = w[j].cell[c];
+                    const unsigned long long v = hit[j] ? slot_cell(w[j], c) : 0ULL;
                     switch (g.elem[c]) {
                         case 8: ((unsigned long long*)g.dst[c])[base + j * 256] = v; break;
                         case 4: ((unsigned int*)g.dst[c])[base + j * 256] = (unsigned int)v; break;
@@ -828,21 +873,18 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
                 }
             }
 #pragma unroll
-            for (int j = 0; j < ROWS; j++) {
-                out[base + j * 256] = w[j].head;
-                matched += w[j].head >= 0;
-            }
+            for (int j = 0; j < ROWS; j++) store_match_word(match_bits, base + j * 256, hit[j], &matched);
         }
     }
-    for (int off = 16; off > 0; off >>= 1) matched += __shfl_xor_sync(0xffffffffu, matched, off);
-    if ((threadIdx.x & 31) == 0 && matched) atomicAdd(match_count, (unsigned long long)matched);
+    add_match_count(match_count, matched);
 }
 
 // Which layout a probe page should read.  A wide slot is 32 bytes, a 16-byte slot plus its slot-ordered payload cells 16 + (payload bytes):
 // with one payload column a probe page that arrives in key order reads fewer bytes from the narrow layout (whole lines are used either
 // way), while a page without key locality pays a 32-byte sector per ARRAY it touches and is better off with the wide slot.  256 pairs of
 // neighbouring rows, spread over the page, vote: a pair is local when its two slots lie within 8 lines of each other.
-// choice: 0 = narrow, 1 = wide.  No host round trip: both probe kernels are launched and the one not chosen returns at once.
+// choice: 0 = key-ordered (the 16-byte slots, or the keyed table in the lean kernel's 4-row shape), 1 = random access (the wide table, or
+// the keyed table in the random-access shape).  No host round trip: both probe kernels are launched and the one not chosen returns at once.
 template <int MODE>
 __global__ void __launch_bounds__(256) join_probe_locality_kernel(const long long* __restrict__ keys, int64_t tiles, unsigned int mask, unsigned long long kmin, int shift,
                                                                   int* __restrict__ layout_choice)
@@ -864,42 +906,53 @@ static int launch_locality(tgpu_ctx* ctx, const JoinGeom& geo, const long long* 
     return TGPU_OK;
 }
 
-template <int ROWS, int MINB, int LD = 0>
-static int launch_wide_shape(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const WideSlot* wide, int special_head, int* out,
-                             const GatherCols& g, unsigned long long* matches, const int* layout_choice)
+template <int ROWS, int MINB, int LD = 0, class S>
+static int launch_wide_shape(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned int* match_bits,
+                             const GatherCols& g, unsigned long long* matches, const int* layout_choice, int run_on)
 {
     const unsigned int mask32 = (unsigned int)geo.mask;
     if (geo.mode == 2) {
-        auto k = join_probe_wide_kernel<2, ROWS, MINB, LD>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, geo.kmin, geo.shift, special_head, out, g, matches, layout_choice);
+        auto k = join_probe_wide_kernel<2, ROWS, MINB, LD, S>;
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, geo.kmin, geo.shift, special_head, match_bits, g, matches, layout_choice, run_on);
     }
     else if (geo.mode == 1) {
-        auto k = join_probe_wide_kernel<1, ROWS, MINB, LD>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, out, g, matches, layout_choice);
+        auto k = join_probe_wide_kernel<1, ROWS, MINB, LD, S>;
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, match_bits, g, matches, layout_choice, run_on);
     }
     else {
-        auto k = join_probe_wide_kernel<0, ROWS, MINB, LD>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, out, g, matches, layout_choice);
+        auto k = join_probe_wide_kernel<0, ROWS, MINB, LD, S>;
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, match_bits, g, matches, layout_choice, run_on);
     }
     return TGPU_OK;
 }
 
+// Random-access shape of the probe over a wide or keyed table (runs when layout_choice is null or 1).
 // rows in flight per thread x CTAs per SM; TGPU_JOIN_WIDE_SHAPE=<rows><ctas> picks one of the built shapes (sweeps)
-static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const WideSlot* wide, int special_head, int* out, const GatherCols& g,
-                       unsigned long long* matches, const int* layout_choice)
+template <class S>
+static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned int* match_bits,
+                       const GatherCols& g, unsigned long long* matches, const int* layout_choice)
 {
     const char* e = getenv("TGPU_JOIN_WIDE_SHAPE");
     int shape = e ? atoi(e) : 28;
     const char* le = getenv("TGPU_JOIN_WIDE_LOAD");
     int ld = le ? atoi(le) : 3;
-    if (shape == 28 && ld == 3) return launch_wide_shape<2, 8, 3>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
+    if (shape == 28 && ld == 3) return launch_wide_shape<2, 8, 3>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
     switch (shape) {
-        case 18: return launch_wide_shape<1, 8>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
-        case 26: return launch_wide_shape<2, 6>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
-        case 45: return launch_wide_shape<4, 5>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
-        case 44: return launch_wide_shape<4, 4>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
-        default: return launch_wide_shape<2, 8>(ctx, geo, keys, tiles, wide, special_head, out, g, matches, layout_choice);
+        case 18: return launch_wide_shape<1, 8>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+        case 26: return launch_wide_shape<2, 6>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+        case 45: return launch_wide_shape<4, 5>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+        case 44: return launch_wide_shape<4, 4>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+        default: return launch_wide_shape<2, 8>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
     }
+}
+
+// Key-ordered shape of the probe over a keyed table (runs when layout_choice is 0): 8 CTAs per SM and plain read-only loads like the lean
+// kernel, but 2 rows in flight per thread rather than 4: four keyed rows do not fit the 32 registers that 8 CTAs per SM allow (ptxas spills
+// 88-144 bytes per thread), two take 28-30 registers without spilling
+static int launch_keyed_ordered(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const KeyedSlot* keyed, int special_head,
+                                unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice)
+{
+    return launch_wide_shape<2, 8, 0>(ctx, geo, keys, tiles, keyed, special_head, match_bits, g, matches, layout_choice, 0);
 }
 
 // build payload re-laid out in SLOT order (one pass at build time): the fused probe then reads the payload right next
@@ -1026,7 +1079,8 @@ struct tgpu_lookup {
     DevPage store;                      // key column first, then build output columns
     int32_t num_output = 0;
     std::vector<DevBuf> by_slot;        // build output columns in table-slot order (fused probe fast path)
-    DevBuf wide;                        // WideSlot[capacity + 1]: slots with the payload of their head row (<= 2 build output columns)
+    DevBuf wide;                        // WideSlot[capacity + 1]: slots with the payload of their head row (2 build output columns)
+    DevBuf keyed;                       // KeyedSlot[capacity + 1]: key + payload cell (1 build output column; instead of `wide`)
     bool generic = false;               // keyed by row hash + verification against build_keys
     int attempts = 1;                   // generic only: hash functions the build needed (> 1 iff two keys shared a 64-bit hash)
     std::vector<DevColumn> build_keys;  // generic only: the real key columns of the build side
@@ -1104,7 +1158,8 @@ int lookup_positions(tgpu_ctx* ctx, const tgpu_lookup* lk, const DevColumn& key,
         if (tiles > 0) {
             GatherCols none;
             memset(&none, 0, sizeof(none));
-            TG_TRY(launch_lean<false>(ctx, lk->geo, (const long long*)key.data, tiles, (const int4*)table, lk->special_head, d_out, none, (unsigned long long*)nullptr));
+            TG_TRY(launch_lean<false>(ctx, lk->geo, (const long long*)key.data, tiles, (const int4*)table, lk->special_head, d_out, nullptr, none,
+                                      (unsigned long long*)nullptr));
             done = tiles * 1024;
         }
     }
@@ -1460,12 +1515,21 @@ struct JoinBuildOp : tgpu_op {
                           c.elem_size(), lk->by_slot[b].p);
             }
         }
+        // slots that carry the payload of their head row: 16-byte keyed slots for one output column, 32-byte wide slots for two
         if (slot_payload && lk->num_output <= 2 && !lk->has_dups && !lk->generic && cap + 1 < (1LL << 31) && !getenv("TGPU_JOIN_NO_WIDE")) {
-            TG_TRY(lk->wide.alloc(ctx, (size_t)(cap + 1) * sizeof(WideSlot)));
             const DevColumn& c0 = lk->store.cols[1];
             const DevColumn* c1 = lk->num_output > 1 ? &lk->store.cols[2] : nullptr;
-            TG_LAUNCH(ctx, join_wide_table_kernel, tg_grid(ctx, cap + 1, 1024, 8), 256, 0, lk->table.as<JoinSlot>(), cap, lk->special_head, c0.data, c0.elem_size(),
-                      c1 ? c1->data : (const void*)nullptr, c1 ? c1->elem_size() : 0, lk->wide.as<WideSlot>());
+            const int grid = tg_grid(ctx, cap + 1, 1024, 8);
+            if (!c1) {
+                TG_TRY(lk->keyed.alloc(ctx, (size_t)(cap + 1) * sizeof(KeyedSlot)));
+                TG_LAUNCH(ctx, join_wide_table_kernel<KeyedSlot>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->special_head, c0.data, c0.elem_size(),
+                          (const void*)nullptr, 0, lk->keyed.as<KeyedSlot>());
+            }
+            else {
+                TG_TRY(lk->wide.alloc(ctx, (size_t)(cap + 1) * sizeof(WideSlot)));
+                TG_LAUNCH(ctx, join_wide_table_kernel<WideSlot>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->special_head, c0.data, c0.elem_size(),
+                          c1->data, c1->elem_size(), lk->wide.as<WideSlot>());
+            }
         }
         TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         lookup = lk.release();
@@ -1498,7 +1562,7 @@ struct JoinProbeOp : tgpu_op {
     struct Deferred {
         bool active = false;
         DevPage in;
-        std::shared_ptr<DevBuf> jp;
+        std::shared_ptr<DevBuf> match_bits;     // bit i: probe row i matched (32-bit words, Arrow LSB order)
         std::vector<DevColumn> built;
         int64_t n = 0;
     } deferred;
@@ -1529,8 +1593,10 @@ struct JoinProbeOp : tgpu_op {
             const DevColumn& c = lookup->store.cols[1 + b];
             if (c.elem_size() == 0 || c.elem_size() > 8 || c.validity) return TGPU_OK;      // (the fused gather moves 1 / 2 / 4 / 8-byte payloads)
         }
-        auto jp = std::make_shared<DevBuf>();
-        TG_TRY(jp->alloc(ctx, (size_t)n * 4));
+        // which probe rows matched, one bit per row (store_match_word); it is the build columns' validity of a PROBE_OUTER page
+        auto match_bits = std::make_shared<DevBuf>();
+        TG_TRY(match_bits->alloc(ctx, (size_t)((n + 31) / 32) * 4));
+        unsigned int* bits = match_bits->as<unsigned int>();
         GatherCols g;
         memset(&g, 0, sizeof(g));
         g.count = lookup->num_output;
@@ -1566,18 +1632,30 @@ struct JoinProbeOp : tgpu_op {
                 const char* we = getenv("TGPU_JOIN_WIDE");
                 int payload_bytes = 0;
                 for (int c = 0; c < g.count; c++) payload_bytes += g.elem[c];
-                const bool have_wide = lookup->wide.p && !getenv("TGPU_JOIN_NO_WIDE") && !getenv("TGPU_JOIN_SPAN") && !(we && !strcmp(we, "never"));
-                const bool always = have_wide && ((we && !strcmp(we, "always")) || payload_bytes >= 16 || !g.by_slot);
-                if (always)
-                    TG_TRY(launch_wide(ctx, lookup->geo, (const long long*)key.data, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, jp->as<int>(), g, d_matches, nullptr));
+                // A keyed table (one payload column) serves both kinds of page: the locality vote picks the key-ordered or the random-access
+                // shape of the same kernel, and TGPU_JOIN_WIDE=always pins the random-access one
+                const long long* keys = (const long long*)key.data;
+                const bool layouts_on = !getenv("TGPU_JOIN_NO_WIDE") && !getenv("TGPU_JOIN_SPAN") && !(we && !strcmp(we, "never"));
+                const bool have_keyed = lookup->keyed.p && layouts_on;
+                const bool have_wide = lookup->wide.p && layouts_on;
+                const bool always = (have_wide || have_keyed) && ((we && !strcmp(we, "always")) || payload_bytes >= 16 || !g.by_slot);
+                int* d_choice = (int*)(d_matches + 1);
+                if (always && have_keyed)
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, nullptr));
+                else if (always)
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, bits, g, d_matches, nullptr));
+                else if (have_keyed) {
+                    TG_TRY(launch_locality(ctx, lookup->geo, keys, tiles, d_choice));
+                    TG_TRY(launch_keyed_ordered(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
+                }
                 else if (have_wide) {
-                    int* d_choice = (int*)(d_matches + 1);
-                    TG_TRY(launch_locality(ctx, lookup->geo, (const long long*)key.data, tiles, d_choice));
-                    TG_TRY(launch_lean<true>(ctx, lookup->geo, (const long long*)key.data, tiles, (const int4*)table, lookup->special_head, jp->as<int>(), g, d_matches));
-                    TG_TRY(launch_wide(ctx, lookup->geo, (const long long*)key.data, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, jp->as<int>(), g, d_matches, d_choice));
+                    TG_TRY(launch_locality(ctx, lookup->geo, keys, tiles, d_choice));
+                    TG_TRY(launch_lean<true>(ctx, lookup->geo, keys, tiles, (const int4*)table, lookup->special_head, nullptr, bits, g, d_matches));
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
                 }
                 else
-                    TG_TRY(launch_lean<true>(ctx, lookup->geo, (const long long*)key.data, tiles, (const int4*)table, lookup->special_head, jp->as<int>(), g, d_matches));
+                    TG_TRY(launch_lean<true>(ctx, lookup->geo, keys, tiles, (const int4*)table, lookup->special_head, nullptr, bits, g, d_matches));
                 done = tiles * 1024;
             }
         }
@@ -1589,14 +1667,15 @@ struct JoinProbeOp : tgpu_op {
                 for (int c = 0; c < gt.count; c++) gt.dst[c] = (char*)gt.dst[c] + done * gt.elem[c];
             }
             int tgrid = tg_grid(ctx, n - done, 256 * ROWS, 8);
-            if (fast) TG_LAUNCH(ctx, k_fast, tgrid, 256, 0, kr, KEY_INT, n - done, table, lookup->geo, lookup->special_head, jp->as<int>() + done, gt, d_matches);
-            else TG_LAUNCH(ctx, k_any, tgrid, 256, 0, kr, key_kind_of(key.type), n - done, table, lookup->geo, lookup->special_head, jp->as<int>() + done, gt, d_matches);
+            // done is a multiple of 1024: the tail's bitmap starts at a word boundary
+            if (fast) TG_LAUNCH(ctx, k_fast, tgrid, 256, 0, kr, KEY_INT, n - done, table, lookup->geo, lookup->special_head, bits + done / 32, gt, d_matches);
+            else TG_LAUNCH(ctx, k_any, tgrid, 256, 0, kr, key_kind_of(key.type), n - done, table, lookup->geo, lookup->special_head, bits + done / 32, gt, d_matches);
         }
         TG_TIMED_END(ctx);
         *handled = true;
         deferred.active = true;
         deferred.in = std::move(in);
-        deferred.jp = jp;
+        deferred.match_bits = match_bits;
         deferred.built = std::move(built);
         deferred.n = n;
         return TGPU_OK;
@@ -1640,7 +1719,7 @@ struct JoinProbeOp : tgpu_op {
     {
         deferred.active = false;
         DevPage in = std::move(deferred.in);
-        std::shared_ptr<DevBuf> jp = std::move(deferred.jp);
+        std::shared_ptr<DevBuf> match_bits = std::move(deferred.match_bits);
         std::vector<DevColumn> built = std::move(deferred.built);
         const int64_t n = deferred.n;
         const bool outer = join_type == TGPU_JOIN_PROBE_OUTER;     // (tracking join types never take the fast path)
@@ -1653,12 +1732,9 @@ struct JoinProbeOp : tgpu_op {
             // (LookupJoinPageBuilder.build :144-150 "outputProbeBlocksDirectly")
             outp.rows = n;
             for (int32_t ch : output_channels) outp.cols.push_back(in.cols[ch]);
+            // a PROBE_OUTER page with misses: the match bitmap is the build columns' validity as it stands (bits past n are 0)
             std::shared_ptr<DevBuf> validity;
-            if (matches < n) {
-                validity = std::make_shared<DevBuf>();
-                TG_TRY(validity->alloc(ctx, (size_t)((n + 7) / 8)));
-                TG_LAUNCH(ctx, join_match_validity_kernel, tg_grid(ctx, (n + 7) / 8, 256, 8), 256, 0, jp->as<int>(), n, validity->as<uint8_t>());
-            }
+            if (matches < n) validity = match_bits;
             for (auto& c : built) {
                 if (validity) { c.own_validity = validity; c.validity = validity->as<uint8_t>(); }
                 outp.cols.push_back(std::move(c));
@@ -1669,7 +1745,7 @@ struct JoinProbeOp : tgpu_op {
             // compact the matched rows (stable): selection list, then sequential-read gathers
             DevBuf flags, sel;
             TG_TRY(flags.alloc(ctx, (size_t)n));
-            TG_LAUNCH(ctx, join_match_flags_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, jp->as<int>(), n, flags.as<uint8_t>());
+            TG_LAUNCH(ctx, join_match_flags_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, match_bits->as<unsigned int>(), n, flags.as<uint8_t>());
             TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, &ctx->d_scratch->join_probe_count));
             outp.rows = matches;
             for (int32_t ch : output_channels) {
@@ -2011,7 +2087,7 @@ extern "C" int64_t tgpu_lookup_memory_bytes(const tgpu_lookup* lookup)
     if (!lookup) return 0;
     int64_t b = (int64_t)lookup->table.bytes + (int64_t)lookup->links.bytes + lookup->store.memory_bytes();
     for (auto& s : lookup->by_slot) b += (int64_t)s.bytes;
-    b += (int64_t)lookup->wide.bytes;
+    b += (int64_t)lookup->wide.bytes + (int64_t)lookup->keyed.bytes;
     return b;
 }
 
