@@ -291,9 +291,22 @@ void tgpu_partial_agg_controller_on_flush(tgpu_partial_agg_controller* controlle
 int tgpu_agg_rows_with_partial_aggregation_disabled(tgpu_op* op, int64_t* out);
 
 int tgpu_agg_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op** out);
+
+/* AggregationOperator (M/operator/AggregationOperator.java:35-176) + Aggregator (M/operator/aggregation/Aggregator.java:31-109):
+ * aggregation without GROUP BY keys (LocalExecutionPlanner.planGlobalAggregation, and the statistics aggregations of table writes).
+ * Reads of tgpu_agg_spec: step (all four), num_aggs / aggs, pre, and num_input_channels / input_channel_types, which are required -
+ * they shape the output row when no page ever arrives.  INVALID_ARGUMENT when anything else is set: num_keys != 0,
+ * max_partial_bytes != 0, global grouping sets (num_global_group_ids, global_group_ids, group_id_key >= 0; set group_id_key to -1)
+ * or a partial aggregation controller.  The aggregate functions and argument types are those of tgpu_agg_create, with NOT_SUPPORTED
+ * in the same places (REAL or VARCHAR arguments, min/max over a long DECIMAL, a fused pre-stage over 128-bit or REAL channels).
+ * Protocol: needs_input is true until finish; get_output returns nothing until finish, then exactly one page of one row, after which
+ * is_finished is true.  The row holds the final values (SINGLE / FINAL) or the intermediate state columns in the layout above
+ * (PARTIAL / INTERMEDIATE).  Empty input gives the empty accumulators' row in every step: count 0 and every other aggregate NULL;
+ * as states, avg is (0, 0.0) and a decimal sum NULL with overflow 0.  DOUBLE results are run-to-run identical for the same pages. */
+int tgpu_aggregation_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op** out);
 /* diagnostics (needs no GPU): generate the kernel specialised for `spec` over input channels of the given tgpu_types
  * (bit c of nullable_mask = channel c carries NULLs), compile it with NVRTC for sm_90a; returns the cubin size and
- * the generated source (or the compiler log on failure) */
+ * the generated source (or the compiler log on failure).  num_keys == 0: the kernel of tgpu_aggregation_create. */
 int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* channel_types, int32_t num_channels, uint32_t nullable_mask,
                           int64_t* cubin_bytes, char* source_out, int64_t source_cap);
 /* Same for the FilterAndProject kernels generated from `program` (tg_fp_filter_jit / tg_fp_project_jit). */

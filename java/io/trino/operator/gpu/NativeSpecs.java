@@ -85,33 +85,14 @@ public final class NativeSpecs
             MemorySegment partialAggregationController)
     {
         try (Arena arena = Arena.ofConfined()) {
-            MemorySegment fns = arena.allocate(AGG_FN, Math.max(1, aggregates.size()));
-            for (int i = 0; i < aggregates.size(); i++) {
-                GpuAggregate aggregate = aggregates.get(i);
-                long at = i * AGG_FN.byteSize();
-                fns.set(JAVA_INT, at, aggregate.function());
-                fns.set(JAVA_INT, at + 4, aggregate.inputChannel());
-                fns.set(JAVA_INT, at + 8, aggregate.maskChannel());
-                fns.set(JAVA_INT, at + 12, aggregate.resultType());      // avg(decimal) in a FINAL step: TGPU_INT64 / TGPU_INT128, else 0
-            }
-            MemorySegment types = arena.allocate(JAVA_INT, Math.max(1, inputChannelTypes.length));
-            for (int i = 0; i < inputChannelTypes.length; i++) {
-                types.setAtIndex(JAVA_INT, i, inputChannelTypes[i]);
-            }
-            MemorySegment spec = arena.allocate(AGG_SPEC);
+            MemorySegment spec = aggregationSpec(arena, step, aggregates, inputChannelTypes, preProgram);
             spec.set(JAVA_INT, 0, groupByChannels.size());
             spec.set(ADDRESS, 8, ints(arena, groupByChannels));
-            spec.set(JAVA_INT, 16, stepCode(step));
-            spec.set(JAVA_INT, 20, aggregates.size());
-            spec.set(ADDRESS, 24, fns);
             spec.set(JAVA_LONG, 32, expectedGroups);
             spec.set(JAVA_LONG, 40, maxPartialMemory);
-            spec.set(ADDRESS, 48, preProgram);
             spec.set(JAVA_INT, 56, globalAggregationGroupIds.size());
             spec.set(ADDRESS, 64, ints(arena, globalAggregationGroupIds));
             spec.set(JAVA_INT, 72, groupIdKey);
-            spec.set(JAVA_INT, 76, inputChannelTypes.length);
-            spec.set(ADDRESS, 80, types);
             spec.set(ADDRESS, 88, partialAggregationController);       // MemorySegment.NULL = Optional.empty()
             return create(gpu, TrinoGpuLibrary.AGG_CREATE, spec, arena);
         }
@@ -121,6 +102,48 @@ public final class NativeSpecs
         catch (Throwable e) {
             throw new RuntimeException(e);
         }
+    }
+
+    /** AggregationOperator (tgpu_aggregation_create): no keys, no flush threshold, no grouping sets, no controller */
+    public static MemorySegment createGlobalAggregation(GpuContexts.Handle gpu, Step step, List<GpuAggregate> aggregates, int[] inputChannelTypes, MemorySegment preProgram)
+    {
+        try (Arena arena = Arena.ofConfined()) {
+            MemorySegment spec = aggregationSpec(arena, step, aggregates, inputChannelTypes, preProgram);
+            spec.set(JAVA_INT, 72, -1);                                 // group_id_key
+            return create(gpu, TrinoGpuLibrary.AGGREGATION_CREATE, spec, arena);
+        }
+        catch (RuntimeException e) {
+            throw e;
+        }
+        catch (Throwable e) {
+            throw new RuntimeException(e);
+        }
+    }
+
+    // tgpu_agg_spec with the fields both aggregation operators read; the others zero / NULL
+    private static MemorySegment aggregationSpec(Arena arena, Step step, List<GpuAggregate> aggregates, int[] inputChannelTypes, MemorySegment preProgram)
+    {
+        MemorySegment fns = arena.allocate(AGG_FN, Math.max(1, aggregates.size()));
+        for (int i = 0; i < aggregates.size(); i++) {
+            GpuAggregate aggregate = aggregates.get(i);
+            long at = i * AGG_FN.byteSize();
+            fns.set(JAVA_INT, at, aggregate.function());
+            fns.set(JAVA_INT, at + 4, aggregate.inputChannel());
+            fns.set(JAVA_INT, at + 8, aggregate.maskChannel());
+            fns.set(JAVA_INT, at + 12, aggregate.resultType());      // avg(decimal) in a FINAL step: TGPU_INT64 / TGPU_INT128, else 0
+        }
+        MemorySegment types = arena.allocate(JAVA_INT, Math.max(1, inputChannelTypes.length));
+        for (int i = 0; i < inputChannelTypes.length; i++) {
+            types.setAtIndex(JAVA_INT, i, inputChannelTypes[i]);
+        }
+        MemorySegment spec = arena.allocate(AGG_SPEC);                 // zero-filled: no keys, NULL pointers
+        spec.set(JAVA_INT, 16, stepCode(step));
+        spec.set(JAVA_INT, 20, aggregates.size());
+        spec.set(ADDRESS, 24, fns);
+        spec.set(ADDRESS, 48, preProgram);
+        spec.set(JAVA_INT, 76, inputChannelTypes.length);
+        spec.set(ADDRESS, 80, types);
+        return spec;
     }
 
     public static MemorySegment createJoinBuild(GpuContexts.Handle gpu, List<Integer> hashChannels, List<Integer> outputChannels, long expectedPositions)

@@ -40,6 +40,7 @@ public final class TrinoGpuLibrary
     // operator factories
     static final MethodHandle FILTER_PROJECT_CREATE = handle("tgpu_filter_project_create", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
     static final MethodHandle AGG_CREATE = handle("tgpu_agg_create", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
+    static final MethodHandle AGGREGATION_CREATE = handle("tgpu_aggregation_create", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
     // PartialAggregationController lives in the library so that GPU operators report their flushes without an upcall
     static final MethodHandle PA_CONTROLLER_CREATE = handle("tgpu_partial_agg_controller_create", FunctionDescriptor.of(JAVA_INT, JAVA_LONG, JAVA_DOUBLE, ADDRESS));
     static final MethodHandle PA_CONTROLLER_DESTROY = handle("tgpu_partial_agg_controller_destroy", FunctionDescriptor.ofVoid(ADDRESS));

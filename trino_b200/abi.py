@@ -184,6 +184,7 @@ SIGNATURES = {
     "tgpu_ctx_last_kernel_ms": (C.c_int, [VP, C.POINTER(C.c_float)]),
     "tgpu_filter_project_create": (C.c_int, [VP, C.POINTER(ExprProgram), C.POINTER(VP)]),
     "tgpu_agg_create": (C.c_int, [VP, C.POINTER(AggSpec), C.POINTER(VP)]),
+    "tgpu_aggregation_create": (C.c_int, [VP, C.POINTER(AggSpec), C.POINTER(VP)]),
     "tgpu_agg_group_count": (C.c_int, [VP, C.POINTER(C.c_int64)]),
     "tgpu_agg_rows_with_partial_aggregation_disabled": (C.c_int, [VP, C.POINTER(C.c_int64)]),
     "tgpu_partial_agg_controller_create": (C.c_int, [C.c_int64, C.c_double, C.POINTER(VP)]),

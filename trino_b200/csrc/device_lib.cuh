@@ -4,7 +4,7 @@
 //
 // Contents: column refs, validity/loads, the reference's hash mixers, the per-operation semantics of the
 // expression evaluator (one function, folded at compile time when op/type are constants), accumulator
-// arithmetic, and the body of the small-group fused aggregation kernel as a template over a row program.
+// arithmetic, and the bodies of the fused aggregation kernels (small-group, global, general) as templates over a row program.
 #ifndef TG_DEVICE_LIB_CUH
 #define TG_DEVICE_LIB_CUH
 
@@ -462,6 +462,104 @@ __device__ __forceinline__ void agg_small_body(P& prog, const DColumns& cols, in
         out.blk_first[b * (L + 2) + s] = lfirst[s];
         if (s < L) out.blk_keys[b * L + s] = tkeys[s];
     }
+}
+
+// ---- global aggregation (no GROUP BY keys): kernel body as a template over the same row program -----------------------------
+// Fixed-order CTA reduction of per-thread accumulator words: an xor-shuffle tree inside every warp (a 128-bit integer sum travels as
+// its LO/HI pair with the carry, as in agg_small_body), then the warps folded in warp order through shared memory `wpart`
+// ([warps][A]); thread a writes the CTA's word a to out[a].  `kind_of(a)` = accumulator kind of word a.
+template <class KindOf>
+__device__ __forceinline__ void tgd_cta_reduce(const unsigned long long* acc, int A, KindOf kind_of, unsigned long long* wpart, unsigned long long* out)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+#pragma unroll
+    for (int a = 0; a < A; a++) {
+        const int kind = kind_of(a);
+        if (kind == ACC_SUM_I64_HI) continue;
+        if (kind == ACC_SUM_I64_LO) {
+            unsigned long long lo = acc[a], hi = acc[a + 1];
+            for (int off = 16; off > 0; off >>= 1) {
+                unsigned long long ol = __shfl_xor_sync(0xffffffffu, lo, off), oh = __shfl_xor_sync(0xffffffffu, hi, off);
+                unsigned long long o = lo; lo += ol; hi += oh + (lo < o ? 1 : 0);
+            }
+            if (lane == 0) { wpart[warp * A + a] = lo; wpart[warp * A + a + 1] = hi; }
+        }
+        else {
+            unsigned long long r = acc[a];
+            for (int off = 16; off > 0; off >>= 1) r = acc_combine(kind, r, __shfl_xor_sync(0xffffffffu, r, off));
+            if (lane == 0) wpart[warp * A + a] = r;
+        }
+    }
+    __syncthreads();
+    for (int a = threadIdx.x; a < A; a += blockDim.x) {
+        const int kind = kind_of(a);
+        if (kind == ACC_SUM_I64_HI) continue;
+        if (kind == ACC_SUM_I64_LO) {
+            unsigned long long lo = 0, hi = 0;
+            for (int w = 0; w < nwarps; w++) { unsigned long long o = lo; lo += wpart[w * A + a]; hi += wpart[w * A + a + 1] + (lo < o ? 1 : 0); }
+            out[a] = lo;
+            out[a + 1] = hi;
+        }
+        else {
+            unsigned long long r = acc_init(kind);
+            for (int w = 0; w < nwarps; w++) r = acc_combine(kind, r, wpart[w * A + a]);
+            out[a] = r;
+        }
+    }
+}
+
+// AggregationOperator's hot loop: every row of the page folds into ONE group, so the accumulators are per-thread registers
+// (acc[P::A] at stride 1: the generated accumulate() indexes them with constants), with no table, no first-row stamps and no atomics
+// in the row loop.  A thread owns 4 consecutive rows per trip of a grid-stride loop.  Deferred loads: the columns only the filter reads
+// come first (load4_early / load_early); the other columns (projection and aggregate inputs) are read only when one of the thread's 4
+// rows passed the filter - for an 8-byte column the 4 rows are one 32-byte sector, which a thread whose rows all fail never touches.
+// Output: the CTA's accumulator words at part[blockIdx.x * A] (folded in CTA order by agg_global_fold_kernel) and the error bits.
+// P supplies, besides the members agg_small_body uses: load_early / load_late / load4_early / load4_late (the two halves of load /
+// load4) and filter(regs, &err) (the filter alone; its errors count on every row).
+template <class P>
+__device__ __forceinline__ void agg_global_body(P& prog, const DColumns& cols, int64_t n, unsigned long long* __restrict__ part, unsigned int* __restrict__ err_out)
+{
+    constexpr int A = P::A, R = 4, T = TGD_S_THREADS;
+    static_assert(A >= 1, "at least one accumulator word");
+    __shared__ unsigned long long wpart[(T / 32) * A];
+    unsigned long long acc[A];
+#pragma unroll
+    for (int a = 0; a < A; a++) acc[a] = acc_init(P::acc_kind(a));
+    uint32_t err = 0;
+    const int64_t stride = (int64_t)gridDim.x * T * R;
+    for (int64_t base = ((int64_t)blockIdx.x * T + threadIdx.x) * R; base < n; base += stride) {
+        typename P::Regs regs[R];
+        const bool vec = P::VEC && base + R <= n;
+        if (vec) prog.load4_early(cols, base, regs);
+        else {
+#pragma unroll
+            for (int j = 0; j < R; j++)
+                if (base + j < n) prog.load_early(cols, base + j, regs[j]);
+        }
+        bool pass[R];
+        bool any = false;
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            pass[j] = base + j < n && prog.filter(regs[j], &err);
+            any |= pass[j];
+        }
+        if (!any) continue;
+        if (vec) prog.load4_late(cols, base, regs);
+        else {
+#pragma unroll
+            for (int j = 0; j < R; j++)
+                if (pass[j]) prog.load_late(cols, base + j, regs[j]);
+        }
+#pragma unroll
+        for (int j = 0; j < R; j++) {
+            if (!pass[j]) continue;
+            unsigned long long pk = 0;
+            int special = -1;
+            if (prog.row(regs[j], &pk, &special, &err)) prog.accumulate(acc, 1);
+        }
+    }
+    tgd_cta_reduce(acc, A, [](int a) { return P::acc_kind(a); }, wpart, part + (size_t)blockIdx.x * A);
+    if (err) atomicOr(err_out, err);
 }
 
 // ---- general group-by, fused single pass (path G): kernel body as a template over the same row program ---------------------

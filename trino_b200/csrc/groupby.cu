@@ -1,4 +1,4 @@
-// groupby.cu — HashAggregationOperator / GroupByHash / grouped accumulators for sm_90a.
+// groupby.cu — HashAggregationOperator / AggregationOperator / GroupByHash / grouped accumulators for sm_90a.
 //
 // Reference semantics reproduced:
 //   - GroupByHash contract (M/operator/GroupByHash.java:118-125): group ids are dense, 0-based and assigned in
@@ -22,6 +22,11 @@
 //   G (general): global open-addressing table {key, gid, first_row}; provisional inserts record the minimum
 //                row per new key, new groups are ranked with a prefix sum over "representative row" flags,
 //                then accumulators are updated with L2 atomics (RED.ADD.F64 / atomicAdd / atomicMin/Max).
+// Global (AggregationOperator, M/operator/AggregationOperator.java:35-176; tgpu_aggregation_create): no keys, one group created with
+//                the empty accumulators at create, so an empty input still yields its one row through the same output kernel.  One
+//                kernel per page (tg_agg_global_jit, agg_global_body of device_lib.cuh, or its interpreter twin agg_global_kernel): the
+//                pre-stage and the accumulators in registers, loads of the columns the filter does not read deferred until a row
+//                passed, a fixed-order CTA reduction, then agg_global_fold_kernel folds the CTA partials in CTA order (deterministic).
 // Keys are packed exactly into one 64-bit word (single key of any fixed width, or several narrow keys with
 // one null bit each, <= 63 bits); other key shapes return NOT_SUPPORTED so the caller keeps the Java operator.
 #include <algorithm>
@@ -56,6 +61,7 @@ constexpr int MAX_SRCS = 32;
 constexpr int MAX_ACCS = 40;   // (a FINAL decimal sum alone takes 9: four 128-bit pairs and its non-NULL counter)
 constexpr int S_THREADS = TGD_S_THREADS;
 static_assert(TGD_MAX_CHANNELS == TGPU_MAX_CHANNELS, "channel limits differ");
+constexpr int GLOBAL_MIN_BLOCKS = 4;   // resident CTAs per SM the global kernel is compiled for (__launch_bounds__: <= 64 registers)
 constexpr int S_GMAX = 64;             // regular groups the S path can hold (+2 special)
 constexpr int S_SPECIAL_NULL = 0;      // special slot for the NULL key (single-key case)
 constexpr int S_SPECIAL_SENTINEL = 1;  // special slot for a key whose bits equal EMPTY_KEY
@@ -421,6 +427,91 @@ __global__ void __launch_bounds__(256) agg_small_merge_kernel(AggPlan plan, DCol
     }
     __syncthreads();
     if (tid == 0) st.count[0] = count + total_new;
+}
+
+// =====================================================================================================
+// global aggregation (AggregationOperator: no GROUP BY keys, one group)
+// =====================================================================================================
+// Interpreter twin of tg_agg_global_jit (agg_global_body), for processes without NVRTC: the pre-stage through vm_run, sources through
+// fetch_src, accumulators in thread-private words, then the same fixed-order CTA reduction.  part: [gridDim.x][plan.num_accs].
+__global__ void __launch_bounds__(S_THREADS) agg_global_kernel(AggPlan plan, DColumns cols, const DProgram* __restrict__ prog, int64_t n,
+                                                              unsigned long long* __restrict__ part, unsigned int* __restrict__ err_out)
+{
+    __shared__ int64_t temps_base[TGPU_MAX_TEMPS * S_THREADS];
+    __shared__ unsigned long long wpart[(S_THREADS / 32) * MAX_ACCS];
+    const int A = plan.num_accs;
+    const int T = S_THREADS;
+    int64_t* temps = temps_base + threadIdx.x;
+    unsigned long long acc[MAX_ACCS];
+    for (int a = 0; a < A; a++) acc[a] = acc_init(plan.accs[a].kind);
+    uint32_t err = 0;
+    uint32_t read_errs = 0;      // the 4-bit error fields (vm_run) of the temps the aggregation reads
+    for (int i = 0; i < plan.num_srcs; i++)
+        if (plan.srcs[i].is_temp) read_errs |= 0xFu << (4 * plan.srcs[i].index);
+    for (int64_t row = (int64_t)blockIdx.x * T + threadIdx.x; row < n; row += (int64_t)gridDim.x * T) {
+        uint32_t nb = 0;
+        if (plan.has_pre) {
+            uint32_t te = 0;
+            if (prog->filter_temp >= 0) {
+                nb = vm_run(prog, 0, prog->num_filter_insns, cols, row, temps, T, 0, &te);
+                int ft = prog->filter_temp;
+                err |= vm_temp_error(te, ft);      // the filter's errors count on every row
+                if ((nb >> ft) & 1 || temps[ft * T] == 0) continue;
+            }
+            nb = vm_run(prog, prog->num_filter_insns, prog->num_insns, cols, row, temps, T, nb, &te);
+            uint32_t e = te & read_errs;         // a projection raises only when the aggregation reads it
+            e |= e >> 16;
+            e |= e >> 8;
+            e |= e >> 4;
+            err |= e & 0xFu;
+        }
+        int last_src = -2;
+        Fetched v;
+        v.bits = 0; v.is_null = false;
+        for (int a = 0; a < A; a++) {
+            const AccDesc& d = plan.accs[a];
+            if (d.kind == ACC_SUM_I64_HI) continue;
+            if (!mask_selected(plan, d.mask, cols, row, temps, T, nb)) continue;
+            if (d.src >= 0 && d.src != last_src) { v = fetch_src(plan.srcs[d.src], cols, row, temps, T, nb); last_src = d.src; }
+            if (d.kind != ACC_ROWS && v.is_null) continue;
+            acc_update_private(d.kind, &acc[a], 1, v.bits);
+        }
+    }
+    tgd_cta_reduce(acc, A, [&](int a) { return plan.accs[a].kind; }, wpart, part + (size_t)blockIdx.x * A);
+    if (err) atomicOr(err_out, err);
+}
+
+// single-CTA fold of the B CTA partials of one page into the one-group state: a warp per accumulator, lanes fold CTAs lane, lane + 32,
+// ... in order, then an xor tree - the same order for the same page, so DOUBLE sums are run-to-run identical.  C = words per partial
+// (the specialised kernel's compact accumulator space, map.of_plan translates).
+__global__ void __launch_bounds__(256) agg_global_fold_kernel(AggPlan plan, const unsigned long long* __restrict__ part, int B, int C, AccMap map, AggState st)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    for (int a = warp; a < plan.num_accs; a += nwarps) {
+        const int kind = plan.accs[a].kind;
+        if (kind == ACC_SUM_I64_HI) continue;
+        const int c = map.of_plan[a];
+        unsigned long long* s = &st.acc[(size_t)a * st.cap];
+        if (kind == ACC_SUM_I64_LO) {
+            unsigned long long lo = 0, hi = 0;
+            for (int b = lane; b < B; b += 32) { unsigned long long o = lo; lo += part[(size_t)b * C + c]; hi += part[(size_t)b * C + c + 1] + (lo < o ? 1 : 0); }
+            for (int off = 16; off > 0; off >>= 1) {
+                unsigned long long ol = __shfl_xor_sync(0xffffffffu, lo, off), oh = __shfl_xor_sync(0xffffffffu, hi, off);
+                unsigned long long o = lo; lo += ol; hi += oh + (lo < o ? 1 : 0);
+            }
+            if (lane == 0) {
+                unsigned long long o = s[0];
+                s[0] = o + lo;
+                s[st.cap] += hi + (s[0] < o ? 1 : 0);
+            }
+        }
+        else {
+            unsigned long long r = acc_init(kind);
+            for (int b = lane; b < B; b += 32) r = acc_combine(kind, r, part[(size_t)b * C + c]);
+            for (int off = 16; off > 0; off >>= 1) r = acc_combine(kind, r, __shfl_xor_sync(0xffffffffu, r, off));
+            if (lane == 0) s[0] = acc_combine(kind, s[0], r);
+        }
+    }
 }
 
 // =====================================================================================================
@@ -1340,8 +1431,9 @@ static int general_rows_per_thread()
     return r == 1 || r == 2 || r == 4 || r == 8 ? r : TGD_G_ROWS;
 }
 
+// `global`: the AggregationOperator kernel tg_agg_global_jit (no keys; loads split around the filter) instead of the keyed kernels
 static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* prog, const int* elems, int num_channels, int L, int min_blocks,
-                                        uint32_t nullable_mask, AccMap* map, bool vec = false)
+                                        uint32_t nullable_mask, AccMap* map, bool vec = false, bool global = false)
 {
     std::string s;
     bool used[TGPU_MAX_CHANNELS] = {false};
@@ -1395,6 +1487,7 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         for (int r = 0; r < plan.num_accs; r++)
             if (plan.accs[r].kind == ACC_ROWS && plan.accs[r].mask == d.mask) map->of_plan[a] = map->of_plan[r];
     }
+    if (global && compact == 0) kinds[compact++] = ACC_ROWS;      // (no aggregate at all: one unused counter keeps the kernel well-formed)
     map->compact_count = compact;
 
     appendf(s, "struct Prog {\n  static constexpr int L = %d, A = %d, R = 4, GR = %d;\n  static constexpr bool VEC = %s, SPECIALS = %s;\n", L, compact, general_rows_per_thread(),
@@ -1407,74 +1500,110 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         if (used[c]) appendf(s, "    long long c%d; bool c%dn;\n", c, c);
     s += "  };\n";
     for (int i = 0; i < plan.num_srcs; i++) appendf(s, "  long long v%d; bool vn%d;\n", i, i);
-    // all global loads of a row, nothing else: the body issues them for R rows back to back
-    s += "  __device__ __forceinline__ void load(const DColumns& cols, long long row, Regs& r) {\n";
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        if (!used[c]) continue;
-        appendf(s, "    r.c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
-        if ((nullable_mask >> c) & 1) appendf(s, " r.c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
-        else appendf(s, " r.c%dn = false;\n", c);
-    }
-    s += "  }\n";
-    // the same for FOUR CONSECUTIVE rows starting at a multiple of 4 (VEC kernels: every column base is 16-byte aligned): one or two
-    // 16-byte loads per wide column, one 4-byte load per INT8 column, the four validity bits from one byte
-    s += "  __device__ __forceinline__ void load4(const DColumns& cols, long long row0, Regs (&r)[4]) {\n";
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        if (!used[c]) continue;
-        switch (elems[c]) {
-            case 8:
-                appendf(s, "    { const longlong2* p = (const longlong2*)((const char*)cols.cols[%d].data + row0 * 8); longlong2 a = p[0], b = p[1];"
-                           " r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = b.x; r[3].c%d = b.y; }\n", c, c, c, c, c);
-                break;
-            case 4:
-                appendf(s, "    { int4 a = *(const int4*)((const char*)cols.cols[%d].data + row0 * 4); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                        c, c, c, c, c);
-                break;
-            case 2:
-                appendf(s, "    { short4 a = *(const short4*)((const char*)cols.cols[%d].data + row0 * 2); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                        c, c, c, c, c);
-                break;
-            default:
-                appendf(s, "    { char4 a = *(const char4*)((const char*)cols.cols[%d].data + row0); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                        c, c, c, c, c);
-                break;
+    // global kernel: the columns the filter reads are loaded first, the others only for rows that passed it (agg_global_body)
+    bool early[TGPU_MAX_CHANNELS] = {false};
+    const bool has_filter = prog && prog->filter_temp >= 0;
+    if (has_filter)
+        for (int i = 0; i < prog->num_filter_insns; i++) {
+            const DInsn& in = prog->insns[i];
+            const DOperand* ops[3] = {&in.a, &in.b, &in.c};
+            for (auto* o : ops)
+                if (o->kind == TGPU_OPND_COLUMN) early[o->index] = true;
         }
-        if ((nullable_mask >> c) & 1)
-            appendf(s, "    { const uint8_t* v = cols.cols[%d].validity; unsigned int b = v ? ((unsigned int)v[row0 >> 3] >> (row0 & 7)) : 0xfu;"
-                       " r[0].c%dn = !(b & 1); r[1].c%dn = !(b & 2); r[2].c%dn = !(b & 4); r[3].c%dn = !(b & 8); }\n", c, c, c, c, c);
-        else appendf(s, "    r[0].c%dn = r[1].c%dn = r[2].c%dn = r[3].c%dn = false;\n", c, c, c, c);
+    for (int c = 0; c < TGPU_MAX_CHANNELS; c++) early[c] = early[c] || !has_filter;
+    auto loads = [&](const char* name, const char* name4, int which /* 0 all, 1 early, 2 late */) {
+        auto wanted = [&](int c) { return used[c] && (which == 0 || (which == 1) == early[c]); };
+        // all global loads of a row, nothing else: the body issues them for R rows back to back
+        appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row, Regs& r) {\n", name);
+        for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
+            if (!wanted(c)) continue;
+            appendf(s, "    r.c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
+            if ((nullable_mask >> c) & 1) appendf(s, " r.c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
+            else appendf(s, " r.c%dn = false;\n", c);
+        }
+        s += "  }\n";
+        // the same for FOUR CONSECUTIVE rows starting at a multiple of 4 (VEC kernels: every column base is 16-byte aligned): one or two
+        // 16-byte loads per wide column, one 4-byte load per INT8 column, the four validity bits from one byte
+        appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row0, Regs (&r)[4]) {\n", name4);
+        for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
+            if (!wanted(c)) continue;
+            switch (elems[c]) {
+                case 8:
+                    appendf(s, "    { const longlong2* p = (const longlong2*)((const char*)cols.cols[%d].data + row0 * 8); longlong2 a = p[0], b = p[1];"
+                               " r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = b.x; r[3].c%d = b.y; }\n", c, c, c, c, c);
+                    break;
+                case 4:
+                    appendf(s, "    { int4 a = *(const int4*)((const char*)cols.cols[%d].data + row0 * 4); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                            c, c, c, c, c);
+                    break;
+                case 2:
+                    appendf(s, "    { short4 a = *(const short4*)((const char*)cols.cols[%d].data + row0 * 2); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                            c, c, c, c, c);
+                    break;
+                default:
+                    appendf(s, "    { char4 a = *(const char4*)((const char*)cols.cols[%d].data + row0); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                            c, c, c, c, c);
+                    break;
+            }
+            if ((nullable_mask >> c) & 1)
+                appendf(s, "    { const uint8_t* v = cols.cols[%d].validity; unsigned int b = v ? ((unsigned int)v[row0 >> 3] >> (row0 & 7)) : 0xfu;"
+                           " r[0].c%dn = !(b & 1); r[1].c%dn = !(b & 2); r[2].c%dn = !(b & 4); r[3].c%dn = !(b & 8); }\n", c, c, c, c, c);
+            else appendf(s, "    r[0].c%dn = r[1].c%dn = r[2].c%dn = r[3].c%dn = false;\n", c, c, c, c);
+        }
+        s += "  }\n";
+    };
+    if (global) {
+        loads("load_early", "load4_early", 1);
+        loads("load_late", "load4_late", 2);
     }
-    s += "  }\n";
+    else loads("load", "load4", 0);
+    auto opnd_error = [](const DOperand& o) { return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : std::string("0u"); };
+    auto emit_insn = [&](const DInsn& in) {
+        if (in.op == TGPU_EX_IN) {
+            int li = (int)in.b.imm;
+            appendf(s, "    { Value a = %s; bool hit = false;\n", gen_operand(in.a).c_str());
+            for (int k = 0; k < prog->in_count[li]; k++) {
+                unsigned long long c = (unsigned long long)prog->in_values[prog->in_offset[li] + k];
+                if (in.vtype == TGPU_V_DOUBLE) appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
+                else appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
+            }
+            appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, opnd_error(in.a).c_str());
+        }
+        else {
+            // operands are read into locals first: dst may be one of them, and vm_error needs their values
+            appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", gen_operand(in.a).c_str(),
+                    gen_operand(in.b).c_str(), gen_operand(in.c).c_str(), in.op, in.vtype);
+            appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
+                    opnd_error(in.a).c_str(), opnd_error(in.b).c_str(), opnd_error(in.c).c_str(), in.dst, in.dst, in.dst);
+        }
+    };
+    auto emit_columns_and_temps = [&](bool only_early) {
+        for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++)
+            if (used[c] && (!only_early || early[c])) appendf(s, "    const long long c%d = r.c%d; const bool c%dn = r.c%dn;\n", c, c, c, c);
+        if (prog)
+            for (int t = 0; t < TGPU_MAX_TEMPS; t++) appendf(s, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    };
+    if (global) {
+        // the filter alone, over the early columns (its errors count on every row); row() evaluates it again for the rows that passed
+        s += "  __device__ __forceinline__ bool filter(const Regs& r, unsigned int* err) {\n";
+        if (has_filter) {
+            emit_columns_and_temps(true);
+            for (int i = 0; i < prog->num_filter_insns; i++) emit_insn(prog->insns[i]);
+            appendf(s, "    *err |= te%d;\n    return !(tn%d || t%d == 0);\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
+        }
+        else s += "    return true;\n";
+        s += "  }\n";
+    }
     s += "  __device__ __forceinline__ bool row(const Regs& r, unsigned long long* pk, int* special, unsigned int* err) {\n";
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++)
-        if (used[c]) appendf(s, "    const long long c%d = r.c%d; const bool c%dn = r.c%dn;\n", c, c, c, c);
+    emit_columns_and_temps(false);
     if (prog) {
-        for (int t = 0; t < TGPU_MAX_TEMPS; t++) appendf(s, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
         // the filter's errors count on every row, a projection's only when the aggregation reads it (see vm_error)
         auto filter_check = [&]() {
             appendf(s, "    *err |= te%d;\n    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
         };
-        auto opnd_error = [](const DOperand& o) { return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : std::string("0u"); };
         for (int i = 0; i < prog->num_insns; i++) {
-            const DInsn& in = prog->insns[i];
             if (i == prog->num_filter_insns && prog->filter_temp >= 0) filter_check();
-            if (in.op == TGPU_EX_IN) {
-                int li = (int)in.b.imm;
-                appendf(s, "    { Value a = %s; bool hit = false;\n", gen_operand(in.a).c_str());
-                for (int k = 0; k < prog->in_count[li]; k++) {
-                    unsigned long long c = (unsigned long long)prog->in_values[prog->in_offset[li] + k];
-                    if (in.vtype == TGPU_V_DOUBLE) appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
-                    else appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
-                }
-                appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, opnd_error(in.a).c_str());
-            }
-            else {
-                // operands are read into locals first: dst may be one of them, and vm_error needs their values
-                appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", gen_operand(in.a).c_str(),
-                        gen_operand(in.b).c_str(), gen_operand(in.c).c_str(), in.op, in.vtype);
-                appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
-                        opnd_error(in.a).c_str(), opnd_error(in.b).c_str(), opnd_error(in.c).c_str(), in.dst, in.dst, in.dst);
-            }
+            emit_insn(prog->insns[i]);
         }
         if (prog->num_filter_insns == prog->num_insns && prog->filter_temp >= 0) filter_check();
         for (int i = 0; i < plan.num_srcs; i++)
@@ -1491,7 +1620,7 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
             s += "    if ((u << 1) == 0) u = 0;\n    if ((u & 0x7FFFFFFFFFFFFFFFULL) > 0x7FF0000000000000ULL) u = 0x7FF8000000000000ULL;\n";
         s += "    if (u == TGD_EMPTY_KEY) { *special = 1; return true; }\n    *pk = u;\n";
     }
-    else {
+    else if (plan.num_keys > 1) {
         s += "    unsigned long long k = 0;\n";
         int shift = 0;
         for (int kk = 0; kk < plan.num_keys; kk++) {
@@ -1514,6 +1643,14 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         else appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, v%d);\n", cond.c_str(), d.kind, map->of_plan[a], d.src);
     }
     s += "  }\n";
+    if (global) {
+        // AggregationOperator: the one-group kernel alone (agg_global_body), no key table and no record reductions
+        s += "};\n";
+        appendf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) tg_agg_global_jit(DColumns cols, long long n, unsigned long long* part, unsigned int* err) {\n",
+                S_THREADS, min_blocks);
+        s += "  Prog p;\n  agg_global_body(p, cols, n, part, err);\n}\n";
+        return s;
+    }
     // the same accumulators as reductions on a fused-G slot record (plan order, the record encoding of gf_accumulate: NONNULL counts the
     // NULL inputs, the 128-bit integer sum is two carry-free 64-bit sums of the value's halves)
     s += "  __device__ __forceinline__ void accumulate_global(unsigned long long* acc) {\n";
@@ -1594,6 +1731,11 @@ struct AggOp : tgpu_op {
     int32_t group_id_key = -1;               // index into key_channels of the $group_id key
     std::vector<int32_t> input_types;        // tgpu_type of every aggregation-input channel (only needed to shape the default rows)
     bool saw_group = false;                  // a group was ever created (across PARTIAL flushes)
+    // AggregationOperator (tgpu_aggregation_create): no keys, ONE group that exists from create on, so the output row of an empty input
+    // comes out of the ordinary output kernel
+    bool global = false;
+    std::vector<int> global_types;           // channel types every page must have once its 128-bit channels are split (planned at create)
+    DevBuf gl_part;                          // CTA partials of the global kernel: [grid][accumulator words]
 
     // resolved at the first page (needs column types)
     bool planned = false;
@@ -1609,8 +1751,9 @@ struct AggOp : tgpu_op {
     int64_t st_cap = 0;
     int64_t group_count = 0;
     // path S scratch
-    struct JitVariant { void* fn = nullptr; AccMap map; };
+    struct JitVariant { void* fn = nullptr; AccMap map; int ctas_per_sm = 0; };
     std::map<uint64_t, JitVariant> jit_variants;   // keyed by (L, which channels carry a validity bitmap)
+    std::map<uint64_t, JitVariant> jit_global_variants;   // tg_agg_global_jit, keyed by (vector loader, which channels carry a validity bitmap)
     std::map<uint64_t, void*> jit_g_variants;      // fused general kernel, keyed by the page layout (element widths, validity bitmaps)
     std::vector<int> jit_elems;
     DevBuf f_tickets;
@@ -1854,7 +1997,7 @@ struct AggOp : tgpu_op {
         src_channel.clear();
         plan.has_pre = has_pre ? 1 : 0;
         int nk = (int)key_channels.size();
-        if (nk < 1) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "global aggregation (no GROUP BY keys) stays on the Java AggregationOperator");
+        if (nk < 1 && !global) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "global aggregation (no GROUP BY keys) is tgpu_aggregation_create's operator");
         if (nk > MAX_KEYS) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "more than %d group-by keys", MAX_KEYS);
         plan.num_keys = nk;
         int total_bits = 0;
@@ -2608,6 +2751,110 @@ struct AggOp : tgpu_op {
         return TGPU_OK;
     }
 
+    // ---- global aggregation (AggregationOperator) ---------------------------------------------------
+    // plan from the declared input types (no page may ever arrive) and create the one group with the empty accumulators
+    int start_global()
+    {
+        DevPage shape;
+        shape.rows = 0;
+        shape.cols.resize(input_types.size());
+        for (size_t c = 0; c < input_types.size(); c++) {
+            shape.cols[c].type = input_types[c];
+            shape.cols[c].length = 0;
+        }
+        TG_TRY(prepare_wide(&shape));
+        TG_TRY(encode_string_keys(&shape));      // (no keys: rejects REAL aggregate inputs as the keyed operator does)
+        TG_TRY(make_plan(shape));
+        for (auto& c : shape.cols) global_types.push_back(c.type);
+        TG_TRY(st_count.alloc(ctx, 64));
+        int32_t init[4] = {1, -1, -1, 0};
+        TG_CUDA(ctx, cudaMemcpyAsync(st_count.p, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
+        group_count = 0;
+        st_cap = 0;
+        TG_TRY(alloc_state(1));
+        group_count = 1;
+        std::vector<unsigned long long> acc(std::max(plan.num_accs, 1));
+        for (int a = 0; a < plan.num_accs; a++) acc[a] = acc_init(plan.accs[a].kind);
+        TG_CUDA(ctx, cudaMemcpyAsync(st_acc.p, acc.data(), acc.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return TGPU_OK;
+    }
+
+    int add_input_global(const tgpu_page* page)
+    {
+        DevPage in;
+        TG_TRY(tg_ingest_page(ctx, page, &in));
+        if ((int)in.cols.size() != (int)input_types.size())
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "page has %zu channels, input_channel_types names %zu", in.cols.size(), input_types.size());
+        TG_TRY(prepare_wide(&in));
+        TG_TRY(encode_string_keys(&in));
+        for (size_t c = 0; c < in.cols.size(); c++)
+            if (in.cols[c].type != global_types[c])
+                return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "channel %zu is type %d, input_channel_types says %d", c, in.cols[c].type, global_types[c]);
+        if (has_pre && prog_max_channel >= (int)in.cols.size())
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "pre-stage reads channel %d, page has %zu", prog_max_channel, in.cols.size());
+        DColumns cols;
+        TG_TRY(fill_cols(in, &cols));
+        return run_global(in, cols);
+    }
+
+    // one page: the fused kernel (specialised, or its interpreter twin), the fold of its CTA partials into the state, one readback
+    int run_global(const DevPage& in, const DColumns& cols)
+    {
+        const int64_t n = in.rows;
+        constexpr int R = 4;            // rows per thread and trip (agg_global_body)
+        AccMap map;
+        void* jit_fn = nullptr;
+        int grid;
+        if (jit_available()) {
+            uint32_t nullable = 0;
+            int elems[TGPU_MAX_CHANNELS] = {0};
+            bool vec = true;               // 16-byte loads of 4 consecutive rows unless a (sliced) column starts off a 16-byte boundary
+            for (size_t c = 0; c < in.cols.size() && c < TGPU_MAX_CHANNELS; c++) {
+                elems[c] = in.cols[c].elem_size();
+                if (in.cols[c].validity) nullable |= 1u << c;
+                vec = vec && ((uintptr_t)in.cols[c].data & 15) == 0;
+            }
+            const uint64_t vkey = nullable | (vec ? 1ULL << 63 : 0);
+            auto it = jit_global_variants.find(vkey);
+            if (it == jit_global_variants.end()) {
+                JitVariant v;
+                std::string src = gen_agg_small_source(plan, has_pre ? &host_prog : nullptr, elems, (int)in.cols.size(), 4, GLOBAL_MIN_BLOCKS, nullable, &v.map, vec, true);
+                TG_TRY(jit_get_function(ctx, src, "tg_agg_global_jit", &v.fn));
+                v.ctas_per_sm = jit_blocks_per_sm(v.fn, S_THREADS, 0);
+                it = jit_global_variants.emplace(vkey, v).first;
+            }
+            jit_fn = it->second.fn;
+            map = it->second.map;
+            grid = (int)std::min<int64_t>(tg_div_up(n, (int64_t)S_THREADS * R), (int64_t)ctx->sm_count * it->second.ctas_per_sm);
+        }
+        else {
+            map.compact_count = plan.num_accs;
+            for (int a = 0; a < MAX_ACCS; a++) map.of_plan[a] = a;
+            grid = tg_grid(ctx, n, S_THREADS * R, GLOBAL_MIN_BLOCKS);
+        }
+        grid = std::max(grid, 1);
+        const size_t need = (size_t)grid * std::max(map.compact_count, 1) * 8;
+        if (gl_part.bytes < need) TG_TRY(gl_part.alloc(ctx, need));
+        int* d_flags = ctx->d_scratch->agg_small_flags;          // [1]: error bits
+        unsigned int* d_err = (unsigned int*)d_flags + 1;
+        TG_CUDA(ctx, cudaMemsetAsync(d_flags, 0, 8, ctx->stream));
+        unsigned long long* part = gl_part.as<unsigned long long>();
+        TG_TIMED_BEGIN(ctx);
+        if (jit_fn) {
+            DColumns cols_arg = cols;
+            long long n_arg = n;
+            void* params[4] = {&cols_arg, &n_arg, &part, &d_err};
+            TG_TRY(jit_launch(ctx, jit_fn, grid, S_THREADS, 0, params));
+        }
+        else TG_LAUNCH(ctx, agg_global_kernel, grid, S_THREADS, 0, plan, cols, has_pre ? d_prog.as<DProgram>() : nullptr, n, part, d_err);
+        TG_TIMED_END(ctx);
+        TG_LAUNCH(ctx, agg_global_fold_kernel, 1, 256, 0, plan, part, grid, map.compact_count, map, state());
+        int64_t word = 0;
+        TG_TRY(tg_read_i64(ctx, d_flags, &word));
+        return raise((uint32_t)(word >> 32));
+    }
+
     // ---- Operator protocol --------------------------------------------------------------------------
     bool needs_input() override { return !finishing && !flushing && next_out >= pending.size(); }
 
@@ -2622,6 +2869,7 @@ struct AggOp : tgpu_op {
     int add_input(const tgpu_page* page) override
     {
         if (page->num_rows == 0) return TGPU_OK;
+        if (global) return add_input_global(page);
         if (!builder_open) {
             // HashAggregationOperator.addInput :358-372: the controller is consulted when a builder is created
             builder_open = true;
@@ -2892,6 +3140,7 @@ struct AggOp : tgpu_op {
         int64_t A = plan.num_accs > 0 ? plan.num_accs : 1;
         int64_t b = group_count * (8 + 8 * A + 9 * (int64_t)plan.num_keys);
         if (use_general) b += (int64_t)g_table.bytes + (int64_t)f_recs.bytes;
+        if (global) b += (int64_t)gl_part.bytes;
         for (auto& d : key_dicts)
             if (d) b += d->memory_bytes();
         return planned ? b : 0;
@@ -3239,6 +3488,27 @@ extern "C" int tgpu_agg_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op
     return TGPU_OK;
 }
 
+// AggregationOperator (M/operator/AggregationOperator.java:35-176): the keyed operator's planning, accumulators and output over ONE group
+extern "C" int tgpu_aggregation_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op** out)
+{
+    if (!ctx || !spec || !out) return TGPU_ERR_INVALID_ARGUMENT;
+    if (spec->num_keys != 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator has no group-by keys (num_keys = %d)", spec->num_keys);
+    if (spec->max_partial_bytes != 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator never flushes: max_partial_bytes must be 0");
+    if (spec->num_global_group_ids != 0 || spec->global_group_ids || spec->group_id_key >= 0)
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator has no grouping sets: num_global_group_ids 0, global_group_ids NULL, group_id_key -1");
+    if (spec->partial_aggregation_controller) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator takes no partial aggregation controller");
+    if (spec->num_input_channels < 0 || (spec->num_input_channels > 0 && !spec->input_channel_types))
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator needs input_channel_types: they shape the output row when no page arrives");
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    AggOp* raw = nullptr;
+    TG_TRY(build_agg_op(ctx, spec, &raw));
+    std::unique_ptr<AggOp> op(raw);
+    op->global = true;
+    TG_TRY(op->start_global());
+    *out = op.release();
+    return TGPU_OK;
+}
+
 extern "C" int tgpu_partial_agg_controller_create(int64_t max_partial_memory_bytes, double unique_rows_ratio_threshold, tgpu_partial_agg_controller** out)
 {
     if (!out || max_partial_memory_bytes < 0) return TGPU_ERR_INVALID_ARGUMENT;
@@ -3339,8 +3609,8 @@ extern "C" int tgpu_groupby_hash_get_group_ids(tgpu_op* op, const tgpu_page* pag
     return TGPU_OK;
 }
 
-// test hook (no GPU needed): generate + NVRTC-compile the specialised small-group kernel for a spec whose input
-// channels have the given tgpu_types; returns the cubin size in *cubin_bytes and the generated source length
+// test hook (no GPU needed): generate + NVRTC-compile the specialised small-group kernel (num_keys == 0: the global kernel) for a spec
+// whose input channels have the given tgpu_types; returns the cubin size in *cubin_bytes and the generated source length
 extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* channel_types, int32_t num_channels, uint32_t nullable_mask, int64_t* cubin_bytes, char* source_out, int64_t source_cap)
 {
     if (!spec || !channel_types || !cubin_bytes) return TGPU_ERR_INVALID_ARGUMENT;
@@ -3352,6 +3622,7 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
         o->key_channels.assign(spec->key_channels, spec->key_channels + spec->num_keys);
         o->fns.assign(spec->aggs, spec->aggs + spec->num_aggs);
         o->step = spec->step;
+        o->global = spec->num_keys == 0;        // tgpu_aggregation_create's operator: the one-group kernel
         if (spec->pre) {
             o->has_pre = true;
             int st = tg::expr_compile(&fake, spec->pre, &o->host_prog, &o->prog_max_channel);
@@ -3379,8 +3650,8 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
     if (st != TGPU_OK) return st;
     AccMap map;
     // (TGPU_JIT_SELFTEST_VEC: the variant with the four-consecutive-rows loader, as launched for 16-byte aligned columns)
-    std::string src = gen_agg_small_source(op->plan, op->has_pre ? &op->host_prog : nullptr, elems, num_channels, 4, 2, nullable_mask, &map,
-                                           getenv("TGPU_JIT_SELFTEST_VEC") != nullptr);
+    std::string src = gen_agg_small_source(op->plan, op->has_pre ? &op->host_prog : nullptr, elems, num_channels, 4, op->global ? GLOBAL_MIN_BLOCKS : 2,
+                                           nullable_mask, &map, getenv("TGPU_JIT_SELFTEST_VEC") != nullptr, op->global);
     if (source_out && source_cap > 0) { strncpy(source_out, src.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
     std::string cubin;
     st = tg::jit_compile_cubin(&fake, src, &cubin);

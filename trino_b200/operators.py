@@ -7,6 +7,7 @@ java/ (see INTEGRATION.md) and keep the reference's names, argument meaning and 
   Operator            M/operator/Operator.java:21-102  (needsInput/addInput/getOutput/finish/isFinished/close)
   OperatorFactory     M/operator/OperatorFactory.java:16-30 (createOperator/noMoreOperators/duplicate)
   HashAggregationOperatorFactory   M/operator/HashAggregationOperator.java:63-200
+  AggregationOperatorFactory       M/operator/AggregationOperator.java:35-176 (no GROUP BY keys: one output row)
   HashBuilderOperatorFactory       M/operator/join/unspilled/HashBuilderOperator.java:55-140
   LookupJoinOperatorFactory        M/operator/join/unspilled/LookupJoinOperatorFactory.java
   FilterAndProjectOperatorFactory  M/operator/FilterAndProjectOperator.java:97-150
@@ -452,7 +453,8 @@ class Aggregator:
         self.function, self.input_channel, self.mask_channel, self.result_type = function, input_channel, mask_channel, result_type
 
 
-class HashAggregationOperator(Operator):
+class _StateOperator(Operator):
+    """An aggregation operator whose intermediate states may be ROW-typed / VARBINARY on the Java side"""
     # ROW-typed intermediate states (AccumulatorCompiler.java:687-760): set by the factory when the neighbouring stage is a Java
     # operator that speaks the reference's state types.  in_first: flat channel of each original input channel; out_widths: see
     # page.compose_row_blocks
@@ -470,6 +472,8 @@ class HashAggregationOperator(Operator):
             out = compose_state_blocks(out, self._out_widths)
         return out
 
+
+class HashAggregationOperator(_StateOperator):
     def group_count(self):
         v = C.c_int64()
         self.ctx.check(self.ctx.lib.tgpu_agg_group_count(self.h, C.byref(v)))
@@ -511,6 +515,34 @@ class PartialAggregationController:
             self.h = None
 
 
+_FLAT_STATE = {abi.AGG_AVG: 2, abi.AGG_SUM_DECIMAL: 2, abi.AGG_AVG_DECIMAL: 3}           # flat state columns per function (default 1)
+_DECIMAL_STATE = {abi.AGG_SUM_DECIMAL: "decimal_sum", abi.AGG_AVG_DECIMAL: "decimal_avg"}
+
+
+def _state_widths(aggregators):
+    """the reference's state type per aggregate: ROW(BIGINT, DOUBLE) for avg (2 flat columns), VARBINARY for the decimal states"""
+    return [_DECIMAL_STATE.get(a.function, _FLAT_STATE.get(a.function, 1)) for a in aggregators]
+
+
+def _flat_channels(aggregators, channels):
+    """channels numbered as the Java plan numbers them (one channel per ROW state) -> the flattened page's channels the library sees"""
+    wide = {a.input_channel: _FLAT_STATE[a.function] for a in aggregators if a.function in _FLAT_STATE}
+    top = max(list(channels) + [0])
+    first, at = [], 0
+    for c in range(top + 1):
+        first.append(at)
+        at += wide.get(c, 1)
+    return [first[c] if c >= 0 else c for c in channels]
+
+
+def _agg_fns(aggregators, inputs):
+    fns = (abi.AggFn * max(1, len(aggregators)))()
+    for i, a in enumerate(aggregators):
+        fns[i].function, fns[i].input_channel, fns[i].mask_channel = a.function, inputs[i], a.mask_channel
+        fns[i].reserved = getattr(a, "result_type", 0)
+    return fns
+
+
 class HashAggregationOperatorFactory(OperatorFactory):
     def __init__(self, ctx, group_by_channels, step, aggregators, expected_groups=10_000, max_partial_memory=0, pre=None,
                  global_aggregation_group_ids=(), group_id_channel=None, input_types=None, partial_aggregation_controller=None,
@@ -524,32 +556,16 @@ class HashAggregationOperatorFactory(OperatorFactory):
         self.controller = partial_aggregation_controller
         self.row_typed_states = row_typed_states
 
-    _FLAT = {abi.AGG_AVG: 2, abi.AGG_SUM_DECIMAL: 2, abi.AGG_AVG_DECIMAL: 3}           # flat state columns per function (default 1)
-    _DECIMAL = {abi.AGG_SUM_DECIMAL: "decimal_sum", abi.AGG_AVG_DECIMAL: "decimal_avg"}
-
-    def _state_widths(self):
-        """the reference's state type per aggregate: ROW(BIGINT, DOUBLE) for avg (2 flat columns), VARBINARY for the decimal states"""
-        return [self._DECIMAL.get(a.function, self._FLAT.get(a.function, 1)) for a in self.aggregators]
-
     def _create(self):
         from_state = self.step in (abi.STEP_FINAL, abi.STEP_INTERMEDIATE)
         to_state = self.step in (abi.STEP_PARTIAL, abi.STEP_INTERMEDIATE)
         keys_list, agg_inputs = list(self.group_by_channels), [a.input_channel for a in self.aggregators]
         if self.row_typed_states and from_state:
             # channels are numbered as the Java plan numbers them (one channel per ROW state); the library sees the flattened page
-            wide = {a.input_channel: self._FLAT[a.function] for a in self.aggregators if a.function in self._FLAT}
-            top = max(keys_list + agg_inputs + [0])
-            first, at = [], 0
-            for c in range(top + 1):
-                first.append(at)
-                at += wide.get(c, 1)
-            keys_list = [first[c] for c in keys_list]
-            agg_inputs = [first[c] if c >= 0 else c for c in agg_inputs]
+            flat = _flat_channels(self.aggregators, keys_list + agg_inputs)
+            keys_list, agg_inputs = flat[:len(keys_list)], flat[len(keys_list):]
         keys = _i32(keys_list)
-        fns = (abi.AggFn * max(1, len(self.aggregators)))()
-        for i, a in enumerate(self.aggregators):
-            fns[i].function, fns[i].input_channel, fns[i].mask_channel = a.function, agg_inputs[i], a.mask_channel
-            fns[i].reserved = getattr(a, "result_type", 0)
+        fns = _agg_fns(self.aggregators, agg_inputs)
         gids = _i32(self.global_ids)
         types = _i32(list(self.input_types or []))
         spec = abi.AggSpec(len(self.group_by_channels), C.cast(keys, C.POINTER(C.c_int32)), self.step, len(self.aggregators),
@@ -563,9 +579,9 @@ class HashAggregationOperatorFactory(OperatorFactory):
         self.ctx.check(self.ctx.lib.tgpu_agg_create(self.ctx.h, C.byref(spec), C.byref(h)))
         op = HashAggregationOperator(self.ctx, h)
         if self.row_typed_states and to_state:
-            op._out_widths = [1] * len(self.group_by_channels) + self._state_widths()
+            op._out_widths = [1] * len(self.group_by_channels) + _state_widths(self.aggregators)
         if self.row_typed_states and from_state:
-            op._in_decimal = {a.input_channel: self._DECIMAL[a.function] for a in self.aggregators if a.function in self._DECIMAL}
+            op._in_decimal = {a.input_channel: _DECIMAL_STATE[a.function] for a in self.aggregators if a.function in _DECIMAL_STATE}
         return op
 
     def duplicate(self):
@@ -573,6 +589,46 @@ class HashAggregationOperatorFactory(OperatorFactory):
                                               self.max_partial_memory, self.pre, self.global_ids, self.group_id_channel, self.input_types,
                                               # HashAggregationOperatorFactory.duplicate :238: a fresh controller for the duplicated plan node
                                               self.controller.duplicate() if self.controller is not None else None, self.row_typed_states)
+
+
+class AggregationOperator(_StateOperator):
+    """M/operator/AggregationOperator.java:35-176: needs input until finish(), then exactly one page of one row"""
+
+
+class AggregationOperatorFactory(OperatorFactory):
+    """AggregationOperatorFactory (M/operator/AggregationOperator.java:43-88), the operator of aggregations without GROUP BY keys.
+    input_types: tgpu_type of every input channel of the pages the library sees (for a FINAL step over ROW-typed states: of the
+    flattened state columns); required, they shape the output row when no page arrives.  pre: a fused PageProcessorProgram (raw steps)."""
+
+    def __init__(self, ctx, step, aggregators, pre=None, input_types=None, row_typed_states=False):
+        super().__init__()
+        if input_types is None:
+            raise ValueError("AggregationOperatorFactory needs input_types")
+        self.ctx, self.step, self.aggregators, self.pre = ctx, step, list(aggregators), pre
+        self.input_types, self.row_typed_states = list(input_types), row_typed_states
+
+    def _create(self):
+        from_state = self.step in (abi.STEP_FINAL, abi.STEP_INTERMEDIATE)
+        to_state = self.step in (abi.STEP_PARTIAL, abi.STEP_INTERMEDIATE)
+        agg_inputs = [a.input_channel for a in self.aggregators]
+        if self.row_typed_states and from_state:
+            agg_inputs = _flat_channels(self.aggregators, agg_inputs)
+        fns = _agg_fns(self.aggregators, agg_inputs)
+        types = _i32(self.input_types)
+        spec = abi.AggSpec(0, None, self.step, len(self.aggregators), C.cast(fns, C.POINTER(abi.AggFn)), 1, 0,
+                           C.pointer(self.pre.struct) if self.pre is not None else None, 0, None, -1,
+                           len(self.input_types), C.cast(types, C.POINTER(C.c_int32)), None)
+        h = C.c_void_p()
+        self.ctx.check(self.ctx.lib.tgpu_aggregation_create(self.ctx.h, C.byref(spec), C.byref(h)))
+        op = AggregationOperator(self.ctx, h)
+        if self.row_typed_states and to_state:
+            op._out_widths = _state_widths(self.aggregators)
+        if self.row_typed_states and from_state:
+            op._in_decimal = {a.input_channel: _DECIMAL_STATE[a.function] for a in self.aggregators if a.function in _DECIMAL_STATE}
+        return op
+
+    def duplicate(self):
+        return AggregationOperatorFactory(self.ctx, self.step, self.aggregators, self.pre, self.input_types, self.row_typed_states)
 
 
 class GroupByHash:
