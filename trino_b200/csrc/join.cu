@@ -453,10 +453,10 @@ __device__ __forceinline__ unsigned int lean_next(unsigned int pos, unsigned int
 
 // persistent-tile kernels: exactly as many CTAs as are co-resident, so that no partial second wave runs at low occupancy
 template <class K>
-static int lean_grid(tgpu_ctx* ctx, K kernel, int64_t tiles)
+static int lean_grid(tgpu_ctx* ctx, K kernel, int64_t tiles, int threads = 256, size_t smem = 0)
 {
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0) != cudaSuccess || per_sm < 1) per_sm = 4;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 4;
     return (int)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * per_sm);
 }
 
@@ -575,6 +575,10 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned int 
         "}\n" ::"r"(smem_u32(bar)),
         "r"(parity)
         : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(unsigned long long* bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
 template <bool GATHER>
@@ -946,12 +950,173 @@ static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
     }
 }
 
-// Key-ordered shape of the probe over a keyed table (runs when layout_choice is 0): 8 CTAs per SM and plain read-only loads like the lean
+// ---- pipelined key-ordered probe over the keyed table (mode 2) -------------------------------------------------------------------------
+// A key-ordered page moves only the bytes it must: its keys in, the payload out, every table line once.  The thread-per-row kernel
+// (join_probe_wide_kernel<2,2,8,0,KeyedSlot>) reaches 0.88 of a device copy's bandwidth on these bytes, and more rows per thread do not
+// change that (2048 to 5120 rows in flight per SM: the same time from 3072 on).  What does is taking the reads off the threads: bulk copies
+// of whole tiles are long sequential DRAM requests, where each thread otherwise loads its keys, waits, loads the dependent slots and waits
+// again before it stores.  One producer warp per CTA bulk-copies (cp.async.bulk, completion on an mbarrier) the keys of the CTA's tiles
+// into a ring of KP_STAGES shared-memory buffers.  As soon as the keys of a tile have landed it computes the span of order-preserving
+// table lines they fall in (a key-ordered tile touches one short run of lines: about 33 for lineitem against orders) and copies that
+// span, plus the line behind it for walks that overflow their home line, into one of two line buffers.  Meanwhile 8 consumer warps
+// resolve the tile before it from shared memory and store payload and match bits, so the line copy of tile i + 1 overlaps the work on
+// tile i.  Staging the lines as well as the keys is worth it: the same ring with slots loaded per row was about 1 % slower.  A tile whose span
+// exceeds SPAN_LINES lines (keys far outside the build range, a page that is not key-ordered after all) reads its slots from global
+// memory, and so does a line walk that leaves the staged span.  Rows per thread and the order of tiles over the CTAs are those of the
+// other probe kernels: payload stores and match words are coalesced the same way, and neighbouring tiles run at the same time, so a
+// line two tiles share is usually an L2 hit.
+constexpr int KP_THREADS = 288;          // 8 consumer warps (rows threadIdx.x + j * 256, as in the other kernels) + 1 producer warp
+constexpr int KP_STAGES = 2;             // key tiles in the ring (2, 3 and 4 measured: 2 is as fast and needs the least shared memory)
+constexpr int KP_CTAS = 4;               // CTAs per SM: 4 x 288 threads, <= 56 registers (5 CTAs at <= 40 registers is slower)
+
+struct KeyedPipeSmem {
+    long long keys[KP_STAGES][1024];
+    KeyedSlot lines[2][SPAN_LINES * 8];
+    unsigned long long key_full[KP_STAGES], key_empty[KP_STAGES], line_full[2], line_empty[2];
+    unsigned int first_line[2], staged_lines[2];      // staged_lines 0: the tile's slots are read from global memory
+};
+
+__global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_kernel(const long long* __restrict__ keys, int64_t tiles, const KeyedSlot* __restrict__ keyed,
+                                                                              unsigned int mask, unsigned long long kmin, int shift, int special_head,
+                                                                              unsigned int* __restrict__ match_bits, GatherCols g, unsigned long long* __restrict__ match_count,
+                                                                              const int* __restrict__ layout_choice)
+{
+    if (layout_choice && *layout_choice != 0) return;
+    extern __shared__ __align__(128) unsigned char kp_smem[];
+    KeyedPipeSmem& sm = *reinterpret_cast<KeyedPipeSmem*>(kp_smem);
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < KP_STAGES; s++) {
+            mbar_init(&sm.key_full[s], 1);
+            mbar_init(&sm.key_empty[s], 8);            // one arrival per consumer warp
+        }
+        for (int b = 0; b < 2; b++) {
+            mbar_init(&sm.line_full[b], 1);
+            mbar_init(&sm.line_empty[b], 8);
+        }
+    }
+    __syncthreads();
+    const int64_t my_tiles = (tiles - 1 - blockIdx.x) / gridDim.x + 1;      // the grid is at most `tiles` CTAs: each has one or more
+    if (threadIdx.x >= 256) {
+        // producer warp.  Tile i of the CTA is tile blockIdx.x + i * gridDim.x of the page; its keys go to stage i % KP_STAGES, its lines to
+        // buffer i & 1.  Key copies run up to KP_STAGES tiles ahead of the span; a stage is refilled once the consumers released it.
+        const unsigned int line_mask = mask >> 3;
+        if (lane == 0)
+            for (int64_t i = 0; i < KP_STAGES && i < my_tiles; i++) {
+                mbar_expect_tx(&sm.key_full[i], 8192u);
+                bulk_g2s(sm.keys[i], keys + (blockIdx.x + i * gridDim.x) * 1024, 8192u, &sm.key_full[i]);
+            }
+        for (int64_t i = 0; i < my_tiles; i++) {
+            const int s = (int)(i % KP_STAGES), b = (int)(i & 1);
+            mbar_wait(&sm.key_full[s], (unsigned int)(i / KP_STAGES) & 1u);
+            unsigned int lo = 0xffffffffu, hi = 0;
+#pragma unroll 8
+            for (int m = 0; m < 32; m++) {
+                const unsigned int line = lean_slot<2>((unsigned long long)sm.keys[s][m * 32 + lane], mask, kmin, shift) >> 3;
+                lo = min(lo, line);
+                hi = max(hi, line);
+            }
+            lo = __reduce_min_sync(0xffffffffu, lo);
+            hi = __reduce_max_sync(0xffffffffu, hi);
+            if (lane == 0) {
+                if (i >= 2) mbar_wait(&sm.line_empty[b], (unsigned int)((i - 2) >> 1) & 1u);     // the consumers are done with tile i - 2
+                const unsigned int lines = min(hi + 1u, line_mask) - lo + 1u;
+                sm.first_line[b] = lo;
+                sm.staged_lines[b] = lines <= (unsigned int)SPAN_LINES ? lines : 0u;
+                if (lines <= (unsigned int)SPAN_LINES) {
+                    mbar_expect_tx(&sm.line_full[b], lines * 128u);
+                    bulk_g2s(sm.lines[b], keyed + (size_t)lo * 8, lines * 128u, &sm.line_full[b]);
+                }
+                else mbar_arrive(&sm.line_full[b]);
+            }
+            // refill the stage of tile i - 1 with tile i - 1 + KP_STAGES
+            const int64_t next = i - 1 + KP_STAGES;
+            if (lane == 0 && i >= 1 && next < my_tiles) {
+                const int sn = (int)((i - 1) % KP_STAGES);
+                mbar_wait(&sm.key_empty[sn], (unsigned int)((i - 1) / KP_STAGES) & 1u);
+                mbar_expect_tx(&sm.key_full[sn], 8192u);
+                bulk_g2s(sm.keys[sn], keys + (blockIdx.x + next * gridDim.x) * 1024, 8192u, &sm.key_full[sn]);
+            }
+            __syncwarp();
+        }
+        return;
+    }
+    unsigned int matched = 0;
+    for (int64_t i = 0; i < my_tiles; i++) {
+        const int s = (int)(i % KP_STAGES), b = (int)(i & 1);
+        const int64_t base = (blockIdx.x + i * gridDim.x) * 1024 + threadIdx.x;
+        mbar_wait(&sm.key_full[s], (unsigned int)(i / KP_STAGES) & 1u);
+        mbar_wait(&sm.line_full[b], (unsigned int)(i >> 1) & 1u);
+        const unsigned int first_slot = sm.first_line[b] << 3, staged_slots = sm.staged_lines[b] << 3;
+        unsigned long long k[4];
+        unsigned int pos[4];
+        KeyedSlot w[4];
+        bool hit[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            k[j] = (unsigned long long)sm.keys[s][threadIdx.x + j * 256];
+            pos[j] = lean_slot<2>(k[j], mask, kmin, shift);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const unsigned int local = pos[j] - first_slot;
+            w[j] = local < staged_slots ? sm.lines[b][local] : wide_load<0>(keyed + pos[j]);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            unsigned int p = pos[j];
+            hit[j] = false;
+            while (true) {
+                if (w[j].key == k[j]) { hit[j] = true; break; }
+                if (w[j].key == EMPTY_KEY) break;
+                p = lean_next<2>(p, (unsigned int)k[j] & 7u, mask);
+                const unsigned int local = p - first_slot;
+                w[j] = local < staged_slots ? sm.lines[b][local] : wide_load<0>(keyed + p);
+            }
+            if (k[j] == EMPTY_KEY) {                       // INT64_MIN lives outside the table, in the slot behind the last one
+                hit[j] = special_head >= 0;
+                if (hit[j]) w[j] = wide_load<0>(keyed + (mask + 1u));
+            }
+        }
+        // the warp is done with the tile's keys and lines: hand them back to the producer before the stores
+        __syncwarp();
+        if (lane == 0) {
+            mbar_arrive(&sm.key_empty[s]);
+            mbar_arrive(&sm.line_empty[b]);
+        }
+        if (g.count > 0) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const unsigned long long v = hit[j] ? w[j].cell : 0ULL;
+                switch (g.elem[0]) {
+                    case 8: ((unsigned long long*)g.dst[0])[base + j * 256] = v; break;
+                    case 4: ((unsigned int*)g.dst[0])[base + j * 256] = (unsigned int)v; break;
+                    case 2: ((unsigned short*)g.dst[0])[base + j * 256] = (unsigned short)v; break;
+                    default: ((unsigned char*)g.dst[0])[base + j * 256] = (unsigned char)v; break;
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) store_match_word(match_bits, base + j * 256, hit[j], &matched);
+    }
+    add_match_count(match_count, matched);
+}
+
+// Key-ordered shape of the probe over a keyed table (runs when layout_choice is 0): the pipelined kernel above for order-preserving tables
+// and key columns whose tiles the bulk copy can read (16-byte aligned).  Otherwise 8 CTAs per SM and plain read-only loads like the lean
 // kernel, but 2 rows in flight per thread rather than 4: four keyed rows do not fit the 32 registers that 8 CTAs per SM allow (ptxas spills
 // 88-144 bytes per thread), two take 28-30 registers without spilling
 static int launch_keyed_ordered(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const KeyedSlot* keyed, int special_head,
                                 unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice)
 {
+    if (geo.mode == 2 && ((uintptr_t)keys & 15) == 0) {
+        auto k = join_probe_keyed_pipe_kernel;
+        const int smem = (int)sizeof(KeyedPipeSmem);
+        TG_CUDA(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles, KP_THREADS, smem), KP_THREADS, smem, keys, tiles, keyed, (unsigned int)geo.mask, geo.kmin, geo.shift,
+                  special_head, match_bits, g, matches, layout_choice);
+        return TGPU_OK;
+    }
     return launch_wide_shape<2, 8, 0>(ctx, geo, keys, tiles, keyed, special_head, match_bits, g, matches, layout_choice, 0);
 }
 
