@@ -1,19 +1,22 @@
 """DRAM traffic of the fused join probe on the bench workload, against a device-to-device copy of the same volume.
 
-    python tools/probe_traffic.py [--sf 100] [--reps 10] [--model keyed|positions]
+    python tools/probe_traffic.py [--sf 100] [--reps 10] [--model packed4|packed8|keyed|positions]
 
 Builds the bench's lineitem JOIN orders (BIGINT key, one 8-byte payload column, key-ordered probe page), times one
 LookupJoinOperator page with the CUDA events the library records around its kernels (tgpu_ctx_last_kernel_ms), and prints the
 bytes the probe moves per page, computed from the shapes:
 
-    keyed     : probe keys 8 B/row + 16-byte keyed slots {key, cell}, each table line read once + payload written 8 B/row
-                + the match bitmap, 1 bit/row
+    packed4   : probe keys 8 B/row + 4-byte packed slots {krel, cell}, each 32-byte table line read once + payload written
+                8 B/row + the match bitmap, 1 bit/row (what the bench's build picks)
+    packed8   : the same with 8-byte packed slots, 64 bytes per line
+    keyed     : the same with 16-byte keyed slots {key, cell}, 128 bytes per line
     positions : probe keys 8 B/row + 16-byte slots {key, head, pad}, each line read once + slot-ordered payload, 64 B per line
                 + payload written 8 B/row + the int32 join position of every row, 4 B/row
 
 The table lines a key-ordered page reads are those of the order-preserving layout between the smallest and the largest build
 key.  A torch copy_ of (reads + writes) / 2 bytes moves the same volume; the kernel's effective GB/s is reported against the
-copy's measured GB/s, not against a data-sheet figure.  Prints one JSON line.
+copy's measured GB/s, not against a data-sheet figure.  Also prints the lookup's device memory (tgpu_lookup_memory_bytes), which
+shows the slot width the build picked.  Prints one JSON line.
 """
 import argparse
 import ctypes as C
@@ -28,6 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 SEED_LINEITEM, SEED_ORDERS = 0x7C01, 0x7C02      # bench.py's generator seeds
+LINE_BYTES = {"packed4": 32, "packed8": 64, "keyed": 128}      # a table line of 8 slots
 
 
 def table_geometry(rows, kmin, kmax):
@@ -57,8 +61,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sf", type=float, default=100.0)
     ap.add_argument("--reps", type=int, default=10)
-    ap.add_argument("--model", default="keyed", choices=["keyed", "positions"],
-                    help="byte model: the keyed table + match bitmap, or 16-byte slots + slot-ordered payload + int32 positions")
+    ap.add_argument("--model", default="packed4", choices=list(LINE_BYTES) + ["positions"],
+                    help="byte model: the keyed table in 4-, 8- or 16-byte slots + match bitmap, or 16-byte slots + slot-ordered payload + int32 positions")
     args = ap.parse_args()
 
     import torch
@@ -87,6 +91,7 @@ def main():
     builder = ops.HashBuilderOperatorFactory(ctx, bridge, [0], [1], n_orders).create_operator()
     builder.add_input(ops.DevicePage([ops.DeviceColumn(abi.INT64, d_okeys, n_orders), date.column(0)], n_orders))
     builder.finish()
+    lookup_bytes = bridge.lookup_source.get_in_memory_size_in_bytes()
     probe_op = ops.LookupJoinOperatorFactory(ctx, bridge, abi.JOIN_INNER, False, [0], [0, 1]).create_operator()
     probe = ops.DevicePage([ops.DeviceColumn(abi.INT64, d_lkeys, n), price.column(0)], n)
 
@@ -106,8 +111,8 @@ def main():
     cap, shift = table_geometry(n_orders, kmin, kmax)
     lines = ((kmax - kmin) >> shift) + 1
     streams = {"probe_keys": 8 * n}
-    if args.model == "keyed":
-        streams["keyed_slots"] = 128 * lines
+    if args.model in LINE_BYTES:
+        streams["keyed_slots"] = LINE_BYTES[args.model] * lines
         streams["payload_written"] = 8 * n
         streams["match_bitmap"] = (n + 31) // 32 * 4
         reads = streams["probe_keys"] + streams["keyed_slots"]
@@ -138,7 +143,8 @@ def main():
     copy_gbs = 2 * half * 8 / (copy_ms * 1e-3) / 1e9
     kernel_gbs = total / (kernel_ms * 1e-3) / 1e9
     print(json.dumps({"tool": "probe_traffic", "gpu": gpu_info(), "model": args.model, "sf": args.sf, "probe_rows": n, "build_rows": n_orders,
-                      "table_capacity": cap, "table_lines_read": lines, "bytes": streams, "bytes_total": total, "bytes_read": reads,
+                      "table_capacity": cap, "table_lines_read": lines,
+                      "lookup_memory_bytes": lookup_bytes, "bytes": streams, "bytes_total": total, "bytes_read": reads,
                       "bytes_written": writes, "kernel_ms_min": kernel_ms, "kernel_ms_all": kms, "kernel_gb_per_s": kernel_gbs,
                       "copy_ms_min": copy_ms, "copy_gb_per_s": copy_gbs, "kernel_over_copy": kernel_gbs / copy_gbs,
                       "rows_per_s": n / (kernel_ms * 1e-3)}))

@@ -727,6 +727,7 @@ static int launch_lean(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys
 // Built next to the 16-byte table (which the index-only probe, the duplicate chains and every generic kernel keep using).
 struct __align__(32) WideSlot {
     static constexpr int CELLS = 2;
+    static constexpr bool LINE_RELATIVE = false;
     unsigned long long key;
     int head;
     int pad;
@@ -741,14 +742,42 @@ struct __align__(32) WideSlot {
 // was inserted, so its head is >= 0); the special key INT64_MIN keeps its cell in slot mask + 1, as in the wide table.
 struct __align__(16) KeyedSlot {
     static constexpr int CELLS = 1;
+    static constexpr bool LINE_RELATIVE = false;
     unsigned long long key;
     unsigned long long cell;
+};
+
+// ---- packed keyed slots: the keyed slot in 4 or 8 bytes, for order-preserving tables (mode 2) ---------------------------------------------
+// Under mode 2 a key in line L is kmin + (L << shift) + r, with r in [0, 2^shift) in its home line and a small negative r after it was
+// displaced to a later line: the slot stores krel = key - kmin - ((slot >> 3) << shift).  The payload cell is stored relative to the smallest
+// cell of the table, cmin (the cells sign-extended from their width; a DOUBLE by its bits).  The build picks the narrowest of the two that
+// holds every occupied slot's krel and cell, else it keeps the 16-byte keyed slot.  Empty is krel = INT16_MIN / INT32_MIN, which no stored
+// key uses.  The probe compares the full 64-bit rel = k - kmin - ((pos >> 3) << shift) of an OCCUPIED slot with its sign-extended krel: for a
+// fixed slot rel is a bijection of the key (mod 2^64), so only the stored key matches, also against a key that reaches the same slot through
+// the wrap of the slot mask.  An empty slot is excluded explicitly (slot_matches): a probe key whose rel equals the empty marker exists
+// whenever the lines cover few enough key values.  The payload is cmin + cell (mod 2^64), truncated to the column's width by the store.
+struct __align__(4) PackedSlot4 {
+    static constexpr int CELLS = 1;
+    static constexpr bool LINE_RELATIVE = true;
+    static constexpr long long KREL_MIN = INT16_MIN, KREL_MAX = INT16_MAX;
+    static constexpr unsigned long long CELL_MAX = 0xFFFFULL;
+    short krel;
+    unsigned short cell;
+};
+
+struct __align__(8) PackedSlot8 {
+    static constexpr int CELLS = 1;
+    static constexpr bool LINE_RELATIVE = true;
+    static constexpr long long KREL_MIN = INT32_MIN, KREL_MAX = INT32_MAX;
+    static constexpr unsigned long long CELL_MAX = 0xFFFFFFFFULL;
+    int krel;
+    unsigned int cell;
 };
 
 // sm_90 has no 256-bit load: a wide slot is read as the two 128-bit halves of its 32-byte sector, which costs one DRAM sector all the same.
 // LD: 0 = plain read-only loads; 3 = the same with an explicit 64-byte L2 fetch size
 template <int LD>
-__device__ __forceinline__ WideSlot wide_load(const WideSlot* p)
+__device__ __forceinline__ WideSlot slot_load(const WideSlot* p)
 {
     WideSlot w;
     unsigned long long kh;
@@ -766,7 +795,7 @@ __device__ __forceinline__ WideSlot wide_load(const WideSlot* p)
 }
 
 template <int LD>
-__device__ __forceinline__ KeyedSlot wide_load(const KeyedSlot* p)
+__device__ __forceinline__ KeyedSlot slot_load(const KeyedSlot* p)
 {
     KeyedSlot w;
     if (LD == 3) asm("ld.global.nc.L2::64B.v2.u64 {%0,%1}, [%2];" : "=l"(w.key), "=l"(w.cell) : "l"(p));
@@ -774,11 +803,54 @@ __device__ __forceinline__ KeyedSlot wide_load(const KeyedSlot* p)
     return w;
 }
 
+template <int LD>
+__device__ __forceinline__ PackedSlot8 slot_load(const PackedSlot8* p)
+{
+    PackedSlot8 w;
+    if (LD == 3) asm("ld.global.nc.L2::64B.v2.u32 {%0,%1}, [%2];" : "=r"(w.krel), "=r"(w.cell) : "l"(p));
+    else asm("ld.global.nc.v2.u32 {%0,%1}, [%2];" : "=r"(w.krel), "=r"(w.cell) : "l"(p));
+    return w;
+}
+
+template <int LD>
+__device__ __forceinline__ PackedSlot4 slot_load(const PackedSlot4* p)
+{
+    unsigned int v;
+    if (LD == 3) asm("ld.global.nc.L2::64B.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    else asm("ld.global.nc.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    PackedSlot4 w;
+    w.krel = (short)(v & 0xFFFFu);
+    w.cell = (unsigned short)(v >> 16);
+    return w;
+}
+
+__device__ __forceinline__ bool slot_empty(const WideSlot& w) { return w.key == EMPTY_KEY; }
+__device__ __forceinline__ bool slot_empty(const KeyedSlot& w) { return w.key == EMPTY_KEY; }
+__device__ __forceinline__ bool slot_empty(const PackedSlot4& w) { return w.krel == INT16_MIN; }
+__device__ __forceinline__ bool slot_empty(const PackedSlot8& w) { return w.krel == INT32_MIN; }
+
+// does the slot at pos hold key k (kmin, shift: the mode 2 geometry; only line-relative slots need them)
+__device__ __forceinline__ bool slot_matches(const WideSlot& w, unsigned long long k, unsigned int, unsigned long long, int) { return w.key == k; }
+__device__ __forceinline__ bool slot_matches(const KeyedSlot& w, unsigned long long k, unsigned int, unsigned long long, int) { return w.key == k; }
+// An empty packed slot never matches: its krel (INT16_MIN / INT32_MIN) is not a stored key's, but a probe key can have exactly that rel
+// (e.g. k = kmin - 2^15 + (L << shift) in line L when the lines cover at most 2^15 key values)
+template <class S>
+__device__ __forceinline__ bool slot_matches(const S& w, unsigned long long k, unsigned int pos, unsigned long long kmin, int shift)
+{
+    const unsigned long long rel = k - kmin - ((unsigned long long)(pos >> 3) << shift);
+    return (long long)rel == (long long)w.krel && !slot_empty(w);
+}
+
 // head row of a slot whose key matched (a keyed slot has none: any non-negative value stands for "matched")
 __device__ __forceinline__ int slot_head(const WideSlot& w) { return w.head; }
-__device__ __forceinline__ int slot_head(const KeyedSlot&) { return 0; }
-__device__ __forceinline__ unsigned long long slot_cell(const WideSlot& w, int c) { return w.cell[c]; }
-__device__ __forceinline__ unsigned long long slot_cell(const KeyedSlot& w, int) { return w.cell; }
+template <class S>
+__device__ __forceinline__ int slot_head(const S&) { return 0; }
+
+// payload cell c of a matched slot (cmin: the packed slots' cell offset)
+__device__ __forceinline__ unsigned long long slot_value(const WideSlot& w, int c, unsigned long long) { return w.cell[c]; }
+__device__ __forceinline__ unsigned long long slot_value(const KeyedSlot& w, int, unsigned long long) { return w.cell; }
+template <class S>
+__device__ __forceinline__ unsigned long long slot_value(const S& w, int, unsigned long long cmin) { return cmin + (unsigned long long)w.cell; }
 
 __device__ __forceinline__ void put_slot(WideSlot* s, unsigned long long key, int head, unsigned long long c0, unsigned long long c1)
 {
@@ -822,14 +894,80 @@ __global__ void join_wide_table_kernel(const JoinSlot* __restrict__ table, int64
     }
 }
 
+// a payload cell as a signed 64-bit value: sign-extended from its width, so that small negative integers stay a small range
+__device__ __forceinline__ long long cell_sext(const void* src, int elem, int row)
+{
+    switch (elem) {
+        case 8: return ((const long long*)src)[row];
+        case 4: return ((const int*)src)[row];
+        case 2: return ((const short*)src)[row];
+        default: return ((const signed char*)src)[row];
+    }
+}
+
+// which packed slot holds the keyed table of a mode 2 build: min / max of krel over the occupied slots, and of the cell over the occupied
+// slots and INT64_MIN's (special_head >= 0).  range: {krel min, krel max, cell min, cell max}, initialised to empty ranges
+__global__ void join_packed_range_kernel(const JoinSlot* __restrict__ table, int64_t slots, unsigned long long kmin, int shift, int special_head,
+                                         const void* __restrict__ src, int elem, long long* __restrict__ range)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    long long klo = INT64_MAX, khi = INT64_MIN, clo = INT64_MAX, chi = INT64_MIN;
+    for (; i <= slots; i += stride) {
+        int head = special_head;
+        if (i < slots) {
+            const unsigned long long key = table[i].key;
+            if (key == EMPTY_KEY) continue;
+            const long long krel = (long long)(key - kmin - ((unsigned long long)(i >> 3) << shift));
+            klo = min(klo, krel);
+            khi = max(khi, krel);
+            head = table[i].head;
+        }
+        if (head < 0) continue;
+        const long long c = cell_sext(src, elem, head);
+        clo = min(clo, c);
+        chi = max(chi, c);
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        klo = min(klo, (long long)__shfl_xor_sync(0xffffffffu, klo, off));
+        khi = max(khi, (long long)__shfl_xor_sync(0xffffffffu, khi, off));
+        clo = min(clo, (long long)__shfl_xor_sync(0xffffffffu, clo, off));
+        chi = max(chi, (long long)__shfl_xor_sync(0xffffffffu, chi, off));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (klo <= khi) { atomicMin(range, klo); atomicMax(range + 1, khi); }
+        if (clo <= chi) { atomicMin(range + 2, clo); atomicMax(range + 3, chi); }
+    }
+}
+
+// the packed table: slot i < slots from the 16-byte table, slot `slots` holds INT64_MIN's cell (as join_wide_table_kernel)
+template <class S>
+__global__ void join_packed_table_kernel(const JoinSlot* __restrict__ table, int64_t slots, unsigned long long kmin, int shift, int special_head,
+                                         const void* __restrict__ src, int elem, unsigned long long cmin, S* __restrict__ packed)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i <= slots; i += stride) {
+        const unsigned long long key = i < slots ? table[i].key : EMPTY_KEY;
+        const int head = i < slots ? table[i].head : special_head;
+        S w;
+        w.krel = key == EMPTY_KEY ? (decltype(w.krel))S::KREL_MIN : (decltype(w.krel))(long long)(key - kmin - ((unsigned long long)(i >> 3) << shift));
+        w.cell = head >= 0 ? (decltype(w.cell))((unsigned long long)cell_sext(src, elem, head) - cmin) : 0;
+        packed[i] = w;
+    }
+}
+
 // same contract as join_probe_lean_kernel<MODE, true>: whole 1024-row tiles of a BIGINT key without NULLs; ROWS rows of a thread are in
-// flight together (a tile is 4 rows per thread, taken ROWS at a time).  S is the slot type of the table (WideSlot or KeyedSlot).
-// With layout_choice set the kernel runs only when join_probe_locality_kernel chose run_on for the page.
+// flight together (a tile is 4 rows per thread, taken ROWS at a time).  S is the slot type of the table (WideSlot, KeyedSlot, or under
+// MODE 2 a packed slot, whose cells are relative to cmin).  With layout_choice set the kernel runs only when join_probe_locality_kernel
+// chose run_on for the page.
 template <int MODE, int ROWS, int MINB, int LD, class S>
 __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long long* __restrict__ keys, int64_t tiles, const S* __restrict__ wide, unsigned int mask,
-                                                                  unsigned long long kmin, int shift, int special_head, unsigned int* __restrict__ match_bits, GatherCols g,
-                                                                  unsigned long long* __restrict__ match_count, const int* __restrict__ layout_choice, int run_on)
+                                                                  unsigned long long kmin, int shift, int special_head, unsigned long long cmin,
+                                                                  unsigned int* __restrict__ match_bits, GatherCols g, unsigned long long* __restrict__ match_count,
+                                                                  const int* __restrict__ layout_choice, int run_on)
 {
+    static_assert(MODE == 2 || !S::LINE_RELATIVE, "packed slots need order-preserving lines");
     if (layout_choice && *layout_choice != run_on) return;
     unsigned int matched = 0;
     for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
@@ -845,20 +983,20 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
 #pragma unroll
             for (int j = 0; j < ROWS; j++) pos[j] = lean_slot<MODE>(k[j], mask, kmin, shift);
 #pragma unroll
-            for (int j = 0; j < ROWS; j++) w[j] = wide_load<LD>(wide + pos[j]);
+            for (int j = 0; j < ROWS; j++) w[j] = slot_load<LD>(wide + pos[j]);
 #pragma unroll
             for (int j = 0; j < ROWS; j++) {
                 unsigned int p = pos[j];
                 int r = -1;
                 while (true) {
-                    if (w[j].key == k[j]) { r = slot_head(w[j]); break; }
-                    if (w[j].key == EMPTY_KEY) break;
+                    if (slot_matches(w[j], k[j], p, kmin, shift)) { r = slot_head(w[j]); break; }
+                    if (slot_empty(w[j])) break;
                     p = lean_next<MODE>(p, (unsigned int)k[j] & 7u, mask);
-                    w[j] = wide_load<LD>(wide + p);
+                    w[j] = slot_load<LD>(wide + p);
                 }
                 if (k[j] == EMPTY_KEY) {                       // INT64_MIN lives outside the table, in the slot behind the last one
                     r = special_head;
-                    if (r >= 0) w[j] = wide_load<LD>(wide + (mask + 1u));
+                    if (r >= 0) w[j] = slot_load<LD>(wide + (mask + 1u));
                 }
                 hit[j] = r >= 0;
             }
@@ -867,7 +1005,7 @@ __global__ void __launch_bounds__(256, MINB) join_probe_wide_kernel(const long l
                 if (c >= g.count) break;
 #pragma unroll
                 for (int j = 0; j < ROWS; j++) {
-                    const unsigned long long v = hit[j] ? slot_cell(w[j], c) : 0ULL;
+                    const unsigned long long v = hit[j] ? slot_value(w[j], c, cmin) : 0ULL;
                     switch (g.elem[c]) {
                         case 8: ((unsigned long long*)g.dst[c])[base + j * 256] = v; break;
                         case 4: ((unsigned int*)g.dst[c])[base + j * 256] = (unsigned int)v; break;
@@ -911,42 +1049,47 @@ static int launch_locality(tgpu_ctx* ctx, const JoinGeom& geo, const long long* 
 }
 
 template <int ROWS, int MINB, int LD = 0, class S>
-static int launch_wide_shape(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned int* match_bits,
-                             const GatherCols& g, unsigned long long* matches, const int* layout_choice, int run_on)
+static int launch_wide_shape(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned long long cmin,
+                             unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice, int run_on)
 {
     const unsigned int mask32 = (unsigned int)geo.mask;
     if (geo.mode == 2) {
         auto k = join_probe_wide_kernel<2, ROWS, MINB, LD, S>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, geo.kmin, geo.shift, special_head, match_bits, g, matches, layout_choice, run_on);
+        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, geo.kmin, geo.shift, special_head, cmin, match_bits, g, matches,
+                  layout_choice, run_on);
+        return TGPU_OK;
     }
-    else if (geo.mode == 1) {
-        auto k = join_probe_wide_kernel<1, ROWS, MINB, LD, S>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, match_bits, g, matches, layout_choice, run_on);
-    }
+    if constexpr (S::LINE_RELATIVE) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "packed join slots need order-preserving lines");
     else {
-        auto k = join_probe_wide_kernel<0, ROWS, MINB, LD, S>;
-        TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, match_bits, g, matches, layout_choice, run_on);
+        if (geo.mode == 1) {
+            auto k = join_probe_wide_kernel<1, ROWS, MINB, LD, S>;
+            TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, cmin, match_bits, g, matches, layout_choice, run_on);
+        }
+        else {
+            auto k = join_probe_wide_kernel<0, ROWS, MINB, LD, S>;
+            TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles), 256, 0, keys, tiles, wide, mask32, 0ULL, 0, special_head, cmin, match_bits, g, matches, layout_choice, run_on);
+        }
+        return TGPU_OK;
     }
-    return TGPU_OK;
 }
 
-// Random-access shape of the probe over a wide or keyed table (runs when layout_choice is null or 1).
+// Random-access shape of the probe over a wide, keyed or packed table (runs when layout_choice is null or 1).
 // rows in flight per thread x CTAs per SM; TGPU_JOIN_WIDE_SHAPE=<rows><ctas> picks one of the built shapes (sweeps)
 template <class S>
-static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned int* match_bits,
-                       const GatherCols& g, unsigned long long* matches, const int* layout_choice)
+static int launch_wide(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* wide, int special_head, unsigned long long cmin,
+                       unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice)
 {
     const char* e = getenv("TGPU_JOIN_WIDE_SHAPE");
     int shape = e ? atoi(e) : 28;
     const char* le = getenv("TGPU_JOIN_WIDE_LOAD");
     int ld = le ? atoi(le) : 3;
-    if (shape == 28 && ld == 3) return launch_wide_shape<2, 8, 3>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+    if (shape == 28 && ld == 3) return launch_wide_shape<2, 8, 3>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
     switch (shape) {
-        case 18: return launch_wide_shape<1, 8>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
-        case 26: return launch_wide_shape<2, 6>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
-        case 45: return launch_wide_shape<4, 5>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
-        case 44: return launch_wide_shape<4, 4>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
-        default: return launch_wide_shape<2, 8>(ctx, geo, keys, tiles, wide, special_head, match_bits, g, matches, layout_choice, 1);
+        case 18: return launch_wide_shape<1, 8>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
+        case 26: return launch_wide_shape<2, 6>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
+        case 45: return launch_wide_shape<4, 5>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
+        case 44: return launch_wide_shape<4, 4>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
+        default: return launch_wide_shape<2, 8>(ctx, geo, keys, tiles, wide, special_head, cmin, match_bits, g, matches, layout_choice, 1);
     }
 }
 
@@ -969,21 +1112,26 @@ constexpr int KP_THREADS = 288;          // 8 consumer warps (rows threadIdx.x +
 constexpr int KP_STAGES = 2;             // key tiles in the ring (2, 3 and 4 measured: 2 is as fast and needs the least shared memory)
 constexpr int KP_CTAS = 4;               // CTAs per SM: 4 x 288 threads, <= 56 registers (5 CTAs at <= 40 registers is slower)
 
+// S: KeyedSlot or a packed slot (a line of 128, 64 or 32 bytes: the bulk copies stay multiples of 16 bytes)
+template <class S>
 struct KeyedPipeSmem {
     long long keys[KP_STAGES][1024];
-    KeyedSlot lines[2][SPAN_LINES * 8];
+    S lines[2][SPAN_LINES * 8];
     unsigned long long key_full[KP_STAGES], key_empty[KP_STAGES], line_full[2], line_empty[2];
     unsigned int first_line[2], staged_lines[2];      // staged_lines 0: the tile's slots are read from global memory
 };
 
-__global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_kernel(const long long* __restrict__ keys, int64_t tiles, const KeyedSlot* __restrict__ keyed,
+template <class S>
+__global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_kernel(const long long* __restrict__ keys, int64_t tiles, const S* __restrict__ keyed,
                                                                               unsigned int mask, unsigned long long kmin, int shift, int special_head,
-                                                                              unsigned int* __restrict__ match_bits, GatherCols g, unsigned long long* __restrict__ match_count,
-                                                                              const int* __restrict__ layout_choice)
+                                                                              unsigned long long cmin, unsigned int* __restrict__ match_bits, GatherCols g,
+                                                                              unsigned long long* __restrict__ match_count, const int* __restrict__ layout_choice)
 {
+    constexpr unsigned int LINE_BYTES = 8 * sizeof(S);
+    static_assert(LINE_BYTES % 16 == 0, "bulk copies move multiples of 16 bytes");
     if (layout_choice && *layout_choice != 0) return;
     extern __shared__ __align__(128) unsigned char kp_smem[];
-    KeyedPipeSmem& sm = *reinterpret_cast<KeyedPipeSmem*>(kp_smem);
+    KeyedPipeSmem<S>& sm = *reinterpret_cast<KeyedPipeSmem<S>*>(kp_smem);
     const int lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         for (int s = 0; s < KP_STAGES; s++) {
@@ -1024,8 +1172,8 @@ __global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_ker
                 sm.first_line[b] = lo;
                 sm.staged_lines[b] = lines <= (unsigned int)SPAN_LINES ? lines : 0u;
                 if (lines <= (unsigned int)SPAN_LINES) {
-                    mbar_expect_tx(&sm.line_full[b], lines * 128u);
-                    bulk_g2s(sm.lines[b], keyed + (size_t)lo * 8, lines * 128u, &sm.line_full[b]);
+                    mbar_expect_tx(&sm.line_full[b], lines * LINE_BYTES);
+                    bulk_g2s(sm.lines[b], keyed + (size_t)lo * 8, lines * LINE_BYTES, &sm.line_full[b]);
                 }
                 else mbar_arrive(&sm.line_full[b]);
             }
@@ -1050,7 +1198,7 @@ __global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_ker
         const unsigned int first_slot = sm.first_line[b] << 3, staged_slots = sm.staged_lines[b] << 3;
         unsigned long long k[4];
         unsigned int pos[4];
-        KeyedSlot w[4];
+        S w[4];
         bool hit[4];
 #pragma unroll
         for (int j = 0; j < 4; j++) {
@@ -1060,22 +1208,22 @@ __global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_ker
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             const unsigned int local = pos[j] - first_slot;
-            w[j] = local < staged_slots ? sm.lines[b][local] : wide_load<0>(keyed + pos[j]);
+            w[j] = local < staged_slots ? sm.lines[b][local] : slot_load<0>(keyed + pos[j]);
         }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             unsigned int p = pos[j];
             hit[j] = false;
             while (true) {
-                if (w[j].key == k[j]) { hit[j] = true; break; }
-                if (w[j].key == EMPTY_KEY) break;
+                if (slot_matches(w[j], k[j], p, kmin, shift)) { hit[j] = true; break; }
+                if (slot_empty(w[j])) break;
                 p = lean_next<2>(p, (unsigned int)k[j] & 7u, mask);
                 const unsigned int local = p - first_slot;
-                w[j] = local < staged_slots ? sm.lines[b][local] : wide_load<0>(keyed + p);
+                w[j] = local < staged_slots ? sm.lines[b][local] : slot_load<0>(keyed + p);
             }
             if (k[j] == EMPTY_KEY) {                       // INT64_MIN lives outside the table, in the slot behind the last one
                 hit[j] = special_head >= 0;
-                if (hit[j]) w[j] = wide_load<0>(keyed + (mask + 1u));
+                if (hit[j]) w[j] = slot_load<0>(keyed + (mask + 1u));
             }
         }
         // the warp is done with the tile's keys and lines: hand them back to the producer before the stores
@@ -1087,7 +1235,7 @@ __global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_ker
         if (g.count > 0) {
 #pragma unroll
             for (int j = 0; j < 4; j++) {
-                const unsigned long long v = hit[j] ? w[j].cell : 0ULL;
+                const unsigned long long v = hit[j] ? slot_value(w[j], 0, cmin) : 0ULL;
                 switch (g.elem[0]) {
                     case 8: ((unsigned long long*)g.dst[0])[base + j * 256] = v; break;
                     case 4: ((unsigned int*)g.dst[0])[base + j * 256] = (unsigned int)v; break;
@@ -1106,18 +1254,19 @@ __global__ void __launch_bounds__(KP_THREADS, KP_CTAS) join_probe_keyed_pipe_ker
 // and key columns whose tiles the bulk copy can read (16-byte aligned).  Otherwise 8 CTAs per SM and plain read-only loads like the lean
 // kernel, but 2 rows in flight per thread rather than 4: four keyed rows do not fit the 32 registers that 8 CTAs per SM allow (ptxas spills
 // 88-144 bytes per thread), two take 28-30 registers without spilling
-static int launch_keyed_ordered(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const KeyedSlot* keyed, int special_head,
-                                unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice)
+template <class S>
+static int launch_keyed_ordered(tgpu_ctx* ctx, const JoinGeom& geo, const long long* keys, int64_t tiles, const S* keyed, int special_head,
+                                unsigned long long cmin, unsigned int* match_bits, const GatherCols& g, unsigned long long* matches, const int* layout_choice)
 {
     if (geo.mode == 2 && ((uintptr_t)keys & 15) == 0) {
-        auto k = join_probe_keyed_pipe_kernel;
-        const int smem = (int)sizeof(KeyedPipeSmem);
+        auto k = join_probe_keyed_pipe_kernel<S>;
+        const int smem = (int)sizeof(KeyedPipeSmem<S>);
         TG_CUDA(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         TG_LAUNCH(ctx, k, lean_grid(ctx, k, tiles, KP_THREADS, smem), KP_THREADS, smem, keys, tiles, keyed, (unsigned int)geo.mask, geo.kmin, geo.shift,
-                  special_head, match_bits, g, matches, layout_choice);
+                  special_head, cmin, match_bits, g, matches, layout_choice);
         return TGPU_OK;
     }
-    return launch_wide_shape<2, 8, 0>(ctx, geo, keys, tiles, keyed, special_head, match_bits, g, matches, layout_choice, 0);
+    return launch_wide_shape<2, 8, 0>(ctx, geo, keys, tiles, keyed, special_head, cmin, match_bits, g, matches, layout_choice, 0);
 }
 
 // build payload re-laid out in SLOT order (one pass at build time): the fused probe then reads the payload right next
@@ -1245,7 +1394,9 @@ struct tgpu_lookup {
     int32_t num_output = 0;
     std::vector<DevBuf> by_slot;        // build output columns in table-slot order (fused probe fast path)
     DevBuf wide;                        // WideSlot[capacity + 1]: slots with the payload of their head row (2 build output columns)
-    DevBuf keyed;                       // KeyedSlot[capacity + 1]: key + payload cell (1 build output column; instead of `wide`)
+    DevBuf keyed;                       // [capacity + 1] slots of keyed_bytes: key + payload cell (1 build output column; instead of `wide`)
+    int keyed_bytes = 0;                // 16: KeyedSlot; 8 / 4: PackedSlot8 / PackedSlot4 (mode 2), cells relative to keyed_cmin
+    unsigned long long keyed_cmin = 0;
     bool generic = false;               // keyed by row hash + verification against build_keys
     int attempts = 1;                   // generic only: hash functions the build needed (> 1 iff two keys shared a 64-bit hash)
     std::vector<DevColumn> build_keys;  // generic only: the real key columns of the build side
@@ -1680,15 +1831,43 @@ struct JoinBuildOp : tgpu_op {
                           c.elem_size(), lk->by_slot[b].p);
             }
         }
-        // slots that carry the payload of their head row: 16-byte keyed slots for one output column, 32-byte wide slots for two
+        // slots that carry the payload of their head row: keyed slots for one output column (packed into 4 or 8 bytes under mode 2 when the
+        // data allow it, else 16 bytes), 32-byte wide slots for two
         if (slot_payload && lk->num_output <= 2 && !lk->has_dups && !lk->generic && cap + 1 < (1LL << 31) && !getenv("TGPU_JOIN_NO_WIDE")) {
             const DevColumn& c0 = lk->store.cols[1];
             const DevColumn* c1 = lk->num_output > 1 ? &lk->store.cols[2] : nullptr;
             const int grid = tg_grid(ctx, cap + 1, 1024, 8);
             if (!c1) {
-                TG_TRY(lk->keyed.alloc(ctx, (size_t)(cap + 1) * sizeof(KeyedSlot)));
-                TG_LAUNCH(ctx, join_wide_table_kernel<KeyedSlot>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->special_head, c0.data, c0.elem_size(),
-                          (const void*)nullptr, 0, lk->keyed.as<KeyedSlot>());
+                lk->keyed_bytes = 16;
+                if (lk->geo.mode == 2) {
+                    DevBuf d_range;
+                    TG_TRY(d_range.alloc(ctx, 4 * sizeof(long long)));
+                    long long range[4] = {INT64_MAX, INT64_MIN, INT64_MAX, INT64_MIN};
+                    TG_CUDA(ctx, cudaMemcpyAsync(d_range.p, range, sizeof(range), cudaMemcpyHostToDevice, ctx->stream));
+                    TG_LAUNCH(ctx, join_packed_range_kernel, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->geo.kmin, lk->geo.shift, lk->special_head, c0.data,
+                              c0.elem_size(), d_range.as<long long>());
+                    TG_CUDA(ctx, cudaMemcpyAsync(range, d_range.p, sizeof(range), cudaMemcpyDeviceToHost, ctx->stream));
+                    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+                    // an empty range (no occupied slot, or no cell) fits every tier
+                    auto fits = [&](long long krel_min, long long krel_max, unsigned long long cell_max) {
+                        const bool krel_ok = range[0] > range[1] || (range[0] > krel_min && range[1] <= krel_max);
+                        const bool cell_ok = range[2] > range[3] || (unsigned long long)range[3] - (unsigned long long)range[2] <= cell_max;
+                        return krel_ok && cell_ok;
+                    };
+                    lk->keyed_cmin = range[2] > range[3] ? 0ULL : (unsigned long long)range[2];
+                    if (fits(PackedSlot4::KREL_MIN, PackedSlot4::KREL_MAX, PackedSlot4::CELL_MAX)) lk->keyed_bytes = 4;
+                    else if (fits(PackedSlot8::KREL_MIN, PackedSlot8::KREL_MAX, PackedSlot8::CELL_MAX)) lk->keyed_bytes = 8;
+                }
+                TG_TRY(lk->keyed.alloc(ctx, (size_t)(cap + 1) * lk->keyed_bytes));
+                if (lk->keyed_bytes == 4)
+                    TG_LAUNCH(ctx, join_packed_table_kernel<PackedSlot4>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->geo.kmin, lk->geo.shift, lk->special_head,
+                              c0.data, c0.elem_size(), lk->keyed_cmin, lk->keyed.as<PackedSlot4>());
+                else if (lk->keyed_bytes == 8)
+                    TG_LAUNCH(ctx, join_packed_table_kernel<PackedSlot8>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->geo.kmin, lk->geo.shift, lk->special_head,
+                              c0.data, c0.elem_size(), lk->keyed_cmin, lk->keyed.as<PackedSlot8>());
+                else
+                    TG_LAUNCH(ctx, join_wide_table_kernel<KeyedSlot>, grid, 256, 0, lk->table.as<JoinSlot>(), cap, lk->special_head, c0.data, c0.elem_size(),
+                              (const void*)nullptr, 0, lk->keyed.as<KeyedSlot>());
             }
             else {
                 TG_TRY(lk->wide.alloc(ctx, (size_t)(cap + 1) * sizeof(WideSlot)));
@@ -1805,19 +1984,23 @@ struct JoinProbeOp : tgpu_op {
                 const bool have_wide = lookup->wide.p && layouts_on;
                 const bool always = (have_wide || have_keyed) && ((we && !strcmp(we, "always")) || payload_bytes >= 16 || !g.by_slot);
                 int* d_choice = (int*)(d_matches + 1);
-                if (always && have_keyed)
-                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, nullptr));
-                else if (always)
-                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, bits, g, d_matches, nullptr));
-                else if (have_keyed) {
+                // the keyed table in its slot type: the random-access shape alone, or the locality vote and both shapes
+                auto run_keyed = [&](const auto* keyed) -> int {
+                    const unsigned long long cmin = lookup->keyed_cmin;
+                    if (always) return launch_wide(ctx, lookup->geo, keys, tiles, keyed, lookup->special_head, cmin, bits, g, d_matches, nullptr);
                     TG_TRY(launch_locality(ctx, lookup->geo, keys, tiles, d_choice));
-                    TG_TRY(launch_keyed_ordered(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
-                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->keyed.as<KeyedSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
-                }
+                    TG_TRY(launch_keyed_ordered(ctx, lookup->geo, keys, tiles, keyed, lookup->special_head, cmin, bits, g, d_matches, d_choice));
+                    return launch_wide(ctx, lookup->geo, keys, tiles, keyed, lookup->special_head, cmin, bits, g, d_matches, d_choice);
+                };
+                if (have_keyed && lookup->keyed_bytes == 4) TG_TRY(run_keyed(lookup->keyed.as<PackedSlot4>()));
+                else if (have_keyed && lookup->keyed_bytes == 8) TG_TRY(run_keyed(lookup->keyed.as<PackedSlot8>()));
+                else if (have_keyed) TG_TRY(run_keyed(lookup->keyed.as<KeyedSlot>()));
+                else if (always)
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, 0ULL, bits, g, d_matches, nullptr));
                 else if (have_wide) {
                     TG_TRY(launch_locality(ctx, lookup->geo, keys, tiles, d_choice));
                     TG_TRY(launch_lean<true>(ctx, lookup->geo, keys, tiles, (const int4*)table, lookup->special_head, nullptr, bits, g, d_matches));
-                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, bits, g, d_matches, d_choice));
+                    TG_TRY(launch_wide(ctx, lookup->geo, keys, tiles, lookup->wide.as<WideSlot>(), lookup->special_head, 0ULL, bits, g, d_matches, d_choice));
                 }
                 else
                     TG_TRY(launch_lean<true>(ctx, lookup->geo, keys, tiles, (const int4*)table, lookup->special_head, nullptr, bits, g, d_matches));
