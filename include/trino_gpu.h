@@ -312,6 +312,10 @@ int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* channel_type
 /* Same for the FilterAndProject kernels generated from `program` (tg_fp_filter_jit / tg_fp_project_jit). */
 int tgpu_jit_selftest_filter_project(const tgpu_expr_program* program, const int32_t* channel_types, int32_t num_channels, uint32_t nullable_mask,
                                      int64_t* cubin_bytes, char* source_out, int64_t source_cap);
+/* Same for the join filter kernels generated from `program` over the join-sources layout (tg_jf_positions_jit / tg_jf_pairs_jit):
+   channel_types / nullable_mask describe all num_channels layout channels, the first num_build_channels of them build channels. */
+int tgpu_jit_selftest_join_filter(const tgpu_expr_program* program, int32_t num_build_channels, const int32_t* channel_types, int32_t num_channels,
+                                  uint32_t nullable_mask, int64_t* cubin_bytes, char* source_out, int64_t source_cap);
 /* GroupByHash.getGroupCount() */
 int tgpu_agg_group_count(tgpu_op* op, int64_t* out);
 
@@ -354,6 +358,20 @@ typedef struct tgpu_join_probe_spec {
 } tgpu_join_probe_spec;
 
 int tgpu_join_build_create(tgpu_ctx* ctx, const tgpu_join_build_spec* spec, tgpu_op** out);
+/* HashBuilderOperatorFactory with a filterFunctionFactory: `filter` is a tgpu_expr_program with filter_temp >= 0 and no
+   projections, over the join-sources layout; num_build_channels = buildLayout.size().
+   The layout (LocalExecutionPlanner.compileJoinFilterFunction, M/sql/planner/LocalExecutionPlanner.java:3199-3215) is the build
+   channels, then the probe channels: channel c < num_build_channels reads build channel c at the build position, any other channel
+   reads probe channel c - num_build_channels at the probe row.  NULL or FALSE makes a position ineligible (JoinHash.isJoinPositionEligible,
+   M/operator/join/JoinHash.java:154-157): the probes emit only eligible positions, outputSingleMatch takes the first eligible one of the
+   chain, an outer probe row without one gets its NULL-build row, and LOOKUP_OUTER / FULL_OUTER mark only emitted positions visited.
+   The filter runs for every candidate of a chain (under outputSingleMatch up to the first eligible one) and its errors are raised
+   there only.  tgpu_lookup_get_join_positions and tgpu_lookup_key_domain do not apply it.
+   INVALID_ARGUMENT: projections, no filter_temp, num_build_channels < 0, a build page whose channel count is not num_build_channels,
+   or a channel outside the layout (the probe side is checked at each probe page).  NOT_SUPPORTED (at the first page that shows the
+   type): the filter computes on a VARCHAR, long DECIMAL (INT128) or REAL channel, as in FilterAndProject.                        */
+int tgpu_join_build_create_filtered(tgpu_ctx* ctx, const tgpu_join_build_spec* spec, const tgpu_expr_program* filter,
+                                    int32_t num_build_channels, tgpu_op** out);
 /* valid after finish(): lendPartitionLookupSource (PartitionedLookupSourceFactory.java:100).  The
  * lookup stays alive until tgpu_lookup_release, independent of the build operator handle.       */
 int tgpu_join_build_get_lookup(tgpu_op* build, tgpu_lookup** out);

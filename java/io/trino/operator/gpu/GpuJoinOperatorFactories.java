@@ -2,7 +2,8 @@
  * GPU counterparts of the join, filter/project and partitioned-output factories, instantiated at the LocalExecutionPlanner sites named
  * in SURVEY.md §8(b): hash build (M/sql/planner/LocalExecutionPlanner.java:3038-3054), probe (OperatorFactories.join called at :3061-3069),
  * filter/project (:2111-2153), partitioned output (:556-633).  The planner takes these branches only for shapes the library supports
- * (no join filter function, no sort channel; SystemPartitionFunction.HASH; expressions of BIGINT/DOUBLE/BOOLEAN operators) and keeps the
+ * (a join filter function only as a translated program, no sort channel; SystemPartitionFunction.HASH; expressions of BIGINT/DOUBLE/BOOLEAN
+ * operators) and keeps the
  * Java factories otherwise - TGPU_ERR_NOT_SUPPORTED never reaches a running query.  NOT compiled here (no JDK).
  */
 package io.trino.operator.gpu;
@@ -20,6 +21,7 @@ import io.trino.sql.planner.plan.PlanNodeId;
 import java.lang.foreign.Arena;
 import java.lang.foreign.MemorySegment;
 import java.util.List;
+import java.util.Optional;
 
 import static com.google.common.base.Preconditions.checkState;
 import static com.google.common.util.concurrent.MoreExecutors.directExecutor;
@@ -40,10 +42,20 @@ public final class GpuJoinOperatorFactories
         private final List<Integer> hashChannels;
         private final List<Integer> outputChannels;
         private final long expectedPositions;
+        // filterFunctionFactory's RowExpression translated by GpuExpressionTranslator to a tgpu_expr_program (filter only) over
+        // createJoinSourcesLayout(buildLayout, probeLayout), kept alive by the factory, and buildLayout.size(); empty = no join filter function
+        private final Optional<MemorySegment> filter;
+        private final int buildLayoutSize;
         private boolean closed;
 
         public GpuHashBuilderOperatorFactory(int operatorId, PlanNodeId planNodeId, JoinBridgeManager<PartitionedLookupSourceFactory> bridgeManager, int[] inputTypes,
                 List<Integer> hashChannels, List<Integer> outputChannels, long expectedPositions)
+        {
+            this(operatorId, planNodeId, bridgeManager, inputTypes, hashChannels, outputChannels, expectedPositions, Optional.empty(), inputTypes.length);
+        }
+
+        public GpuHashBuilderOperatorFactory(int operatorId, PlanNodeId planNodeId, JoinBridgeManager<PartitionedLookupSourceFactory> bridgeManager, int[] inputTypes,
+                List<Integer> hashChannels, List<Integer> outputChannels, long expectedPositions, Optional<MemorySegment> filter, int buildLayoutSize)
         {
             this.operatorId = operatorId;
             this.planNodeId = planNodeId;
@@ -52,6 +64,8 @@ public final class GpuJoinOperatorFactories
             this.hashChannels = List.copyOf(hashChannels);
             this.outputChannels = List.copyOf(outputChannels);
             this.expectedPositions = expectedPositions;
+            this.filter = filter;
+            this.buildLayoutSize = buildLayoutSize;
         }
 
         @Override
@@ -60,7 +74,9 @@ public final class GpuJoinOperatorFactories
             checkState(!closed, "Factory is already closed");
             OperatorContext operatorContext = driverContext.addOperatorContext(operatorId, planNodeId, "GpuHashBuilderOperator");
             GpuContexts.Handle gpu = GpuContexts.forCurrentDriver(driverContext);
-            MemorySegment op = NativeSpecs.createJoinBuild(gpu, hashChannels, outputChannels, expectedPositions);
+            MemorySegment op = filter.isPresent()
+                    ? NativeSpecs.createJoinBuildFiltered(gpu, hashChannels, outputChannels, expectedPositions, filter.get(), buildLayoutSize)
+                    : NativeSpecs.createJoinBuild(gpu, hashChannels, outputChannels, expectedPositions);
             PartitionedLookupSourceFactory bridge = bridgeManager.getJoinBridge();
             return new GpuOperator(operatorContext, gpu.context(), op, gpu.marshaller(inputTypes), new int[0])
             {

@@ -165,6 +165,32 @@ public final class NativeSpecs
         }
     }
 
+    /** HashBuilderOperatorFactory with a filterFunctionFactory: `filter` is a tgpu_expr_program over the join-sources layout, buildLayoutSize its build channels */
+    public static MemorySegment createJoinBuildFiltered(GpuContexts.Handle gpu, List<Integer> hashChannels, List<Integer> outputChannels, long expectedPositions,
+            MemorySegment filter, int buildLayoutSize)
+    {
+        try (Arena arena = Arena.ofConfined()) {
+            MemorySegment spec = arena.allocate(JOIN_BUILD_SPEC);
+            spec.set(JAVA_INT, 0, hashChannels.size());
+            spec.set(ADDRESS, 8, ints(arena, hashChannels));
+            spec.set(JAVA_INT, 16, outputChannels.size());
+            spec.set(ADDRESS, 24, ints(arena, outputChannels));
+            spec.set(JAVA_LONG, 32, expectedPositions);
+            MemorySegment out = arena.allocate(ADDRESS);
+            int status = (int) TrinoGpuLibrary.JOIN_BUILD_CREATE_FILTERED.invokeExact(gpu.context(), spec, filter, buildLayoutSize, out);
+            if (status != 0) {
+                throw GpuOperator.failure(status, gpu.context());
+            }
+            return out.get(ADDRESS, 0);
+        }
+        catch (RuntimeException e) {
+            throw e;
+        }
+        catch (Throwable e) {
+            throw new RuntimeException(e);
+        }
+    }
+
     /** joinType: 0 INNER, 1 PROBE_OUTER, 2 LOOKUP_OUTER, 3 FULL_OUTER (LookupJoinOperatorFactory.JoinType) */
     public static MemorySegment createJoinProbe(GpuContexts.Handle gpu, MemorySegment lookup, int joinType, boolean outputSingleMatch, List<Integer> probeJoinChannels,
             List<Integer> probeOutputChannels)

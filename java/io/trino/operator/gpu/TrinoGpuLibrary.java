@@ -47,6 +47,7 @@ public final class TrinoGpuLibrary
     static final MethodHandle PA_CONTROLLER_IS_DISABLED = handle("tgpu_partial_agg_controller_is_disabled", FunctionDescriptor.of(JAVA_INT, ADDRESS));
     static final MethodHandle AGG_ROWS_WITH_PA_DISABLED = handle("tgpu_agg_rows_with_partial_aggregation_disabled", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
     static final MethodHandle JOIN_BUILD_CREATE = handle("tgpu_join_build_create", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
+    static final MethodHandle JOIN_BUILD_CREATE_FILTERED = handle("tgpu_join_build_create_filtered", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, ADDRESS));
     static final MethodHandle JOIN_BUILD_GET_LOOKUP = handle("tgpu_join_build_get_lookup", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
     static final MethodHandle JOIN_PROBE_CREATE = handle("tgpu_join_probe_create", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     static final MethodHandle LOOKUP_RELEASE = handle("tgpu_lookup_release", FunctionDescriptor.ofVoid(ADDRESS));

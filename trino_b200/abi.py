@@ -192,10 +192,13 @@ SIGNATURES = {
     "tgpu_partial_agg_controller_is_disabled": (C.c_int, [VP]),
     "tgpu_partial_agg_controller_on_flush": (None, [VP, C.c_int64, C.c_int64, C.c_int64]),
     "tgpu_jit_selftest_filter_project": (C.c_int, [C.POINTER(ExprProgram), C.POINTER(C.c_int32), C.c_int32, C.c_uint32, C.POINTER(C.c_int64), C.c_char_p, C.c_int64]),
+    "tgpu_jit_selftest_join_filter": (C.c_int, [C.POINTER(ExprProgram), C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_uint32, C.POINTER(C.c_int64), C.c_char_p,
+                                                C.c_int64]),
     "tgpu_jit_selftest_agg": (C.c_int, [C.POINTER(AggSpec), C.POINTER(C.c_int32), C.c_int32, C.c_uint32, C.POINTER(C.c_int64), C.c_char_p, C.c_int64]),
     "tgpu_groupby_hash_create": (C.c_int, [VP, C.c_int32, C.POINTER(C.c_int32), C.c_int64, C.POINTER(VP)]),
     "tgpu_groupby_hash_get_group_ids": (C.c_int, [VP, PP, VP]),
     "tgpu_join_build_create": (C.c_int, [VP, C.POINTER(JoinBuildSpec), C.POINTER(VP)]),
+    "tgpu_join_build_create_filtered": (C.c_int, [VP, C.POINTER(JoinBuildSpec), C.POINTER(ExprProgram), C.c_int32, C.POINTER(VP)]),
     "tgpu_join_build_get_lookup": (C.c_int, [VP, C.POINTER(VP)]),
     "tgpu_lookup_release": (None, [VP]),
     "tgpu_lookup_position_count": (C.c_int64, [VP]),

@@ -34,6 +34,7 @@ struct TgScratch {
     // join probe / lookup outer
     long long join_probe_count;       // matched probe rows
     long long join_outer_count;       // unvisited build rows
+    uint32_t join_filter_flags[2];    // join filter function: [0] error bits of the evaluated candidates
     // FilterAndProject
     uint32_t fp_flags[2];             // [0] error bits, [1] any-NULL bit per computed column
     long long fp_count;               // selected rows

@@ -72,6 +72,67 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
     return TGPU_OK;
 }
 
+int expr_raise(tgpu_ctx* ctx, int64_t errbits)
+{
+    if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
+    if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
+    if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
+    return TGPU_OK;
+}
+
+// ---- NVRTC code generation of programs -------------------------------------------------------------------------------
+void fp_appendf(std::string& s, const char* fmt, ...)
+{
+    char buf[1024];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof(buf), fmt, ap);
+    va_end(ap);
+    s += buf;
+}
+
+static std::string fp_operand(const DOperand& o)
+{
+    char buf[128];
+    switch (o.kind) {
+        case TGPU_OPND_COLUMN: snprintf(buf, sizeof(buf), "Value{c%d, c%dn}", o.index, o.index); break;
+        case TGPU_OPND_TEMP: snprintf(buf, sizeof(buf), "Value{t%d, tn%d}", o.index, o.index); break;
+        case TGPU_OPND_CONST: snprintf(buf, sizeof(buf), "Value{(long long)0x%llxULL, false}", (unsigned long long)o.imm); break;
+        default: snprintf(buf, sizeof(buf), "Value{0, true}"); break;
+    }
+    return buf;
+}
+
+// the error operand o carries (see vm_error): a temp's, never a column's or a constant's
+static std::string fp_operand_error(const DOperand& o)
+{
+    return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : "0u";
+}
+
+void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
+{
+    for (int i = first; i < last; i++) {
+        const DInsn& in = prog.insns[i];
+        if (in.op == TGPU_EX_IN) {
+            int li = (int)in.b.imm;
+            fp_appendf(s, "    { Value a = %s; bool hit = false;\n", fp_operand(in.a).c_str());
+            for (int k = 0; k < prog.in_count[li]; k++) {
+                unsigned long long c = (unsigned long long)prog.in_values[prog.in_offset[li] + k];
+                if (in.vtype == TGPU_V_DOUBLE) fp_appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
+                else fp_appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
+            }
+            fp_appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, fp_operand_error(in.a).c_str());
+        }
+        else {
+            // operands are read into locals first: dst may be one of them, and vm_error needs their values
+            fp_appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", fp_operand(in.a).c_str(),
+                       fp_operand(in.b).c_str(), fp_operand(in.c).c_str(), in.op, in.vtype);
+            fp_appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
+                       fp_operand_error(in.a).c_str(), fp_operand_error(in.b).c_str(), fp_operand_error(in.c).c_str(), in.dst, in.dst, in.dst);
+        }
+    }
+}
+
 }  // namespace tg
 
 namespace {
@@ -79,6 +140,8 @@ namespace {
 using namespace tg;
 
 constexpr int FP_THREADS = 256;
+
+// ---- NVRTC specialisation of the two PageProcessor kernels ----------------------------------------------------------
 
 // filter pass: one row per thread, writes 1/0 selection flags
 __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* __restrict__ prog, DColumns cols, int64_t n, uint8_t* __restrict__ flags,
@@ -127,59 +190,6 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
     if (nulls_seen) atomicOr(any_null, nulls_seen);
 }
 
-
-// ---- NVRTC specialisation of the two PageProcessor kernels ----------------------------------------------------------
-static void fp_appendf(std::string& s, const char* fmt, ...)
-{
-    char buf[1024];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    s += buf;
-}
-
-static std::string fp_operand(const DOperand& o)
-{
-    char buf[128];
-    switch (o.kind) {
-        case TGPU_OPND_COLUMN: snprintf(buf, sizeof(buf), "Value{c%d, c%dn}", o.index, o.index); break;
-        case TGPU_OPND_TEMP: snprintf(buf, sizeof(buf), "Value{t%d, tn%d}", o.index, o.index); break;
-        case TGPU_OPND_CONST: snprintf(buf, sizeof(buf), "Value{(long long)0x%llxULL, false}", (unsigned long long)o.imm); break;
-        default: snprintf(buf, sizeof(buf), "Value{0, true}"); break;
-    }
-    return buf;
-}
-
-// the error operand o carries (see vm_error): a temp's, never a column's or a constant's
-static std::string fp_operand_error(const DOperand& o)
-{
-    return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : "0u";
-}
-
-static void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
-{
-    for (int i = first; i < last; i++) {
-        const DInsn& in = prog.insns[i];
-        if (in.op == TGPU_EX_IN) {
-            int li = (int)in.b.imm;
-            fp_appendf(s, "    { Value a = %s; bool hit = false;\n", fp_operand(in.a).c_str());
-            for (int k = 0; k < prog.in_count[li]; k++) {
-                unsigned long long c = (unsigned long long)prog.in_values[prog.in_offset[li] + k];
-                if (in.vtype == TGPU_V_DOUBLE) fp_appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
-                else fp_appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
-            }
-            fp_appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, fp_operand_error(in.a).c_str());
-        }
-        else {
-            // operands are read into locals first: dst may be one of them, and vm_error needs their values
-            fp_appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", fp_operand(in.a).c_str(),
-                       fp_operand(in.b).c_str(), fp_operand(in.c).c_str(), in.op, in.vtype);
-            fp_appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
-                       fp_operand_error(in.a).c_str(), fp_operand_error(in.b).c_str(), fp_operand_error(in.c).c_str(), in.dst, in.dst, in.dst);
-        }
-    }
-}
 
 // straight-line typed code for one program over channels of the given element sizes
 static std::string gen_fp_source(const DProgram& prog, const int* elems, int num_channels, uint32_t nullable_mask, const std::vector<int>& pass_channels)
@@ -553,13 +563,7 @@ struct FilterProjectOp : tgpu_op {
         return TGPU_OK;
     }
 
-    int raise(int64_t errbits)
-    {
-        if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
-        if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
-        if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
-        return TGPU_OK;
-    }
+    int raise(int64_t errbits) { return expr_raise(ctx, errbits); }
 
     int get_output(OwnedPage** out) override
     {

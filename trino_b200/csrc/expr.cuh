@@ -46,14 +46,18 @@ struct DProgram {
 
 #if defined(__CUDACC__)
 
-__device__ __forceinline__ Value vm_fetch(const DOperand& o, const DColumns& cols, int64_t row, const int64_t* temps, int tstride, uint32_t nullbits)
+// Channels below `split` are read at `split_row`, the others at `row`: a join filter reads the build channels of the join-sources
+// layout at the build position and the probe channels at the probe row.  split = 0 (the default) reads every channel at `row`.
+__device__ __forceinline__ Value vm_fetch(const DOperand& o, const DColumns& cols, int64_t row, const int64_t* temps, int tstride, uint32_t nullbits,
+                                          int split = 0, int64_t split_row = 0)
 {
     Value v;
     switch (o.kind) {
         case TGPU_OPND_COLUMN: {
             const ColRef& c = cols.cols[o.index];
-            v.is_null = !tg_valid(c.validity, row);
-            v.bits = tg_load_i64(c, row);
+            const int64_t r = o.index < split ? split_row : row;
+            v.is_null = !tg_valid(c.validity, r);
+            v.bits = tg_load_i64(c, r);
             break;
         }
         case TGPU_OPND_TEMP:
@@ -82,15 +86,15 @@ __device__ __forceinline__ uint32_t vm_temp_error(uint32_t errs, int t) { return
 
 // Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
 // [temp][thread] array (stride tstride).  Returns the updated null bitmask; *errs holds the TG_ERR_BIT_* each temp
-// carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.
+// carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.  `split` / `split_row`: see vm_fetch.
 __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
-                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs)
+                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs, int split = 0, int64_t split_row = 0)
 {
     uint32_t te = *errs;
     for (int pc = first; pc < last; pc++) {
         const DInsn& in = prog->insns[pc];
-        Value a = vm_fetch(in.a, cols, row, temps, tstride, nullbits);
-        Value b = vm_fetch(in.b, cols, row, temps, tstride, nullbits);
+        Value a = vm_fetch(in.a, cols, row, temps, tstride, nullbits, split, split_row);
+        Value b = vm_fetch(in.b, cols, row, temps, tstride, nullbits, split, split_row);
         Value c;
         c.bits = 0; c.is_null = true;
         uint32_t own = 0, ec = 0;
@@ -112,7 +116,7 @@ __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, in
         }
         else {
             if (in.op == TGPU_EX_BETWEEN) {
-                c = vm_fetch(in.c, cols, row, temps, tstride, nullbits);
+                c = vm_fetch(in.c, cols, row, temps, tstride, nullbits, split, split_row);
                 ec = vm_carried(in.c, te);
             }
             Value res = vm_apply(in.op, in.vtype, a, b, c, &own);
@@ -132,5 +136,13 @@ __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, in
 
 // host side: validate + flatten a tgpu_expr_program into a DProgram (defined in expr.cu)
 int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* program, DProgram* out, int32_t* max_channel);
+
+// NVRTC code generation shared by the operators that specialise a program (defined in expr.cu): printf-style append, and the
+// straight-line code of instructions [first, last) over locals c<k> / c<k>n (channel k's value and NULL flag) and t<i> / tn<i> / te<i>
+// (temp i's value, NULL flag and carried error bits), which the caller declares
+void fp_appendf(std::string& s, const char* fmt, ...);
+void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last);
+// fail with the error one set of TG_ERR_BIT_* bits stands for (TGPU_OK when none is set)
+int expr_raise(tgpu_ctx* ctx, int64_t errbits);
 
 }  // namespace tg

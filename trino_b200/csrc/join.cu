@@ -12,6 +12,9 @@
 //   expand: PageJoiner.joinCurrentPosition / outerJoinCurrentPosition (PageJoiner.java:203-242) and
 //           LookupJoinPageBuilder.build (LookupJoinPageBuilder.java:119-160): output rows in probe order,
 //           within one probe row in chain order; probe columns first, then build output columns.
+//   filter: JoinHash.isJoinPositionEligible (M/operator/join/JoinHash.java:154-157): a JoinFilterFunction over the
+//           join-sources layout (build channels, then probe channels) drops the positions it does not accept, before
+//           outputSingleMatch picks the first one and before an outer join falls back to its NULL-build row.
 //
 // Design: the table is an open-addressing array of 16-byte slots {int64 key, int32 head} so that one
 // probe touches exactly one 32-byte sector; the deterministic "head = highest row" of the sequential
@@ -21,11 +24,14 @@
 #include <algorithm>
 #include <mutex>
 
+#include "expr.cuh"
+#include "jit.cuh"
 #include "rowkeys.cuh"
 
 namespace {
 
 using tg::KeyCols;
+using tg::DProgram;
 
 constexpr unsigned long long EMPTY_KEY = 0x8000000000000000ULL;   // INT64_MIN is kept out of the table
 
@@ -1373,6 +1379,156 @@ __global__ void join_fill_kernel(const int* __restrict__ jp, int64_t n, const in
     }
 }
 
+// --- join filter function -----------------------------------------------------------------------------
+// JoinFilterFunction.filter(leftPosition, rightPosition) (M/sql/gen/JoinFilterFunctionCompiler.java:94-131): the filter's channels are
+// the join-sources layout.  DColumns slot c < nb holds build channel c, read at the build position; slot c >= nb holds probe channel
+// c - nb, read at the probe row.  NULL or FALSE: the position is not eligible.
+constexpr int JF_THREADS = 256;
+
+__device__ __forceinline__ bool jf_eval(const DProgram* __restrict__ prog, const DColumns& cols, int nb, int64_t probe_row, int64_t build_pos,
+                                        int64_t* temps, uint32_t* err)
+{
+    uint32_t te = 0;
+    const uint32_t nulls = tg::vm_run(prog, 0, prog->num_filter_insns, cols, probe_row, temps, JF_THREADS, 0, &te, nb, build_pos);
+    const int ft = prog->filter_temp;
+    *err = tg::vm_temp_error(te, ft);
+    return !((nulls >> ft) & 1) && temps[ft * JF_THREADS] != 0;
+}
+
+// lookup without position links: each probe row has at most one candidate; jp[i] = -1 where it is not eligible
+__global__ void __launch_bounds__(JF_THREADS) join_filter_positions_kernel(const DProgram* __restrict__ prog, DColumns cols, int nb, int64_t n,
+                                                                          int* __restrict__ jp, unsigned int* __restrict__ err_out)
+{
+    __shared__ int64_t temps[TGPU_MAX_TEMPS * JF_THREADS];
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    uint32_t err = 0;
+    for (; i < n; i += stride) {
+        const int b = jp[i];
+        if (b < 0) continue;
+        uint32_t e = 0;
+        if (!jf_eval(prog, cols, nb, i, b, temps + threadIdx.x, &e)) jp[i] = -1;
+        err |= e;
+    }
+    if (err) atomicOr(err_out, err);
+}
+
+// candidate pairs (probe row pp[k], build position pb[k]): verdict[k] = eligible | error bits << 1
+__global__ void __launch_bounds__(JF_THREADS) join_filter_pairs_kernel(const DProgram* __restrict__ prog, DColumns cols, int nb, int64_t m,
+                                                                      const int* __restrict__ pp, const int* __restrict__ pb, uint8_t* __restrict__ verdict)
+{
+    __shared__ int64_t temps[TGPU_MAX_TEMPS * JF_THREADS];
+    int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; k < m; k += stride) {
+        uint32_t e = 0;
+        const bool ok = jf_eval(prog, cols, nb, pp[k], pb[k], temps + threadIdx.x, &e);
+        verdict[k] = (uint8_t)((ok ? 1u : 0u) | (e << 1));
+    }
+}
+
+// PageJoiner.joinCurrentPosition over the candidate pairs of probe row i, [off[i], off[i + 1]) in chain order: eligible pairs are kept,
+// outputSingleMatch keeps the first one and evaluates no further pair; an outer join with no kept pair emits one NULL-build row
+// (outerJoinCurrentPosition).  verdict[k] becomes 1 for the kept pairs; counts[i] = output rows of row i; the error bits of the
+// evaluated pairs are or-ed into *err_out
+__global__ void join_filter_select_kernel(const long long* __restrict__ off, int64_t n, int single_match, int outer, uint8_t* __restrict__ verdict,
+                                          int* __restrict__ counts, unsigned int* __restrict__ err_out)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    uint32_t err = 0;
+    for (; i < n; i += stride) {
+        int kept = 0;
+        bool done = false;
+        for (long long k = off[i]; k < off[i + 1]; k++) {
+            const uint8_t v = verdict[k];
+            bool keep = false;
+            if (!done) {
+                err |= v >> 1;
+                keep = v & 1;
+                if (keep) { kept++; done = single_match != 0; }
+            }
+            verdict[k] = keep ? 1 : 0;
+        }
+        counts[i] = kept ? kept : (outer ? 1 : 0);
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) counts[n] = 0;
+    if (err) atomicOr(err_out, err);
+}
+
+__global__ void join_filter_fill_kernel(const long long* __restrict__ off, int64_t n, const uint8_t* __restrict__ keep, const int* __restrict__ pb, int outer,
+                                        const long long* __restrict__ out_off, int* __restrict__ out_probe, int* __restrict__ out_build)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) {
+        long long o = out_off[i];
+        const long long first = o;
+        for (long long k = off[i]; k < off[i + 1]; k++) {
+            if (!keep[k]) continue;
+            out_probe[o] = (int)i;
+            out_build[o] = pb[k];
+            o++;
+        }
+        if (o == first && outer) {
+            out_probe[o] = (int)i;
+            out_build[o] = -1;
+        }
+    }
+}
+
+// NVRTC form of the two evaluation kernels, specialised for one program over the given channel element sizes / nullability
+std::string gen_join_filter_source(const DProgram& prog, int nb, const int* elems, int num_channels, uint32_t nullable_mask)
+{
+    std::string s, loads, temps;
+    bool used[TGPU_MAX_CHANNELS] = {false};
+    for (int i = 0; i < prog.num_filter_insns; i++) {
+        const tg::DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
+        for (auto* o : ops)
+            if (o->kind == TGPU_OPND_COLUMN) used[o->index] = true;
+    }
+    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
+        if (!used[c]) continue;
+        const char* row = c < nb ? "b" : "p";
+        tg::fp_appendf(loads, "    const long long c%d = tg_load_elem<%d>(cols.cols[%d].data, %s);", c, elems[c], c, row);
+        if ((nullable_mask >> c) & 1) tg::fp_appendf(loads, " const bool c%dn = !tg_valid(cols.cols[%d].validity, %s);\n", c, c, row);
+        else tg::fp_appendf(loads, " const bool c%dn = false;\n", c);
+    }
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) tg::fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    const int ft = prog.filter_temp;
+    s += "struct JFProg {\n";
+    s += "  static __device__ __forceinline__ bool eval(const DColumns& cols, long long p, long long b, unsigned int* errp) {\n";
+    s += loads + temps;
+    tg::fp_emit_insns(s, prog, 0, prog.num_filter_insns);
+    tg::fp_appendf(s, "    *errp = te%d;\n    return !tn%d && t%d != 0;\n  }\n};\n", ft, ft, ft);
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_jf_positions_jit(DColumns cols, long long n, int* jp, unsigned int* err_out) {\n";
+    s += "  unsigned int err = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
+    s += "  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {\n";
+    s += "    const int b = jp[i];\n    if (b < 0) continue;\n    unsigned int e = 0;\n";
+    s += "    if (!JFProg::eval(cols, i, b, &e)) jp[i] = -1;\n    err |= e;\n  }\n  if (err) atomicOr(err_out, err);\n}\n";
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_jf_pairs_jit(DColumns cols, long long m, const int* pp, const int* pb, unsigned char* verdict) {\n";
+    s += "  long long stride = (long long)gridDim.x * blockDim.x;\n";
+    s += "  for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += stride) {\n";
+    s += "    unsigned int e = 0;\n    const bool ok = JFProg::eval(cols, pp[k], pb[k], &e);\n";
+    s += "    verdict[k] = (unsigned char)((ok ? 1u : 0u) | (e << 1));\n  }\n}\n";
+    return s;
+}
+
+// validate a join filter program (HashBuilderOperatorFactory's filterFunctionFactory) and flatten it
+int join_filter_compile(tgpu_ctx* ctx, const tgpu_expr_program* program, int32_t num_build_channels, DProgram* out)
+{
+    if (!program) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "join filter program is null");
+    if (program->num_projections != 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a join filter program has no projections (got %d)", program->num_projections);
+    if (program->filter_temp < 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a join filter program needs a filter_temp");
+    if (num_build_channels < 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "num_build_channels %d is negative", num_build_channels);
+    int32_t max_channel = -1;
+    TG_TRY(tg::expr_compile(ctx, program, out, &max_channel));
+    return TGPU_OK;
+}
+
+// a filter reads this channel as a value: only fixed-width integer / DOUBLE / BOOLEAN channels (as FilterAndProject)
+bool join_filter_type_ok(const DevColumn& c) { return c.elem_size() != 0 && c.elem_size() != 16 && c.type != TGPU_FLOAT32; }
+
 int key_kind_of(int type) { return type == TGPU_FLOAT64 ? KEY_DOUBLE : KEY_INT; }
 
 }  // namespace
@@ -1406,6 +1562,14 @@ struct tgpu_lookup {
     std::mutex visited_lock;
     int64_t null_key_rows = -1;         // build rows whose (first) key channel is NULL; -1 = not counted yet
     int64_t nan_key_rows = -1;          // DOUBLE / REAL key: build rows whose key is NaN (members of a semi-join's ChannelSet); -1 = not counted yet
+    // JoinFilterFunction (JoinHash.isJoinPositionEligible): the compiled filter over the join-sources layout [build channels, probe channels]
+    bool has_filter = false;
+    DProgram filter;                    // host copy (the NVRTC source is generated from it)
+    DevBuf d_filter;                    // device copy (interpreter kernels)
+    int32_t num_build_channels = 0;     // buildLayout.size(): layout channels below it are build channels
+    std::vector<int32_t> filter_channels;   // layout channels the filter reads, ascending
+    std::vector<DevColumn> filter_cols; // [num_build_channels]: the build channels the filter reads (shared with store / build_keys), others empty
+    int64_t filter_extra_bytes = 0;     // device bytes of the filter's build channels kept for it alone
 };
 
 namespace {
@@ -1602,8 +1766,15 @@ __global__ void join_key_domain_kernel(const JoinSlot* __restrict__ table, int64
 // HashBuilderOperator: NEEDS_INPUT -> (finish) LOOKUP_SOURCE_BUILT -> CLOSED
 struct JoinBuildOp : tgpu_op {
     std::vector<int32_t> key_channels, output_channels;
-    std::vector<DevPage> chunks;     // key column + output columns of every input page
-    std::vector<int32_t> col_types;  // types of [key, outputs...] as first seen (an empty build still needs them)
+    std::vector<DevPage> chunks;     // key column + output columns (+ the filter's extra channels) of every input page
+    std::vector<int32_t> col_types;  // types of [key, outputs..., extras...] as first seen (an empty build still needs them)
+    // join filter function: the compiled program, buildLayout.size(), and the build channels it reads that are neither key nor output
+    // channels (kept after the outputs in every chunk)
+    bool has_filter = false;
+    DProgram filter;
+    int32_t num_build_channels = 0;
+    std::vector<int32_t> filter_channels;   // layout channels the filter reads
+    std::vector<int32_t> extra_channels;
     int64_t rows = 0;
     bool finishing = false;
     tgpu_lookup* lookup = nullptr;
@@ -1625,7 +1796,10 @@ struct JoinBuildOp : tgpu_op {
             };
             for (int32_t ch : key_channels) col_types.push_back(type_of(ch));
             for (int32_t ch : output_channels) col_types.push_back(type_of(ch));
+            for (int32_t ch : extra_channels) col_types.push_back(type_of(ch));
         }
+        if (has_filter && page->num_columns != num_build_channels)
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "build page has %d channels, the join filter's build layout %d", page->num_columns, num_build_channels);
         if (page->num_rows == 0) return TGPU_OK;
         if (rows + page->num_rows > (int64_t)INT32_MAX)
             return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "Size of pages index cannot exceed 2 billion entries");   // PagesIndex.java:247-250
@@ -1641,10 +1815,29 @@ struct JoinBuildOp : tgpu_op {
         };
         for (int32_t ch : key_channels) TG_TRY(take(ch));
         for (int32_t ch : output_channels) TG_TRY(take(ch));
+        for (int32_t ch : extra_channels) TG_TRY(take(ch));
         if (!device) TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        for (int32_t ch : filter_channels) {
+            if (ch >= num_build_channels) break;
+            const DevColumn& c = p.cols[kept_at(ch)];
+            if (!join_filter_type_ok(c))
+                return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters over variable-width / 128-bit / REAL channel %d are not supported on the GPU path", ch);
+        }
         rows += p.rows;
         chunks.push_back(std::move(p));
         return TGPU_OK;
+    }
+
+    // column of a chunk that holds build channel ch (the filter's build channels are kept once)
+    size_t kept_at(int32_t ch) const
+    {
+        for (size_t b = 0; b < output_channels.size(); b++)
+            if (output_channels[b] == ch) return key_channels.size() + b;
+        for (size_t k = 0; k < key_channels.size(); k++)
+            if (key_channels[k] == ch) return k;
+        for (size_t e = 0; e < extra_channels.size(); e++)
+            if (extra_channels[e] == ch) return key_channels.size() + output_channels.size() + e;
+        return (size_t)-1;
     }
 
     int concat(DevPage* out)
@@ -1652,7 +1845,7 @@ struct JoinBuildOp : tgpu_op {
         if (chunks.size() == 1) { *out = std::move(chunks[0]); chunks.clear(); return TGPU_OK; }
         DevPage r;
         r.rows = rows;
-        size_t ncols = key_channels.size() + output_channels.size();
+        size_t ncols = key_channels.size() + output_channels.size() + extra_channels.size();
         r.cols.resize(ncols);
         for (size_t c = 0; c < ncols && !chunks.empty(); c++) {
             std::vector<const DevColumn*> parts;
@@ -1676,7 +1869,7 @@ struct JoinBuildOp : tgpu_op {
         TG_TRY(concat(&all));
         const size_t nk = key_channels.size();
         if (rows == 0) {
-            all.cols.resize(nk + output_channels.size());
+            all.cols.resize(nk + output_channels.size() + extra_channels.size());
             for (size_t c = 0; c < all.cols.size(); c++) all.cols[c].type = c < col_types.size() && col_types[c] ? col_types[c] : TGPU_INT64;
         }
         // one fixed-width channel -> the table is keyed by the value itself; anything else -> by the row hash + verification
@@ -1691,8 +1884,20 @@ struct JoinBuildOp : tgpu_op {
             lk->store.cols.push_back(std::move(fp));
         }
         else lk->store.cols.push_back(all.cols[0]);
-        for (size_t c = nk; c < all.cols.size(); c++) lk->store.cols.push_back(all.cols[c]);
+        for (size_t c = nk; c < nk + output_channels.size(); c++) lk->store.cols.push_back(all.cols[c]);
         lk->key_type = lk->store.cols[0].type;
+        if (has_filter) {
+            lk->has_filter = true;
+            lk->filter = filter;
+            lk->num_build_channels = num_build_channels;
+            lk->filter_channels = filter_channels;
+            lk->filter_cols.resize(num_build_channels);
+            for (int32_t ch : filter_channels)
+                if (ch < num_build_channels) lk->filter_cols[ch] = all.cols[kept_at(ch)];     // shares the buffers
+            for (size_t e = 0; e < extra_channels.size(); e++) lk->filter_extra_bytes += all.cols[nk + output_channels.size() + e].memory_bytes();
+            TG_TRY(lk->d_filter.alloc(ctx, sizeof(DProgram)));
+            TG_CUDA(ctx, cudaMemcpyAsync(lk->d_filter.p, &lk->filter, sizeof(DProgram), cudaMemcpyHostToDevice, ctx->stream));
+        }
         int64_t cap = 0;
         auto build_table = [&]() -> int {
             // sizing: IncrementalLoadFactorHashArraySizeSupplier.getHashArraySize :40-47 (capacity is not observable)
@@ -2039,7 +2244,7 @@ struct JoinProbeOp : tgpu_op {
         for (int32_t c = 0; c < page->num_columns; c++) {
             if (page->columns[c].length != page->num_rows) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "column %d has %lld positions, page has %lld", c,
                                                                           (long long)page->columns[c].length, (long long)page->num_rows);
-            bool is_key = c == key_channels[0];
+            bool is_key = c == key_channels[0] || reads_probe_channel(c);    // (the join filter's probe channels go up with the key)
             if (is_key) TG_TRY(tg_ingest_column(ctx, &page->columns[c], false, &p.cols[c]));
             else { p.cols[c].type = page->columns[c].type; p.cols[c].length = page->num_rows; }
         }
@@ -2049,6 +2254,118 @@ struct JoinProbeOp : tgpu_op {
     }
 
     static bool absent(const DevColumn& c) { return c.data == nullptr && c.length > 0; }
+
+    bool reads_probe_channel(int32_t c) const
+    {
+        if (!lookup->has_filter) return false;
+        return std::find(lookup->filter_channels.begin(), lookup->filter_channels.end(), lookup->num_build_channels + c) != lookup->filter_channels.end();
+    }
+
+    // ---- join filter function ----
+    void* jit_jf_positions = nullptr;   // NVRTC kernels for the current page shape (nullptr: interpreter kernels)
+    void* jit_jf_pairs = nullptr;
+    std::string jit_jf_key;
+
+    // the join-sources layout of this page (build channels, then probe channels) as the filter kernels read it; checks the channels
+    int filter_columns(const DevPage& in, DColumns* cols)
+    {
+        memset(cols, 0, sizeof(*cols));
+        const int nb = lookup->num_build_channels;
+        int elems[TGPU_MAX_CHANNELS] = {0};
+        uint32_t nullable = 0;
+        for (int32_t ch : lookup->filter_channels) {
+            const DevColumn* c = nullptr;
+            if (ch < nb) c = &lookup->filter_cols[ch];
+            else if (ch - nb < (int32_t)in.cols.size()) c = &in.cols[ch - nb];
+            else return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "join filter reads channel %d: the layout has %d build and %zu probe channels", ch, nb, in.cols.size());
+            if (!join_filter_type_ok(*c))
+                return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters over variable-width / 128-bit / REAL channel %d are not supported on the GPU path", ch);
+            cols->cols[ch] = tg_colref(*c);
+            elems[ch] = c->elem_size();
+            if (c->validity) nullable |= 1u << ch;
+        }
+        if (!tg::jit_available()) { jit_jf_positions = jit_jf_pairs = nullptr; return TGPU_OK; }
+        std::string key;
+        for (int c = 0; c < TGPU_MAX_CHANNELS; c++) key += (char)('0' + elems[c]);
+        key += ":" + std::to_string(nullable);
+        if (key == jit_jf_key && jit_jf_positions) return TGPU_OK;
+        const std::string src = gen_join_filter_source(lookup->filter, nb, elems, TGPU_MAX_CHANNELS, nullable);
+        TG_TRY(tg::jit_get_function(ctx, src, "tg_jf_positions_jit", &jit_jf_positions));
+        TG_TRY(tg::jit_get_function(ctx, src, "tg_jf_pairs_jit", &jit_jf_pairs));
+        jit_jf_key = key;
+        return TGPU_OK;
+    }
+
+    int raise_filter_errors()
+    {
+        int64_t word = 0;
+        TG_TRY(tg_read_i64(ctx, ctx->d_scratch->join_filter_flags, &word));
+        return tg::expr_raise(ctx, word & 0xFFFFFFFFLL);
+    }
+
+    // no position links: the one candidate of each probe row is dropped (jp[i] = -1) when the filter does not accept it
+    int filter_positions(DColumns cols, int* jp, int64_t n)
+    {
+        unsigned int* d_err = ctx->d_scratch->join_filter_flags;
+        TG_CUDA(ctx, cudaMemsetAsync(d_err, 0, 8, ctx->stream));
+        long long n_arg = n;
+        if (jit_jf_positions) {
+            void* params[4] = {&cols, &n_arg, &jp, &d_err};
+            TG_TRY(tg::jit_launch(ctx, jit_jf_positions, tg_grid(ctx, n, JF_THREADS, tg::jit_blocks_per_sm(jit_jf_positions, JF_THREADS, 0)), JF_THREADS, 0, params));
+        }
+        else TG_LAUNCH(ctx, join_filter_positions_kernel, tg_grid(ctx, n, JF_THREADS, 8), JF_THREADS, 0, lookup->d_filter.as<DProgram>(), cols,
+                       lookup->num_build_channels, n, jp, d_err);
+        return raise_filter_errors();
+    }
+
+    // with position links: candidate pairs in chain order, the filter's verdict on each, then PageJoiner's choice per probe row.
+    // Output rows (probe row, build position or -1) into out_probe / out_build, their number into *total
+    int filter_pairs(DColumns cols, const int* jp, int64_t n, const int* links, bool outer, DevBuf* out_probe, DevBuf* out_build, int64_t* total)
+    {
+        const int grid = tg_grid(ctx, n, 256 * 4, 8);
+        DevBuf counts, offsets;
+        TG_TRY(counts.alloc(ctx, (size_t)(n + 1) * 4));
+        TG_TRY(offsets.alloc(ctx, (size_t)(n + 1) * 8));
+        TG_LAUNCH(ctx, join_count_kernel, grid, 256, 0, jp, n, links, 0, 0, counts.as<int>());
+        TG_TRY(tg_exclusive_sum(ctx, counts.as<int>(), offsets.as<long long>(), n + 1));
+        int64_t m = 0;
+        TG_TRY(tg_read_i64(ctx, offsets.as<long long>() + n, &m));
+        if (m > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "join candidates of one probe page exceed 2^31-1 rows");
+        DevBuf pp, pb, verdict;
+        TG_TRY(pp.alloc(ctx, (size_t)m * 4));
+        TG_TRY(pb.alloc(ctx, (size_t)m * 4));
+        TG_TRY(verdict.alloc(ctx, (size_t)m));
+        if (m > 0) {
+            TG_LAUNCH(ctx, join_fill_kernel, grid, 256, 0, jp, n, links, 0, 0, offsets.as<long long>(), pp.as<int>(), pb.as<int>());
+            long long m_arg = m;
+            const int* pp_arg = pp.as<int>();
+            const int* pb_arg = pb.as<int>();
+            unsigned char* v_arg = verdict.as<unsigned char>();
+            if (jit_jf_pairs) {
+                void* params[5] = {&cols, &m_arg, &pp_arg, &pb_arg, &v_arg};
+                TG_TRY(tg::jit_launch(ctx, jit_jf_pairs, tg_grid(ctx, m, JF_THREADS, tg::jit_blocks_per_sm(jit_jf_pairs, JF_THREADS, 0)), JF_THREADS, 0, params));
+            }
+            else TG_LAUNCH(ctx, join_filter_pairs_kernel, tg_grid(ctx, m, JF_THREADS, 8), JF_THREADS, 0, lookup->d_filter.as<DProgram>(), cols,
+                           lookup->num_build_channels, m, pp_arg, pb_arg, verdict.as<uint8_t>());
+        }
+        unsigned int* d_err = ctx->d_scratch->join_filter_flags;
+        TG_CUDA(ctx, cudaMemsetAsync(d_err, 0, 8, ctx->stream));
+        DevBuf out_counts, out_off;
+        TG_TRY(out_counts.alloc(ctx, (size_t)(n + 1) * 4));
+        TG_TRY(out_off.alloc(ctx, (size_t)(n + 1) * 8));
+        TG_LAUNCH(ctx, join_filter_select_kernel, tg_grid(ctx, n, 256, 8), 256, 0, offsets.as<long long>(), n, single_match, outer ? 1 : 0, verdict.as<uint8_t>(),
+                  out_counts.as<int>(), d_err);
+        TG_TRY(tg_exclusive_sum(ctx, out_counts.as<int>(), out_off.as<long long>(), n + 1));
+        TG_TRY(raise_filter_errors());
+        TG_TRY(tg_read_i64(ctx, out_off.as<long long>() + n, total));
+        if (*total == 0) return TGPU_OK;
+        if (*total > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "join output of one probe page exceeds 2^31-1 rows");
+        TG_TRY(out_probe->alloc(ctx, (size_t)*total * 4));
+        TG_TRY(out_build->alloc(ctx, (size_t)*total * 4));
+        TG_LAUNCH(ctx, join_filter_fill_kernel, tg_grid(ctx, n, 256, 8), 256, 0, offsets.as<long long>(), n, verdict.as<uint8_t>(), pb.as<int>(), outer ? 1 : 0,
+                  out_off.as<long long>(), out_probe->as<int>(), out_build->as<int>());
+        return TGPU_OK;
+    }
 
     int upload_absent(const tgpu_page* page, DevPage* in)
     {
@@ -2134,7 +2451,9 @@ struct JoinProbeOp : tgpu_op {
         const DevColumn& key = in.cols[key_channels[0]];
         if (!lookup->generic && key_channels.size() != 1) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "probe has %zu join channels, build has 1", key_channels.size());
         const bool tracking = join_type == TGPU_JOIN_LOOKUP_OUTER || join_type == TGPU_JOIN_FULL_OUTER;
-        if (!lookup->generic && !tracking && !getenv("TGPU_JOIN_GENERAL_PATH")) {
+        DColumns fcols;
+        if (lookup->has_filter) TG_TRY(filter_columns(in, &fcols));
+        if (!lookup->generic && !tracking && !lookup->has_filter && !getenv("TGPU_JOIN_GENERAL_PATH")) {
             bool handled = false;
             TG_TRY(fast_path(in, key, n, &handled));
             if (handled) return lazy ? complete_fast(page) : TGPU_OK;   // host buffers are the caller's again after this call
@@ -2151,15 +2470,22 @@ struct JoinProbeOp : tgpu_op {
         else TG_TRY(lookup_positions(ctx, lookup, key, jp->as<int>()));
         bool outer = join_type == TGPU_JOIN_PROBE_OUTER || join_type == TGPU_JOIN_FULL_OUTER;
         const int* links = lookup->has_dups ? lookup->links.as<int>() : nullptr;
+        // a join filter without position links only drops candidates: the expansion below then runs as without a filter
+        if (lookup->has_filter && !links) TG_TRY(filter_positions(fcols, jp->as<int>(), n));
+        const bool filtered_pairs = lookup->has_filter && links;
+        DevBuf out_probe, out_build;
         // match counts -> exclusive scan -> output offsets
         DevBuf counts, offsets;
-        TG_TRY(counts.alloc(ctx, (size_t)(n + 1) * 4));
-        TG_TRY(offsets.alloc(ctx, (size_t)(n + 1) * 8));
         int grid = tg_grid(ctx, n, 256 * 4, 8);
-        TG_LAUNCH(ctx, join_count_kernel, grid, 256, 0, jp->as<int>(), n, links, single_match, outer ? 1 : 0, counts.as<int>());
-        TG_TRY(tg_exclusive_sum(ctx, counts.as<int>(), offsets.as<long long>(), n + 1));
         int64_t total = 0;
-        TG_TRY(tg_read_i64(ctx, offsets.as<long long>() + n, &total));
+        if (filtered_pairs) TG_TRY(filter_pairs(fcols, jp->as<int>(), n, links, outer, &out_probe, &out_build, &total));
+        else {
+            TG_TRY(counts.alloc(ctx, (size_t)(n + 1) * 4));
+            TG_TRY(offsets.alloc(ctx, (size_t)(n + 1) * 8));
+            TG_LAUNCH(ctx, join_count_kernel, grid, 256, 0, jp->as<int>(), n, links, single_match, outer ? 1 : 0, counts.as<int>());
+            TG_TRY(tg_exclusive_sum(ctx, counts.as<int>(), offsets.as<long long>(), n + 1));
+            TG_TRY(tg_read_i64(ctx, offsets.as<long long>() + n, &total));
+        }
         if (total == 0) return TGPU_OK;
         if (total > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "join output of one probe page exceeds 2^31-1 rows");
 
@@ -2167,19 +2493,20 @@ struct JoinProbeOp : tgpu_op {
         outp.rows = total;
         // every probe row produced exactly one row and there are no chains: probe rows map 1:1
         // (LookupJoinPageBuilder.build :144-150 "outputProbeBlocksDirectly")
-        bool identity = (total == n) && (!links || single_match);
+        bool identity = !filtered_pairs && (total == n) && (!links || single_match);
         const int* build_idx = nullptr;
         bool build_may_be_null = outer;
-        DevBuf out_probe, out_build;
         if (identity) {
             for (int32_t ch : output_channels) outp.cols.push_back(in.cols[ch]);   // shares ownership, no copy
             build_idx = jp->as<int>();
         }
         else {
-            TG_TRY(out_probe.alloc(ctx, (size_t)total * 4));
-            TG_TRY(out_build.alloc(ctx, (size_t)total * 4));
-            TG_LAUNCH(ctx, join_fill_kernel, grid, 256, 0, jp->as<int>(), n, links, single_match, outer ? 1 : 0, offsets.as<long long>(),
-                      out_probe.as<int>(), out_build.as<int>());
+            if (!filtered_pairs) {
+                TG_TRY(out_probe.alloc(ctx, (size_t)total * 4));
+                TG_TRY(out_build.alloc(ctx, (size_t)total * 4));
+                TG_LAUNCH(ctx, join_fill_kernel, grid, 256, 0, jp->as<int>(), n, links, single_match, outer ? 1 : 0, offsets.as<long long>(),
+                          out_probe.as<int>(), out_build.as<int>());
+            }
             for (int32_t ch : output_channels) {
                 DevColumn c;
                 TG_TRY(tg_gather_column(ctx, in.cols[ch], out_probe.as<int>(), total, false, &c));
@@ -2409,6 +2736,34 @@ extern "C" int tgpu_join_build_create(tgpu_ctx* ctx, const tgpu_join_build_spec*
     return TGPU_OK;
 }
 
+extern "C" int tgpu_join_build_create_filtered(tgpu_ctx* ctx, const tgpu_join_build_spec* spec, const tgpu_expr_program* filter, int32_t num_build_channels,
+                                               tgpu_op** out)
+{
+    if (!ctx || !spec || !filter || !out) return TGPU_ERR_INVALID_ARGUMENT;
+    DProgram prog;
+    TG_TRY(join_filter_compile(ctx, filter, num_build_channels, &prog));
+    std::vector<int32_t> used;
+    for (int i = 0; i < prog.num_filter_insns; i++) {
+        const tg::DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
+        for (auto* o : ops)
+            if (o->kind == TGPU_OPND_COLUMN && std::find(used.begin(), used.end(), o->index) == used.end()) used.push_back(o->index);
+    }
+    std::sort(used.begin(), used.end());
+    tgpu_op* base = nullptr;
+    TG_TRY(tgpu_join_build_create(ctx, spec, &base));
+    std::unique_ptr<JoinBuildOp> op(static_cast<JoinBuildOp*>(base));
+    for (int32_t ch : used) {
+        if (ch >= num_build_channels) continue;
+        if (op->kept_at(ch) == (size_t)-1) op->extra_channels.push_back(ch);
+    }
+    op->has_filter = true;
+    op->filter = prog;
+    op->num_build_channels = num_build_channels;
+    op->filter_channels = used;
+    *out = op.release();
+    return TGPU_OK;
+}
+
 extern "C" int tgpu_join_build_get_lookup(tgpu_op* build, tgpu_lookup** out)
 {
     JoinBuildOp* op = dynamic_cast<JoinBuildOp*>(build);
@@ -2433,7 +2788,7 @@ extern "C" int64_t tgpu_lookup_position_count(const tgpu_lookup* lookup) { retur
 extern "C" int64_t tgpu_lookup_memory_bytes(const tgpu_lookup* lookup)
 {
     if (!lookup) return 0;
-    int64_t b = (int64_t)lookup->table.bytes + (int64_t)lookup->links.bytes + lookup->store.memory_bytes();
+    int64_t b = (int64_t)lookup->table.bytes + (int64_t)lookup->links.bytes + lookup->store.memory_bytes() + lookup->filter_extra_bytes;
     for (auto& s : lookup->by_slot) b += (int64_t)s.bytes;
     b += (int64_t)lookup->wide.bytes + (int64_t)lookup->keyed.bytes;
     return b;
@@ -2480,6 +2835,7 @@ extern "C" int tgpu_semi_join_create(tgpu_ctx* ctx, tgpu_lookup* lookup, int32_t
     if (!ctx || !lookup || !out) return TGPU_ERR_INVALID_ARGUMENT;
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
     if (lookup->generic && lookup->build_keys.size() != 1) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a semi-join set has one channel");
+    if (lookup->has_filter) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a semi-join set (ChannelSet) has no join filter");
     TG_TRY(lookup_count_null_keys(ctx, lookup));
     TG_TRY(lookup_count_nan_keys(ctx, lookup));
     SemiJoinOp* op = new SemiJoinOp(ctx, lookup);
@@ -2576,5 +2932,33 @@ extern "C" int tgpu_lookup_copy_position_links(tgpu_ctx* ctx, const tgpu_lookup*
     }
     TG_CUDA(ctx, cudaMemcpyAsync(out_links_host, lookup->links.p, (size_t)lookup->positions * 4, cudaMemcpyDeviceToHost, ctx->stream));
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return TGPU_OK;
+}
+
+extern "C" int tgpu_jit_selftest_join_filter(const tgpu_expr_program* program, int32_t num_build_channels, const int32_t* channel_types, int32_t num_channels,
+                                             uint32_t nullable_mask, int64_t* cubin_bytes, char* source_out, int64_t source_cap)
+{
+    if (!program || !channel_types || !cubin_bytes || num_channels < 0) return TGPU_ERR_INVALID_ARGUMENT;
+    tgpu_ctx fake;
+    DProgram prog;
+    int st = join_filter_compile(&fake, program, num_build_channels, &prog);
+    if (st != TGPU_OK) return st;
+    for (int i = 0; i < prog.num_filter_insns; i++) {
+        const tg::DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
+        for (auto* o : ops)
+            if (o->kind == TGPU_OPND_COLUMN && o->index >= num_channels) return TGPU_ERR_INVALID_ARGUMENT;     // outside the layout
+    }
+    int elems[TGPU_MAX_CHANNELS] = {0};
+    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
+        DevColumn col;
+        col.type = channel_types[c];
+        elems[c] = col.elem_size();
+    }
+    std::string src = gen_join_filter_source(prog, num_build_channels, elems, std::min<int32_t>(num_channels, TGPU_MAX_CHANNELS), nullable_mask);
+    if (source_out && source_cap > 0) { strncpy(source_out, src.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
+    std::string cubin;
+    st = tg::jit_compile_cubin(&fake, src, &cubin);
+    if (st != TGPU_OK) { if (source_out && source_cap > 0) { strncpy(source_out, fake.err.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; } return st; }
+    *cubin_bytes = (int64_t)cubin.size();
     return TGPU_OK;
 }

@@ -733,17 +733,29 @@ class HashBuilderOperator(Operator):
 
 
 class HashBuilderOperatorFactory(OperatorFactory):
-    def __init__(self, ctx, bridge, hash_channels, output_channels, expected_positions=10_000):
+    def __init__(self, ctx, bridge, hash_channels, output_channels, expected_positions=10_000, filter=None, num_build_channels=None):
+        """filter: the join filter function (filterFunctionFactory) as an expression tree over the join-sources layout - build channels
+        0 .. num_build_channels-1, then the probe channels; num_build_channels = buildLayout.size(), required with a filter"""
         super().__init__()
         self.ctx, self.bridge = ctx, bridge
         self.hash_channels, self.output_channels, self.expected_positions = list(hash_channels), list(output_channels), expected_positions
+        self.filter, self.num_build_channels = filter, num_build_channels
+        self.filter_program = None
+        if filter is not None:
+            if num_build_channels is None:
+                raise ValueError("a join filter needs num_build_channels (the build layout's size)")
+            self.filter_program = PageProcessorProgram(filter, [])
 
     def _create(self):
         kc, oc = _i32(self.hash_channels), _i32(self.output_channels)
         spec = abi.JoinBuildSpec(len(self.hash_channels), C.cast(kc, C.POINTER(C.c_int32)), len(self.output_channels),
                                  C.cast(oc, C.POINTER(C.c_int32)), self.expected_positions)
         h = C.c_void_p()
-        self.ctx.check(self.ctx.lib.tgpu_join_build_create(self.ctx.h, C.byref(spec), C.byref(h)))
+        if self.filter_program is None:
+            self.ctx.check(self.ctx.lib.tgpu_join_build_create(self.ctx.h, C.byref(spec), C.byref(h)))
+        else:
+            self.ctx.check(self.ctx.lib.tgpu_join_build_create_filtered(self.ctx.h, C.byref(spec), C.byref(self.filter_program.struct),
+                                                                         int(self.num_build_channels), C.byref(h)))
         return HashBuilderOperator(self.ctx, h, self.bridge)
 
     def duplicate(self):
