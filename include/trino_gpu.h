@@ -149,10 +149,18 @@ typedef enum tgpu_expr_op {
     TGPU_EX_BETWEEN = 25,          /* a BETWEEN b AND c: c in operand `c` */
     TGPU_EX_CAST_BIGINT_TO_DOUBLE = 30,
     TGPU_EX_CAST_DOUBLE_TO_BIGINT = 31, /* Math.round semantics, range-checked (M/type/DoubleOperators.java) */
-    TGPU_EX_IN = 40                /* a IN (const list): b.imm = index into in_lists, all operands of `vtype` */
+    TGPU_EX_IN = 40,               /* a IN (const list): b.imm = index into in_lists, all operands of `vtype`.  Under
+                                      TGPU_V_VARCHAR the list's values are indices into `strings`                      */
+    TGPU_EX_LIKE = 41              /* a LIKE like_patterns[b.imm] (LikeFunctions.likeVarchar, M/type/LikeFunctions.java:49-56, over
+                                      LikeMatcher.compile(pattern, escape) with optimize = true): BOOLEAN, vtype TGPU_V_VARCHAR */
 } tgpu_expr_op;
 
-typedef enum tgpu_vtype { TGPU_V_BIGINT = 0, TGPU_V_DOUBLE = 1, TGPU_V_BOOLEAN = 2 } tgpu_vtype;
+/* TGPU_V_VARCHAR is an OPERAND type only: =, <>, <, <=, >, >=, BETWEEN, IN, IS [NOT] NULL and LIKE read it and give BOOLEAN; no
+ * instruction produces a string.  A VARCHAR operand is a TGPU_OPND_COLUMN naming a TGPU_UTF8 channel (the bytes between offsets[i]
+ * and offsets[i+1]), a TGPU_OPND_CONST whose imm indexes `strings`, or TGPU_OPND_NULL; a VARCHAR TGPU_OPND_TEMP is INVALID_ARGUMENT.
+ * Equality is bytewise; order is Slice.compareTo (unsigned bytes, a proper prefix first: S/type/AbstractVariableWidthType.java:403-410).
+ * CHAR(n) (padded comparison and LIKE) is not covered: keep Java for it. */
+typedef enum tgpu_vtype { TGPU_V_BIGINT = 0, TGPU_V_DOUBLE = 1, TGPU_V_BOOLEAN = 2, TGPU_V_VARCHAR = 3 } tgpu_vtype;
 typedef enum tgpu_operand_kind { TGPU_OPND_NONE = 0, TGPU_OPND_COLUMN = 1, TGPU_OPND_TEMP = 2, TGPU_OPND_CONST = 3, TGPU_OPND_NULL = 4 } tgpu_operand_kind;
 
 typedef struct tgpu_operand {
@@ -175,6 +183,24 @@ typedef struct tgpu_expr_insn {
 
 typedef struct tgpu_in_list { int32_t count; const int64_t* values; /* raw bits for DOUBLE */ } tgpu_in_list;
 
+/* a byte string in host memory (UTF-8 for patterns and escapes) */
+typedef struct tgpu_bytes {
+    int32_t length;
+    const uint8_t* data;
+} tgpu_bytes;
+
+/* the constant pattern of a LIKE: compiled once at create.  An invalid escape use, an escape of more than one character, a pattern that
+   is not UTF-8 or one past the device limits answers TGPU_ERR_NOT_SUPPORTED at create, so the Java operator keeps the expression and
+   raises where the reference raises. */
+typedef struct tgpu_like_pattern {
+    tgpu_bytes pattern;
+    tgpu_bytes escape;                    /* length 0 = no ESCAPE */
+} tgpu_like_pattern;
+
+#define TGPU_MAX_STRINGS 128              /* string pool entries, holding at most TGPU_MAX_STRING_BYTES bytes in all */
+#define TGPU_MAX_STRING_BYTES 4096
+#define TGPU_MAX_LIKE_PATTERNS 8          /* each with at most 64 matcher states and 1024 pattern bytes */
+
 typedef struct tgpu_projection {
     int32_t kind;        /* 0 = pass an input channel through (any type incl. UTF8/DICT/RLE, like InputPageProjection);
                             1 = computed: value of temp `index` after the program ran */
@@ -194,6 +220,14 @@ typedef struct tgpu_expr_program {
     const tgpu_projection* projections;
     int32_t num_in_lists;
     const tgpu_in_list* in_lists;
+    /* VARCHAR constants (TGPU_OPND_CONST imm and VARCHAR IN-list values index `strings`) and LIKE patterns (TGPU_EX_LIKE b.imm indexes
+       `like_patterns`).  A zeroed tail means no strings.  Past TGPU_MAX_STRINGS / TGPU_MAX_STRING_BYTES / TGPU_MAX_LIKE_PATTERNS:
+       TGPU_ERR_NOT_SUPPORTED.  Only tgpu_filter_project_create evaluates string operations; the fused aggregation pre-stage and join
+       filters answer TGPU_ERR_NOT_SUPPORTED at create for a program that uses TGPU_V_VARCHAR or TGPU_EX_LIKE. */
+    int32_t num_strings;
+    const tgpu_bytes* strings;
+    int32_t num_like_patterns;
+    const tgpu_like_pattern* like_patterns;
 } tgpu_expr_program;
 
 /* FilterAndProjectOperator (M/operator/FilterAndProjectOperator.java:60-95) over a PageProcessor

@@ -46,6 +46,19 @@ public final class NativeSpecs
     static final StructLayout PARTITION_SPEC = MemoryLayout.structLayout(
             JAVA_INT, MemoryLayout.paddingLayout(4), ADDRESS, JAVA_INT, MemoryLayout.paddingLayout(4), ADDRESS, JAVA_INT, JAVA_INT,
             JAVA_INT, MemoryLayout.paddingLayout(4), ADDRESS);
+    // tgpu_bytes { int32 length; (pad); uint8* data }
+    static final StructLayout BYTES = MemoryLayout.structLayout(JAVA_INT.withName("length"), MemoryLayout.paddingLayout(4), ADDRESS.withName("data"));
+    // tgpu_like_pattern { tgpu_bytes pattern; tgpu_bytes escape /* length 0 = no ESCAPE */ }: a `$like` whose `$like_pattern` argument is a constant
+    static final StructLayout LIKE_PATTERN = MemoryLayout.structLayout(BYTES.withName("pattern"), BYTES.withName("escape"));
+    // tgpu_expr_program { int32 num_insns; (pad); tgpu_expr_insn* insns; int32 filter_temp; int32 num_filter_insns; int32 num_projections; (pad);
+    //                     tgpu_projection* projections; int32 num_in_lists; (pad); tgpu_in_list* in_lists; int32 num_strings; (pad); tgpu_bytes* strings;
+    //                     int32 num_like_patterns; (pad); tgpu_like_pattern* like_patterns }  (88 bytes; the last four fields zero = no strings)
+    static final StructLayout EXPR_PROGRAM = MemoryLayout.structLayout(
+            JAVA_INT.withName("num_insns"), MemoryLayout.paddingLayout(4), ADDRESS.withName("insns"),
+            JAVA_INT.withName("filter_temp"), JAVA_INT.withName("num_filter_insns"), JAVA_INT.withName("num_projections"), MemoryLayout.paddingLayout(4),
+            ADDRESS.withName("projections"), JAVA_INT.withName("num_in_lists"), MemoryLayout.paddingLayout(4), ADDRESS.withName("in_lists"),
+            JAVA_INT.withName("num_strings"), MemoryLayout.paddingLayout(4), ADDRESS.withName("strings"),
+            JAVA_INT.withName("num_like_patterns"), MemoryLayout.paddingLayout(4), ADDRESS.withName("like_patterns"));
     public static final int PARTITION_HASH_BUCKET = 0;    // HashBucketFunction (M/sql/planner/HashBucketFunction.java:43-46)
     public static final int PARTITION_LOCAL = 1;          // LocalPartitionGenerator (M/operator/exchange/LocalPartitionGenerator.java:45-77)
 

@@ -23,8 +23,9 @@ PAGE_DEVICE = 1
 EX_MOV, EX_ADD, EX_SUB, EX_MUL, EX_DIV, EX_MOD, EX_NEG = 0, 1, 2, 3, 4, 5, 6
 EX_EQ, EX_NE, EX_LT, EX_LE, EX_GT, EX_GE = 10, 11, 12, 13, 14, 15
 EX_AND, EX_OR, EX_NOT, EX_IS_NULL, EX_IS_NOT_NULL, EX_BETWEEN = 20, 21, 22, 23, 24, 25
-EX_CAST_BIGINT_TO_DOUBLE, EX_CAST_DOUBLE_TO_BIGINT, EX_IN = 30, 31, 40
-V_BIGINT, V_DOUBLE, V_BOOLEAN = 0, 1, 2
+EX_CAST_BIGINT_TO_DOUBLE, EX_CAST_DOUBLE_TO_BIGINT, EX_IN, EX_LIKE = 30, 31, 40, 41
+V_BIGINT, V_DOUBLE, V_BOOLEAN, V_VARCHAR = 0, 1, 2, 3
+MAX_STRINGS, MAX_STRING_BYTES, MAX_LIKE_PATTERNS = 128, 4096, 8
 OPND_NONE, OPND_COLUMN, OPND_TEMP, OPND_CONST, OPND_NULL = 0, 1, 2, 3, 4
 
 AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_SUM_DECIMAL, AGG_AVG_DECIMAL = 0, 1, 2, 3, 4, 5, 6, 7
@@ -76,6 +77,14 @@ class InList(C.Structure):
     _fields_ = [("count", C.c_int32), ("values", C.POINTER(C.c_int64))]
 
 
+class Bytes(C.Structure):
+    _fields_ = [("length", C.c_int32), ("data", C.c_void_p)]
+
+
+class LikePattern(C.Structure):
+    _fields_ = [("pattern", Bytes), ("escape", Bytes)]
+
+
 class Projection(C.Structure):
     _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("vtype", C.c_int32)]
 
@@ -90,6 +99,10 @@ class ExprProgram(C.Structure):
         ("projections", C.POINTER(Projection)),
         ("num_in_lists", C.c_int32),
         ("in_lists", C.POINTER(InList)),
+        ("num_strings", C.c_int32),
+        ("strings", C.POINTER(Bytes)),
+        ("num_like_patterns", C.c_int32),
+        ("like_patterns", C.POINTER(LikePattern)),
     ]
 
 

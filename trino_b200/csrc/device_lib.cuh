@@ -39,9 +39,9 @@ enum {
     TGD_EX_MOV = 0, TGD_EX_ADD = 1, TGD_EX_SUB = 2, TGD_EX_MUL = 3, TGD_EX_DIV = 4, TGD_EX_MOD = 5, TGD_EX_NEG = 6,
     TGD_EX_EQ = 10, TGD_EX_NE = 11, TGD_EX_LT = 12, TGD_EX_LE = 13, TGD_EX_GT = 14, TGD_EX_GE = 15,
     TGD_EX_AND = 20, TGD_EX_OR = 21, TGD_EX_NOT = 22, TGD_EX_IS_NULL = 23, TGD_EX_IS_NOT_NULL = 24, TGD_EX_BETWEEN = 25,
-    TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_IN = 40
+    TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_IN = 40, TGD_EX_LIKE = 41
 };
-enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2 };
+enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2, TGD_V_VARCHAR = 3 };
 enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4 };
 
 enum AccKind {
@@ -75,7 +75,203 @@ struct OutCols {
     uint8_t* pass_nullmap[TGD_MAX_CHANNELS];
 };
 
+// ---- VARCHAR operands of FilterAndProject programs ------------------------------------------------------------------------
+// The UTF8 channels a program's string operations read, in slots: slot k is channel DProgram::str_channel[k].  Kept apart from
+// ColRef / DColumns, which every kernel of the library takes by value.
+#define TGD_MAX_STR_CHANNELS 8
+struct StrCols {
+    const int32_t* offsets[TGD_MAX_STR_CHANNELS];
+    const uint8_t* bytes[TGD_MAX_STR_CHANNELS];
+};
+
+// A constant LIKE pattern as LikeMatcher.compile(pattern, escape, optimize = true) leaves it (M/likematcher/LikeMatcher.java:58-153):
+// length bounds, a constant prefix and suffix, and a matcher for the middle.  FJS: literal terms found in order (bytewise);
+// DFA: the byte-level automaton of DenseDfaMatcher (`_` and `%` consume whole, well-formed UTF-8 sequences); NFA: NfaMatcher, whose `_`
+// consumes one decoded code point and whose literals are UTF-16 code units.  DFA and NFA run as one 64-bit mask of positions:
+// position p is followed by `_` (any_mask), by a literal (lit_pos / lit_val), and may carry a `%` loop (loop_mask); `accept` is the last.
+enum { TGD_LIKE_NONE = 0, TGD_LIKE_FJS = 1, TGD_LIKE_DFA = 2, TGD_LIKE_NFA = 3 };
+#define TGD_LIKE_BYTES 1024
+#define TGD_LIKE_TERMS 32
+#define TGD_LIKE_LITS 64
+struct DLike {
+    int32_t min_size, max_size;                // max_size < 0: unbounded
+    int32_t prefix_len, suffix_len;            // bytes[0, prefix_len) and bytes[prefix_len, prefix_len + suffix_len)
+    int32_t kind;                              // TGD_LIKE_*
+    int32_t exact;                             // the middle must match to its end
+    int32_t num_terms;                         // FJS
+    int32_t accept;                            // DFA / NFA
+    int32_t num_lits;
+    int32_t pad;
+    unsigned long long any_mask, loop_mask;
+    int32_t term_off[TGD_LIKE_TERMS], term_len[TGD_LIKE_TERMS];
+    int32_t lit_pos[TGD_LIKE_LITS], lit_val[TGD_LIKE_LITS];
+    uint8_t bytes[TGD_LIKE_BYTES];
+};
+
 #if defined(__CUDACC__)
+
+struct StrRef {
+    const uint8_t* p;
+    int32_t len;
+};
+
+__device__ __forceinline__ StrRef tg_str(const StrCols& s, int slot, int64_t row)
+{
+    const int32_t b = s.offsets[slot][row], e = s.offsets[slot][row + 1];
+    return StrRef{s.bytes[slot] + b, e - b};
+}
+
+// the n (<= 8) bytes at p as a little-endian word, zero above them.  Only the aligned 8-byte words that hold one of the n bytes are
+// read (one, or two joined by a shift), so a string at the very end of its buffer is never read past the word it ends in.
+__device__ __forceinline__ unsigned long long tg_ld_bytes(const uint8_t* p, int n)
+{
+    if (n <= 0) return 0ULL;
+    const unsigned long long a = (unsigned long long)p;
+    const unsigned long long* w = (const unsigned long long*)(a & ~7ULL);
+    const int sh = (int)(a & 7ULL);
+    unsigned long long v = __ldg(w) >> (sh * 8);
+    if (sh + n > 8) v |= __ldg(w + 1) << ((8 - sh) * 8);
+    return n >= 8 ? v : v & ((1ULL << (n * 8)) - 1ULL);
+}
+
+__device__ __forceinline__ unsigned long long tg_bswap64(unsigned long long x)
+{
+    const unsigned int lo = (unsigned int)x, hi = (unsigned int)(x >> 32);
+    return ((unsigned long long)__byte_perm(lo, 0, 0x0123) << 32) | __byte_perm(hi, 0, 0x0123);
+}
+
+__device__ __forceinline__ bool tg_str_eq(StrRef a, StrRef b)
+{
+    if (a.len != b.len) return false;
+    for (int i = 0; i < a.len; i += 8) {
+        const int n = a.len - i < 8 ? a.len - i : 8;
+        if (tg_ld_bytes(a.p + i, n) != tg_ld_bytes(b.p + i, n)) return false;
+    }
+    return true;
+}
+
+// Slice.compareTo: unsigned bytes, lexicographic, a proper prefix first.  Byte-swapped 8-byte words compare as unsigned integers.
+__device__ __forceinline__ int tg_str_cmp(StrRef a, StrRef b)
+{
+    const int m = a.len < b.len ? a.len : b.len;
+    for (int i = 0; i < m; i += 8) {
+        const int n = m - i < 8 ? m - i : 8;
+        const unsigned long long x = tg_bswap64(tg_ld_bytes(a.p + i, n)), y = tg_bswap64(tg_ld_bytes(b.p + i, n));
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return a.len < b.len ? -1 : a.len > b.len ? 1 : 0;
+}
+
+__device__ __forceinline__ bool tg_str_cmp_op(int op, StrRef a, StrRef b)
+{
+    if (op == TGD_EX_EQ) return tg_str_eq(a, b);
+    if (op == TGD_EX_NE) return !tg_str_eq(a, b);
+    const int c = tg_str_cmp(a, b);
+    switch (op) {
+        case TGD_EX_LT: return c < 0;
+        case TGD_EX_LE: return c <= 0;
+        case TGD_EX_GT: return c > 0;
+        default: return c >= 0;
+    }
+}
+
+__device__ __forceinline__ bool tg_bytes_eq(const uint8_t* p, const uint8_t* q, int n)
+{
+    for (int i = 0; i < n; i++)
+        if (p[i] != q[i]) return false;
+    return true;
+}
+
+// FjsMatcher: every term, in order, at its leftmost occurrence after the previous one
+__device__ __forceinline__ bool tg_like_fjs(const DLike& L, const uint8_t* p, int len)
+{
+    int start = 0;
+    for (int t = 0; t < L.num_terms; t++) {
+        const uint8_t* term = L.bytes + L.term_off[t];
+        const int tl = L.term_len[t];
+        if (start == len) return false;
+        int at = -1;
+        for (int i = start; i + tl <= len; i++)
+            if (p[i] == term[0] && tg_bytes_eq(p + i + 1, term + 1, tl - 1)) { at = i; break; }
+        if (at < 0) return false;
+        start = at + tl;
+    }
+    return !L.exact || start == len;
+}
+
+// positions followed by a literal equal to v
+__device__ __forceinline__ unsigned long long tg_like_lits(const DLike& L, int v)
+{
+    unsigned long long m = 0;
+    for (int k = 0; k < L.num_lits; k++)
+        if (L.lit_val[k] == v) m |= 1ULL << L.lit_pos[k];
+    return m;
+}
+
+// DenseDfaMatcher's language, simulated over bytes: D = positions reached, P1..P3 = positions reached once 1..3 more continuation bytes
+// (10xxxxxx) complete the UTF-8 sequence a `_` or a `%` is consuming
+__device__ __forceinline__ bool tg_like_dfa(const DLike& L, const uint8_t* p, int len)
+{
+    const unsigned long long acc = 1ULL << L.accept;
+    unsigned long long D = 1, P1 = 0, P2 = 0, P3 = 0;
+    for (int i = 0; i < len; i++) {
+        const int b = p[i];
+        const unsigned long long step = ((D & L.any_mask) << 1) | (D & L.loop_mask);
+        unsigned long long nd = (D & tg_like_lits(L, b)) << 1, n1 = 0, n2 = 0, n3 = 0;
+        if (b < 0x80) nd |= step;
+        else if (b < 0xC0) { nd |= P1; n1 = P2; n2 = P3; }
+        else if (b < 0xE0) n1 = step;
+        else if (b < 0xF0) n2 = step;
+        else if (b < 0xF8) n3 = step;
+        D = nd; P1 = n1; P2 = n2; P3 = n3;
+        if ((D | P1 | P2 | P3) == 0) return false;
+        if (!L.exact && (D & acc)) return true;
+    }
+    return (D & acc) != 0;
+}
+
+// NfaMatcher: code points decoded as it decodes them (lead byte and length only; a truncated or stray byte fails the match)
+__device__ __forceinline__ bool tg_like_nfa(const DLike& L, const uint8_t* p, int len)
+{
+    const unsigned long long acc = 1ULL << L.accept;
+    unsigned long long D = 1;
+    int i = 0;
+    while (i < len) {
+        const int h = p[i];
+        int cp;
+        if (h < 0x80) { cp = h; i += 1; }
+        else if ((h & 0xE0) == 0xC0 && i + 1 < len) { cp = ((h & 0x1F) << 6) | (p[i + 1] & 0x3F); i += 2; }
+        else if ((h & 0xF0) == 0xE0 && i + 2 < len) { cp = ((h & 0x0F) << 12) | ((p[i + 1] & 0x3F) << 6) | (p[i + 2] & 0x3F); i += 3; }
+        else if ((h & 0xF8) == 0xF0 && i + 3 < len) {
+            cp = ((h & 0x07) << 18) | ((p[i + 1] & 0x3F) << 12) | ((p[i + 2] & 0x3F) << 6) | (p[i + 3] & 0x3F);
+            i += 4;
+        }
+        else return false;
+        D = ((D & (L.any_mask | tg_like_lits(L, cp))) << 1) | (D & L.loop_mask);
+        if (D == 0) return false;
+        if (!L.exact && (D & acc)) return true;
+    }
+    return (D & acc) != 0;
+}
+
+__device__ __forceinline__ bool tg_like_middle(const DLike& L, const uint8_t* p, int len)
+{
+    switch (L.kind) {
+        case TGD_LIKE_FJS: return tg_like_fjs(L, p, len);
+        case TGD_LIKE_DFA: return tg_like_dfa(L, p, len);
+        case TGD_LIKE_NFA: return tg_like_nfa(L, p, len);
+        default: return true;
+    }
+}
+
+// LikeMatcher.match (M/likematcher/LikeMatcher.java:160-183)
+__device__ __forceinline__ bool tg_like(const DLike& L, StrRef s)
+{
+    if (s.len < L.min_size || (L.max_size >= 0 && s.len > L.max_size)) return false;
+    if (!tg_bytes_eq(s.p, L.bytes, L.prefix_len)) return false;
+    if (!tg_bytes_eq(s.p + s.len - L.suffix_len, L.bytes + L.prefix_len, L.suffix_len)) return false;
+    return tg_like_middle(L, s.p + L.prefix_len, s.len - L.prefix_len - L.suffix_len);
+}
 
 __device__ __forceinline__ bool tg_valid(const uint8_t* validity, int64_t i)
 {
@@ -719,19 +915,19 @@ __device__ __forceinline__ void agg_general_body(P& prog, const DColumns& cols, 
 // of the chunk; a scan of the chunk counts gives every chunk its first output row.  Pass 2 ranks the selected rows of a tile
 // (ballot + a scan over the tile's (iteration, warp) cells), evaluates the projections and copies the pass-through channels
 // straight to output row chunk_off + rank: output order = input order (PageProcessor.java:302-336).
-// P supplies: static bool filter(cols, row, err*), static void row(cols, row, j, out, err*, nulls_seen*).
+// P supplies: static bool filter(cols, strs, row, err*), static void row(cols, strs, row, j, out, err*, nulls_seen*).
 constexpr int FPC_R = 4;          // tile = FPC_R x 256 rows
 constexpr int FPC_T = 256;
 
 template <class P>
-__device__ __forceinline__ void fp_filter_chunks_body(const DColumns& cols, long long n, long long chunk, unsigned char* __restrict__ flags,
+__device__ __forceinline__ void fp_filter_chunks_body(const DColumns& cols, const StrCols& strs, long long n, long long chunk, unsigned char* __restrict__ flags,
                                                       unsigned int* __restrict__ chunk_counts, unsigned int* __restrict__ err_out)
 {
     __shared__ unsigned int warp_sel[FPC_T / 32];
     const long long begin = (long long)blockIdx.x * chunk, end = begin + chunk < n ? begin + chunk : n;
     unsigned int err = 0, mine = 0;
     for (long long row = begin + threadIdx.x; row < end; row += FPC_T) {
-        bool s = P::filter(cols, row, &err);
+        bool s = P::filter(cols, strs, row, &err);
         flags[row] = s ? 1 : 0;
         mine += s ? 1u : 0u;
     }
@@ -747,7 +943,7 @@ __device__ __forceinline__ void fp_filter_chunks_body(const DColumns& cols, long
 }
 
 template <class P>
-__device__ __forceinline__ void fp_project_chunks_body(const DColumns& cols, const unsigned char* __restrict__ flags, long long n, long long chunk,
+__device__ __forceinline__ void fp_project_chunks_body(const DColumns& cols, const StrCols& strs, const unsigned char* __restrict__ flags, long long n, long long chunk,
                                                        const long long* __restrict__ chunk_off, const OutCols& out, unsigned int* __restrict__ err_out,
                                                        unsigned int* __restrict__ any_null)
 {
@@ -785,7 +981,7 @@ __device__ __forceinline__ void fp_project_chunks_body(const DColumns& cols, con
         for (int i = 0; i < FPC_R; i++) {
             if (!sel[i]) continue;
             long long row = tile + (long long)i * FPC_T + threadIdx.x;
-            P::row(cols, row, running + cells[i * NW + warp] + rank[i], out, &err, &nulls_seen);
+            P::row(cols, strs, row, running + cells[i * NW + warp] + rank[i], out, &err, &nulls_seen);
         }
         running += tile_total;
         __syncthreads();

@@ -7,7 +7,240 @@
 #include "expr.cuh"
 #include "jit.cuh"
 
+#include <algorithm>
+
 namespace tg {
+
+// strict UTF-8 -> UTF-16 code units (a Java String); false on malformed input
+static bool utf8_to_utf16(const tgpu_bytes& b, std::u16string* out)
+{
+    out->clear();
+    const uint8_t* p = b.data;
+    int i = 0;
+    while (i < b.length) {
+        const int h = p[i];
+        int n = h < 0x80 ? 0 : (h & 0xE0) == 0xC0 ? 1 : (h & 0xF0) == 0xE0 ? 2 : (h & 0xF8) == 0xF0 ? 3 : -1;
+        if (n < 0 || i + n >= b.length) return false;
+        uint32_t cp = n == 0 ? h : n == 1 ? (h & 0x1F) : n == 2 ? (h & 0x0F) : (h & 0x07);
+        for (int k = 1; k <= n; k++) {
+            if ((p[i + k] & 0xC0) != 0x80) return false;
+            cp = (cp << 6) | (p[i + k] & 0x3F);
+        }
+        static const uint32_t min_cp[4] = {0, 0x80, 0x800, 0x10000};
+        if (cp < min_cp[n] || cp > 0x10FFFF || (cp >= 0xD800 && cp <= 0xDFFF)) return false;
+        if (cp >= 0x10000) {
+            out->push_back((char16_t)(0xD800 + ((cp - 0x10000) >> 10)));
+            out->push_back((char16_t)(0xDC00 + ((cp - 0x10000) & 0x3FF)));
+        }
+        else out->push_back((char16_t)cp);
+        i += n + 1;
+    }
+    return true;
+}
+
+static void utf16_to_utf8(const std::u16string& s, std::string* out)
+{
+    out->clear();
+    for (size_t i = 0; i < s.size(); i++) {
+        uint32_t cp = s[i];
+        if (cp >= 0xD800 && cp <= 0xDBFF && i + 1 < s.size()) cp = 0x10000 + ((cp - 0xD800) << 10) + (s[++i] - 0xDC00);
+        if (cp < 0x80) *out += (char)cp;
+        else if (cp < 0x800) { *out += (char)(0xC0 | (cp >> 6)); *out += (char)(0x80 | (cp & 0x3F)); }
+        else if (cp < 0x10000) { *out += (char)(0xE0 | (cp >> 12)); *out += (char)(0x80 | ((cp >> 6) & 0x3F)); *out += (char)(0x80 | (cp & 0x3F)); }
+        else {
+            *out += (char)(0xF0 | (cp >> 18)); *out += (char)(0x80 | ((cp >> 12) & 0x3F));
+            *out += (char)(0x80 | ((cp >> 6) & 0x3F)); *out += (char)(0x80 | (cp & 0x3F));
+        }
+    }
+}
+
+struct LikeItem {
+    enum { LITERAL, ANY, ZERO_OR_MORE } kind;
+    std::u16string literal;
+    int count = 0;
+};
+
+// LikeMatcher.parse (M/likematcher/LikeMatcher.java:196-274); false where it throws (an invalid escape use)
+static bool like_parse(const std::u16string& pat, int escape, std::vector<LikeItem>* out)
+{
+    std::u16string literal;
+    int any = 0;
+    bool unbounded = false, in_escape = false;
+    auto flush_wild = [&] {
+        if (any) { out->push_back(LikeItem{LikeItem::ANY, {}, any}); any = 0; }
+        if (unbounded) { out->push_back(LikeItem{LikeItem::ZERO_OR_MORE, {}, 0}); unbounded = false; }
+    };
+    for (char16_t ch : pat) {
+        if (in_escape) {
+            if (ch != u'%' && ch != u'_' && (int)ch != escape) return false;
+            literal += ch;
+            in_escape = false;
+        }
+        else if (escape >= 0 && (int)ch == escape) {
+            in_escape = true;
+            flush_wild();
+        }
+        else if (ch == u'%' || ch == u'_') {
+            if (!literal.empty()) { out->push_back(LikeItem{LikeItem::LITERAL, literal, 0}); literal.clear(); }
+            if (ch == u'%') unbounded = true;
+            else any++;
+        }
+        else {
+            flush_wild();
+            literal += ch;
+        }
+    }
+    if (in_escape) return false;
+    if (!literal.empty()) out->push_back(LikeItem{LikeItem::LITERAL, literal, 0});
+    else flush_wild();
+    return true;
+}
+
+// LikeMatcher.compile(pattern, escape, optimize = true) into the device form (device_lib.cuh DLike)
+static int like_compile(tgpu_ctx* ctx, int idx, const tgpu_like_pattern& lp, DLike* L)
+{
+    memset(L, 0, sizeof(*L));
+    if (lp.pattern.length < 0 || (lp.pattern.length > 0 && !lp.pattern.data) || lp.escape.length < 0 || (lp.escape.length > 0 && !lp.escape.data))
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "LIKE pattern %d: bad byte string", idx);
+    std::u16string pat, esc;
+    if (!utf8_to_utf16(lp.pattern, &pat)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d is not UTF-8", idx);
+    if (!utf8_to_utf16(lp.escape, &esc)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE escape %d is not UTF-8", idx);
+    if (esc.size() > 1) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d: the escape is not a single character", idx);
+    std::vector<LikeItem> items;
+    if (!like_parse(pat, esc.empty() ? -1 : (int)esc[0], &items))
+        return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d: escape character must be followed by '%%', '_' or the escape character itself", idx);
+    std::vector<std::string> bytes(items.size());
+    int64_t min_size = 0, max_size = 0;
+    bool unbounded = false;
+    for (size_t i = 0; i < items.size(); i++) {
+        if (items[i].kind == LikeItem::LITERAL) {
+            utf16_to_utf8(items[i].literal, &bytes[i]);
+            min_size += (int64_t)bytes[i].size();
+            max_size += (int64_t)bytes[i].size();
+        }
+        else if (items[i].kind == LikeItem::ANY) { min_size += items[i].count; max_size += 4LL * items[i].count; }
+        else unbounded = true;
+    }
+    if (max_size > INT32_MAX) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d is past the device limits", idx);
+    L->min_size = (int32_t)min_size;
+    L->max_size = unbounded ? -1 : (int32_t)max_size;
+    int start = 0, end = (int)items.size() - 1;
+    std::string stored;
+    if (!items.empty() && items[0].kind == LikeItem::LITERAL) { stored += bytes[0]; L->prefix_len = (int32_t)bytes[0].size(); start++; }
+    if (items.size() > 1 && items.back().kind == LikeItem::LITERAL) { stored += bytes.back(); L->suffix_len = (int32_t)bytes.back().size(); end--; }
+    L->exact = 1;
+    if (start <= end && items[end].kind == LikeItem::ZERO_OR_MORE) { L->exact = 0; end--; }
+    L->kind = TGD_LIKE_NONE;
+    if (start <= end) {
+        bool has_any = false, any_after_zom = false, zom = false;
+        for (int i = start; i <= end; i++) {
+            if (items[i].kind == LikeItem::ANY) { any_after_zom = zom; has_any = true; break; }
+            if (items[i].kind == LikeItem::ZERO_OR_MORE) zom = true;
+        }
+        L->kind = !has_any ? TGD_LIKE_FJS : !any_after_zom ? TGD_LIKE_DFA : TGD_LIKE_NFA;
+        int pos = 0;
+        auto state = [&](int kind_bit, int val) -> bool {
+            if (pos >= 63) return false;
+            if (kind_bit) L->any_mask |= 1ULL << pos;
+            else {
+                if (L->num_lits >= TGD_LIKE_LITS) return false;
+                L->lit_pos[L->num_lits] = pos;
+                L->lit_val[L->num_lits++] = val;
+            }
+            pos++;
+            return true;
+        };
+        for (int i = start; i <= end; i++) {
+            const LikeItem& it = items[i];
+            bool ok = true;
+            if (L->kind == TGD_LIKE_FJS) {
+                if (it.kind != LikeItem::LITERAL) continue;
+                if (L->num_terms >= TGD_LIKE_TERMS) ok = false;
+                else {
+                    L->term_off[L->num_terms] = (int32_t)stored.size();
+                    L->term_len[L->num_terms++] = (int32_t)bytes[i].size();
+                    stored += bytes[i];
+                }
+            }
+            else if (it.kind == LikeItem::ZERO_OR_MORE) L->loop_mask |= 1ULL << pos;
+            else if (it.kind == LikeItem::ANY) for (int k = 0; k < it.count && ok; k++) ok = state(1, 0);
+            else if (L->kind == TGD_LIKE_DFA) for (unsigned char c : bytes[i]) { if (ok) ok = state(0, c); }
+            else for (char16_t c : it.literal) { if (ok) ok = state(0, (int)c); }
+            if (!ok) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d needs more matcher states than the device form holds", idx);
+        }
+        L->accept = pos;
+    }
+    if (stored.size() > TGD_LIKE_BYTES) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "LIKE pattern %d holds more than %d literal bytes", idx, TGD_LIKE_BYTES);
+    memcpy(L->bytes, stored.data(), stored.size());
+    return TGPU_OK;
+}
+
+static bool varchar_op(int op)
+{
+    switch (op) {
+        case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE: case TGPU_EX_BETWEEN:
+        case TGPU_EX_IN: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: case TGPU_EX_LIKE:
+            return true;
+        default: return false;
+    }
+}
+
+// one instruction over VARCHAR operands: operands are UTF8 channels (given a string slot), pool constants or NULL
+static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i, DProgram* out, int32_t* max_channel)
+{
+    const tgpu_expr_insn& s = p->insns[i];
+    DInsn& d = out->insns[i];
+    if (s.vtype != TGPU_V_VARCHAR) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: LIKE needs VARCHAR operands", i);
+    if (!varchar_op(s.op)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: op %d does not take VARCHAR operands", i, s.op);
+    if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
+    const bool unary = s.op == TGPU_EX_IS_NULL || s.op == TGPU_EX_IS_NOT_NULL || s.op == TGPU_EX_IN || s.op == TGPU_EX_LIKE;
+    const tgpu_operand* ops[3] = {&s.a, &s.b, &s.c};
+    DOperand* dops[3] = {&d.a, &d.b, &d.c};
+    const int used = unary ? 1 : s.op == TGPU_EX_BETWEEN ? 3 : 2;
+    for (int k = 0; k < 3; k++) {
+        const tgpu_operand& o = *ops[k];
+        DOperand& x = *dops[k];
+        x.kind = k < used ? o.kind : TGPU_OPND_NONE;
+        x.index = o.index;
+        x.imm = o.imm.i64;
+        if (k >= used) continue;
+        if (o.kind == TGPU_OPND_TEMP) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a VARCHAR operand cannot be a temp", i);
+        if (o.kind == TGPU_OPND_CONST) {
+            if (o.imm.i64 < 0 || o.imm.i64 >= p->num_strings) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: pool string index out of range", i);
+        }
+        else if (o.kind == TGPU_OPND_COLUMN) {
+            if (o.index < 0 || o.index >= TGPU_MAX_CHANNELS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "operand channel %d out of range", o.index);
+            if (o.index > *max_channel) *max_channel = o.index;
+            if (out->str_slot[o.index] < 0) {
+                if (out->num_str_channels >= TGD_MAX_STR_CHANNELS)
+                    return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "string operations read more than %d VARCHAR channels", TGD_MAX_STR_CHANNELS);
+                out->str_slot[o.index] = (int8_t)out->num_str_channels;
+                out->str_channel[out->num_str_channels++] = o.index;
+            }
+        }
+        else if (o.kind != TGPU_OPND_NULL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad VARCHAR operand kind %d", i, o.kind);
+    }
+    if (s.op == TGPU_EX_IN) {
+        if (s.b.imm.i64 < 0 || s.b.imm.i64 >= p->num_in_lists) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: IN list index out of range", i);
+        const tgpu_in_list& l = p->in_lists[s.b.imm.i64];
+        for (int k = 0; k < l.count; k++)
+            if (l.values[k] < 0 || l.values[k] >= p->num_strings) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: pool string index out of range", i);
+    }
+    if (s.op == TGPU_EX_LIKE && (s.b.imm.i64 < 0 || s.b.imm.i64 >= p->num_like_patterns))
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: LIKE pattern index out of range", i);
+    if (s.op == TGPU_EX_IN || s.op == TGPU_EX_LIKE) { d.b.kind = TGPU_OPND_CONST; d.b.imm = s.b.imm.i64; }
+    d.op = s.op;
+    d.vtype = s.vtype;
+    d.dst = s.dst;
+    return TGPU_OK;
+}
+
+bool expr_uses_strings(const DProgram& prog)
+{
+    for (int i = 0; i < prog.num_insns; i++)
+        if (prog.insns[i].vtype == TGPU_V_VARCHAR || prog.insns[i].op == TGPU_EX_LIKE) return true;
+    return false;
+}
 
 int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32_t* max_channel)
 {
@@ -30,6 +263,24 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         for (int k = 0; k < p->in_lists[i].count; k++) out->in_values[off + k] = p->in_lists[i].values[k];
         off += p->in_lists[i].count;
     }
+    memset(out->str_slot, -1, sizeof(out->str_slot));
+    if (p->num_strings < 0 || (p->num_strings > 0 && !p->strings)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "bad string pool");
+    if (p->num_strings > TGPU_MAX_STRINGS) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "more than %d pool strings", TGPU_MAX_STRINGS);
+    int64_t pool_bytes = 0;
+    for (int k = 0; k < p->num_strings; k++) {
+        const tgpu_bytes& b = p->strings[k];
+        if (b.length < 0 || (b.length > 0 && !b.data)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "pool string %d: bad byte string", k);
+        if (pool_bytes + b.length > TGPU_MAX_STRING_BYTES) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "pool strings hold more than %d bytes", TGPU_MAX_STRING_BYTES);
+        out->str_off[k] = (int32_t)pool_bytes;
+        out->str_len[k] = b.length;
+        if (b.length) memcpy(out->str_bytes + pool_bytes, b.data, (size_t)b.length);
+        pool_bytes += b.length;
+    }
+    out->num_strings = p->num_strings;
+    if (p->num_like_patterns < 0 || (p->num_like_patterns > 0 && !p->like_patterns)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "bad LIKE patterns");
+    if (p->num_like_patterns > TGPU_MAX_LIKE_PATTERNS) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "more than %d LIKE patterns", TGPU_MAX_LIKE_PATTERNS);
+    for (int k = 0; k < p->num_like_patterns; k++) TG_TRY(like_compile(ctx, k, p->like_patterns[k], &out->likes[k]));
+    out->num_likes = p->num_like_patterns;
     auto conv = [&](const tgpu_operand& o, DOperand* d) -> int {
         d->kind = o.kind;
         d->index = o.index;
@@ -48,7 +299,11 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         const tgpu_expr_insn& s = p->insns[i];
         DInsn& d = out->insns[i];
         if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
-        if (s.vtype < 0 || s.vtype > TGPU_V_BOOLEAN) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
+        if (s.vtype < 0 || s.vtype > TGPU_V_VARCHAR) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
+        if (s.vtype == TGPU_V_VARCHAR || s.op == TGPU_EX_LIKE) {
+            TG_TRY(compile_varchar_insn(ctx, p, i, out, max_channel));
+            continue;
+        }
         switch (s.op) {
             case TGPU_EX_MOV: case TGPU_EX_ADD: case TGPU_EX_SUB: case TGPU_EX_MUL: case TGPU_EX_DIV: case TGPU_EX_MOD: case TGPU_EX_NEG:
             case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE:
@@ -109,11 +364,131 @@ static std::string fp_operand_error(const DOperand& o)
     return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : "0u";
 }
 
+// a VARCHAR operand of generated code: its NULL flag and its StrRef (channel k: locals c<k>n / s<k>; constants: the tg_pool array)
+static void fp_str_operand(const DProgram& prog, const DOperand& o, std::string* isnull, std::string* ref)
+{
+    char buf[160];
+    if (o.kind == TGPU_OPND_COLUMN) {
+        snprintf(buf, sizeof(buf), "c%dn", o.index); *isnull = buf;
+        snprintf(buf, sizeof(buf), "s%d", o.index); *ref = buf;
+    }
+    else if (o.kind == TGPU_OPND_CONST) {
+        *isnull = "false";
+        snprintf(buf, sizeof(buf), "StrRef{(const uint8_t*)tg_pool + %d, %d}", prog.str_off[o.imm], prog.str_len[o.imm]);
+        *ref = buf;
+    }
+    else { *isnull = "true"; *ref = "StrRef{nullptr, 0}"; }
+}
+
+// `x` (a StrRef) equals pool string k: the length decides first, then packed 8-byte words against immediates (a constant of more than
+// 64 bytes is compared with the pool's copy)
+static std::string fp_str_eq_const(const std::string& x, const DProgram& prog, int64_t k)
+{
+    const uint8_t* b = prog.str_bytes + prog.str_off[k];
+    const int n = prog.str_len[k];
+    std::string e = "(" + x + ".len == " + std::to_string(n);
+    if (n > 64) return e + " && tg_str_eq(" + x + ", StrRef{(const uint8_t*)tg_pool + " + std::to_string(prog.str_off[k]) + ", " + std::to_string(n) + "}))";
+    for (int i = 0; i < n; i += 8) {
+        const int k = n - i < 8 ? n - i : 8;
+        unsigned long long w = 0;
+        for (int j = 0; j < k; j++) w |= (unsigned long long)b[i + j] << (8 * j);
+        char buf[96];
+        snprintf(buf, sizeof(buf), " && tg_ld_bytes(%s.p + %d, %d) == 0x%llxULL", x.c_str(), i, k, w);
+        e += buf;
+    }
+    return e + ")";
+}
+
+// straight-line code of one instruction over VARCHAR operands (result BOOLEAN, never an error)
+static void fp_emit_str_insn(std::string& s, const DProgram& prog, const DInsn& in)
+{
+    std::string an, a, bn, b, cn, c;
+    fp_str_operand(prog, in.a, &an, &a);
+    fp_appendf(s, "    { const bool an = %s; const StrRef a = %s; bool r = false, rn = an;\n", an.c_str(), a.c_str());
+    switch (in.op) {
+        case TGPU_EX_IS_NULL: s += "      r = an; rn = false;\n"; break;
+        case TGPU_EX_IS_NOT_NULL: s += "      r = !an; rn = false;\n"; break;
+        case TGPU_EX_LIKE: fp_appendf(s, "      if (!an) r = tg_like_%d(a);\n", (int)in.b.imm); break;
+        case TGPU_EX_IN: {
+            const int li = (int)in.b.imm;
+            s += "      if (!an) r = false";
+            for (int k = 0; k < prog.in_count[li]; k++) {
+                const int64_t si = prog.in_values[prog.in_offset[li] + k];
+                s += "\n        || " + fp_str_eq_const("a", prog, si);
+            }
+            s += ";\n";
+            break;
+        }
+        case TGPU_EX_BETWEEN:
+            fp_str_operand(prog, in.b, &bn, &b);
+            fp_str_operand(prog, in.c, &cn, &c);
+            fp_appendf(s, "      { const bool n1 = an || %s, n2 = an || %s; const bool f1 = !n1 && tg_str_cmp(a, %s) < 0, f2 = !n2 && tg_str_cmp(a, %s) > 0;\n",
+                       bn.c_str(), cn.c_str(), b.c_str(), c.c_str());
+            s += "        rn = !(f1 || f2) && (n1 || n2); r = !(f1 || f2 || rn); }\n";
+            break;
+        default:
+            fp_str_operand(prog, in.b, &bn, &b);
+            fp_appendf(s, "      rn = an || %s;\n", bn.c_str());
+            if ((in.op == TGPU_EX_EQ || in.op == TGPU_EX_NE) && in.b.kind == TGPU_OPND_CONST)
+                s += std::string("      if (!rn) r = ") + (in.op == TGPU_EX_NE ? "!" : "") + fp_str_eq_const("a", prog, in.b.imm) + ";\n";
+            else fp_appendf(s, "      if (!rn) r = tg_str_cmp_op(%d, a, %s);\n", in.op, b.c_str());
+            break;
+    }
+    fp_appendf(s, "      t%d = r ? 1 : 0; tn%d = rn; te%d = 0u; }\n", in.dst, in.dst, in.dst);
+}
+
+// module-scope data and functions the string operations of `prog` use: the constant pool and one matcher per LIKE pattern, whose
+// length bounds, prefix and suffix are immediates; the middle runs the shared matcher over the compiled pattern
+static std::string fp_string_decls(const DProgram& prog)
+{
+    std::string s;
+    if (prog.num_strings > 0) {
+        int words = 0;
+        for (int k = 0; k < prog.num_strings; k++) words = std::max(words, (prog.str_off[k] + prog.str_len[k] + 7) / 8);
+        s += "__device__ const unsigned long long tg_pool[" + std::to_string(std::max(words, 1)) + "] = {";
+        for (int w = 0; w < std::max(words, 1); w++) {
+            unsigned long long v = 0;
+            for (int j = 0; j < 8 && w * 8 + j < TGPU_MAX_STRING_BYTES; j++) v |= (unsigned long long)prog.str_bytes[w * 8 + j] << (8 * j);
+            fp_appendf(s, "%s0x%llxULL", w ? "," : "", v);
+        }
+        s += "};\n";
+    }
+    for (int k = 0; k < prog.num_likes; k++) {
+        const DLike& L = prog.likes[k];
+        if (L.kind != TGD_LIKE_NONE) {
+            fp_appendf(s, "__device__ const unsigned long long tg_like_data_%d[%d] = {", k, (int)(sizeof(DLike) / 8));
+            const unsigned long long* raw = (const unsigned long long*)&L;
+            for (size_t w = 0; w < sizeof(DLike) / 8; w++) fp_appendf(s, "%s0x%llxULL", w ? "," : "", raw[w]);
+            s += "};\n";
+        }
+        fp_appendf(s, "__device__ __forceinline__ bool tg_like_%d(StrRef s) {\n  if (s.len < %d) return false;\n", k, L.min_size);
+        if (L.max_size >= 0) fp_appendf(s, "  if (s.len > %d) return false;\n", L.max_size);
+        for (int i = 0; i < L.prefix_len; i += 8) {
+            const int n = std::min(8, L.prefix_len - i);
+            unsigned long long w = 0;
+            for (int j = 0; j < n; j++) w |= (unsigned long long)L.bytes[i + j] << (8 * j);
+            fp_appendf(s, "  if (tg_ld_bytes(s.p + %d, %d) != 0x%llxULL) return false;\n", i, n, w);
+        }
+        for (int i = 0; i < L.suffix_len; i += 8) {
+            const int n = std::min(8, L.suffix_len - i);
+            unsigned long long w = 0;
+            for (int j = 0; j < n; j++) w |= (unsigned long long)L.bytes[L.prefix_len + i + j] << (8 * j);
+            fp_appendf(s, "  if (tg_ld_bytes(s.p + s.len - %d, %d) != 0x%llxULL) return false;\n", L.suffix_len - i, n, w);
+        }
+        if (L.kind == TGD_LIKE_NONE) s += "  return true;\n}\n";
+        else fp_appendf(s, "  return %s(*(const DLike*)tg_like_data_%d, s.p + %d, s.len - %d);\n}\n",
+                        L.kind == TGD_LIKE_FJS ? "tg_like_fjs" : L.kind == TGD_LIKE_DFA ? "tg_like_dfa" : "tg_like_nfa", k, L.prefix_len,
+                        L.prefix_len + L.suffix_len);
+    }
+    return s;
+}
+
 void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
 {
     for (int i = first; i < last; i++) {
         const DInsn& in = prog.insns[i];
-        if (in.op == TGPU_EX_IN) {
+        if (in.vtype == TGPU_V_VARCHAR) fp_emit_str_insn(s, prog, in);
+        else if (in.op == TGPU_EX_IN) {
             int li = (int)in.b.imm;
             fp_appendf(s, "    { Value a = %s; bool hit = false;\n", fp_operand(in.a).c_str());
             for (int k = 0; k < prog.in_count[li]; k++) {
@@ -144,7 +519,7 @@ constexpr int FP_THREADS = 256;
 // ---- NVRTC specialisation of the two PageProcessor kernels ----------------------------------------------------------
 
 // filter pass: one row per thread, writes 1/0 selection flags
-__global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* __restrict__ prog, DColumns cols, int64_t n, uint8_t* __restrict__ flags,
+__global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* __restrict__ prog, DColumns cols, StrCols strs, int64_t n, uint8_t* __restrict__ flags,
                                                               unsigned int* __restrict__ err_out)
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
@@ -153,7 +528,7 @@ __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* _
     uint32_t err = 0;
     for (; i < n; i += stride) {
         uint32_t te = 0;
-        uint32_t nb = vm_run(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te);
+        uint32_t nb = vm_run<true>(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te, 0, 0, &strs);
         int ft = prog->filter_temp;
         err |= vm_temp_error(te, ft);
         bool sel = !((nb >> ft) & 1) && temps[ft * FP_THREADS + threadIdx.x] != 0;
@@ -163,7 +538,7 @@ __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* _
 }
 
 // projection pass: output row j <- input row sel[j] (sel == nullptr: identity)
-__global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* __restrict__ prog, DColumns cols, const int32_t* __restrict__ sel, int64_t m,
+__global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* __restrict__ prog, DColumns cols, StrCols strs, const int32_t* __restrict__ sel, int64_t m,
                                                                OutCols out, unsigned int* __restrict__ err_out, unsigned int* __restrict__ any_null)
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
@@ -174,7 +549,7 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
         int64_t row = sel ? sel[j] : j;
         int64_t* t = temps + threadIdx.x;
         uint32_t te = 0;
-        uint32_t nb = vm_run(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te);
+        uint32_t nb = vm_run<true>(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te, 0, 0, &strs);
         for (int c = 0; c < out.count; c++) {
             int tp = out.temp[c];
             err |= vm_temp_error(te, tp);
@@ -194,19 +569,20 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
 // straight-line typed code for one program over channels of the given element sizes
 static std::string gen_fp_source(const DProgram& prog, const int* elems, int num_channels, uint32_t nullable_mask, const std::vector<int>& pass_channels)
 {
-    std::string s;
-    bool used[TGPU_MAX_CHANNELS] = {false};
+    std::string s = fp_string_decls(prog);
+    bool used[TGPU_MAX_CHANNELS] = {false}, str_used[TGPU_MAX_CHANNELS] = {false};     // read as a number / as a string
     for (int i = 0; i < prog.num_insns; i++) {
         const DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
         for (auto* o : ops)
-            if (o->kind == TGPU_OPND_COLUMN) used[o->index] = true;
+            if (o->kind == TGPU_OPND_COLUMN) (prog.insns[i].vtype == TGPU_V_VARCHAR ? str_used : used)[o->index] = true;
     }
     std::string loads, temps;
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        if (!used[c]) continue;
-        fp_appendf(loads, "    const long long c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
+        if (!used[c] && !str_used[c]) continue;
+        if (used[c]) fp_appendf(loads, "    const long long c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
         if ((nullable_mask >> c) & 1) fp_appendf(loads, " const bool c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
         else fp_appendf(loads, " const bool c%dn = false;\n", c);
+        if (str_used[c]) fp_appendf(loads, "    const StrRef s%d = tg_str(strs, %d, row);\n", c, prog.str_slot[c]);
     }
     for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
     // value, NULL flag and carried error of the temp behind each computed output column (the only errors a projection raises)
@@ -214,7 +590,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(output_switch, "        case %d: v = t%d; isn = tn%d; e = te%d; break;\n", t, t, t, t);
     output_switch += "      }\n      err |= e;\n      if (isn) v = 0;\n";
     // filter kernel
-    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_jit(DColumns cols, long long n, unsigned char* flags, unsigned int* err_out) {\n";
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_jit(DColumns cols, StrCols strs, long long n, unsigned char* flags, unsigned int* err_out) {\n";
     s += "  unsigned int err = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
     s += "  for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += stride) {\n";
     s += loads + temps;
@@ -223,7 +599,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     else s += "    flags[row] = 1;\n";
     s += "  }\n  if (err) atomicOr(err_out, err);\n}\n";
     // projection kernel
-    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_jit(DColumns cols, const int* sel, long long m, OutCols out, unsigned int* err_out, unsigned int* any_null) {\n";
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_jit(DColumns cols, StrCols strs, const int* sel, long long m, OutCols out, unsigned int* err_out, unsigned int* any_null) {\n";
     s += "  unsigned int err = 0, nulls_seen = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
     s += "  for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < m; j += stride) {\n";
     s += "    const long long row = sel ? sel[j] : j;\n";
@@ -239,11 +615,11 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         if (ch < 0 || ch >= num_channels || elems[ch] == 0) chunkable = false;     // variable-width pass-through: not in this form
     if (!chunkable) return s;
     s += "struct FProg {\n";
-    s += "  static __device__ __forceinline__ bool filter(const DColumns& cols, long long row, unsigned int* errp) {\n    unsigned int err = 0;\n";
+    s += "  static __device__ __forceinline__ bool filter(const DColumns& cols, const StrCols& strs, long long row, unsigned int* errp) {\n    unsigned int err = 0;\n";
     s += loads + temps;
     fp_emit_insns(s, prog, 0, prog.num_filter_insns);
     fp_appendf(s, "    err |= te%d;\n    *errp |= err;\n    return !tn%d && t%d != 0;\n  }\n", prog.filter_temp, prog.filter_temp, prog.filter_temp);
-    s += "  static __device__ __forceinline__ void row(const DColumns& cols, long long row, long long j, const OutCols& out, unsigned int* errp, unsigned int* nullsp) {\n";
+    s += "  static __device__ __forceinline__ void row(const DColumns& cols, const StrCols& strs, long long row, long long j, const OutCols& out, unsigned int* errp, unsigned int* nullsp) {\n";
     s += "    unsigned int err = 0, nulls_seen = 0;\n";
     s += loads + temps;
     fp_emit_insns(s, prog, 0, prog.num_insns);
@@ -257,11 +633,11 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         if ((nullable_mask >> ch) & 1) fp_appendf(s, "    out.pass_nullmap[%d][j] = tg_valid(cols.cols[%d].validity, row) ? 0 : 1;\n", (int)k, ch);
     }
     s += "    *errp |= err;\n    *nullsp |= nulls_seen;\n  }\n};\n";
-    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_chunks_jit(DColumns cols, long long n, long long chunk, unsigned char* flags, "
-         "unsigned int* counts, unsigned int* err_out) { fp_filter_chunks_body<FProg>(cols, n, chunk, flags, counts, err_out); }\n";
-    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_chunks_jit(DColumns cols, const unsigned char* flags, long long n, long long chunk, "
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_chunks_jit(DColumns cols, StrCols strs, long long n, long long chunk, unsigned char* flags, "
+         "unsigned int* counts, unsigned int* err_out) { fp_filter_chunks_body<FProg>(cols, strs, n, chunk, flags, counts, err_out); }\n";
+    s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_project_chunks_jit(DColumns cols, StrCols strs, const unsigned char* flags, long long n, long long chunk, "
          "const long long* chunk_off, OutCols out, unsigned int* err_out, unsigned int* any_null) "
-         "{ fp_project_chunks_body<FProg>(cols, flags, n, chunk, chunk_off, out, err_out, any_null); }\n";
+         "{ fp_project_chunks_body<FProg>(cols, strs, flags, n, chunk, chunk_off, out, err_out, any_null); }\n";
     return s;
 }
 
@@ -326,9 +702,20 @@ struct FilterProjectOp : tgpu_op {
         }
         for (int i = 0; i < host_prog.num_insns; i++) {
             const DOperand* ops[3] = {&host_prog.insns[i].a, &host_prog.insns[i].b, &host_prog.insns[i].c};
-            for (auto* o : ops)
-                if (o->kind == TGPU_OPND_COLUMN && (in.cols[o->index].elem_size() == 0 || in.cols[o->index].elem_size() == 16 || in.cols[o->index].type == TGPU_FLOAT32))
+            const bool str = host_prog.insns[i].vtype == TGPU_V_VARCHAR;
+            for (auto* o : ops) {
+                if (o->kind != TGPU_OPND_COLUMN) continue;
+                if (str && in.cols[o->index].type != TGPU_UTF8)
+                    return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d as VARCHAR, the page's channel is not UTF8", i, o->index);
+                if (!str && (in.cols[o->index].elem_size() == 0 || in.cols[o->index].elem_size() == 16 || in.cols[o->index].type == TGPU_FLOAT32))
                     return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "expressions over variable-width / 128-bit / REAL channel %d are not supported on the GPU path", o->index);
+            }
+        }
+        StrCols strs;
+        memset(&strs, 0, sizeof(strs));
+        for (int k = 0; k < host_prog.num_str_channels; k++) {
+            strs.offsets[k] = in.cols[host_prog.str_channel[k]].offsets;
+            strs.bytes[k] = (const uint8_t*)in.cols[host_prog.str_channel[k]].data;
         }
         unsigned int* d_err = ctx->d_scratch->fp_flags;
         unsigned int* d_anynull = d_err + 1;
@@ -343,7 +730,7 @@ struct FilterProjectOp : tgpu_op {
             TG_TRY(jit_prepare(in));
             if (jit_project_chunks) {
                 bool handled = false;
-                TG_TRY(add_input_chunked(in, cols, n, d_err, d_anynull, &handled, &m));
+                TG_TRY(add_input_chunked(in, cols, strs, n, d_err, d_anynull, &handled, &m));
                 if (handled) return TGPU_OK;
                 // every row passed the filter: fall through to the identity form (blocks pass through, no copies)
             }
@@ -355,10 +742,10 @@ struct FilterProjectOp : tgpu_op {
             if (jit_filter) {
                 long long n_arg = n;
                 unsigned char* f_arg = flags.as<unsigned char>();
-                void* params[4] = {&cols, &n_arg, &f_arg, &d_err};
+                void* params[5] = {&cols, &strs, &n_arg, &f_arg, &d_err};
                 TG_TRY(jit_launch(ctx, jit_filter, tg_grid(ctx, n, FP_THREADS, jit_blocks_per_sm(jit_filter, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
-            else TG_LAUNCH(ctx, fp_filter_kernel, grid, FP_THREADS, 0, dp, cols, n, flags.as<uint8_t>(), d_err);
+            else TG_LAUNCH(ctx, fp_filter_kernel, grid, FP_THREADS, 0, dp, cols, strs, n, flags.as<uint8_t>(), d_err);
             long long* d_count = &ctx->d_scratch->fp_count;
             TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, d_count));
             TG_TRY(tg_read_i64(ctx, d_count, &m));
@@ -387,10 +774,10 @@ struct FilterProjectOp : tgpu_op {
             TG_TRY(jit_prepare(in));
             if (jit_project) {
                 long long m_arg = m;
-                void* params[6] = {&cols, &d_sel, &m_arg, &cc.oc, &d_err, &d_anynull};
+                void* params[7] = {&cols, &strs, &d_sel, &m_arg, &cc.oc, &d_err, &d_anynull};
                 TG_TRY(jit_launch(ctx, jit_project, tg_grid(ctx, m, FP_THREADS, jit_blocks_per_sm(jit_project, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
-            else TG_LAUNCH(ctx, fp_project_kernel, pgrid, FP_THREADS, 0, dp, cols, d_sel, m, cc.oc, d_err, d_anynull);
+            else TG_LAUNCH(ctx, fp_project_kernel, pgrid, FP_THREADS, 0, dp, cols, strs, d_sel, m, cc.oc, d_err, d_anynull);
             TG_TRY(finish_computed(cc, d_err, &outp));
         }
         pending.push_back(tg_make_owned_page(std::move(outp)));
@@ -449,7 +836,8 @@ struct FilterProjectOp : tgpu_op {
     }
 
     // chunked two-pass form: handled = false (and *m_out = n) when every row is selected
-    int add_input_chunked(const DevPage& in, const DColumns& cols, int64_t n, unsigned int* d_err, unsigned int* d_anynull, bool* handled, int64_t* m_out)
+    int add_input_chunked(const DevPage& in, const DColumns& cols, const StrCols& strs_in, int64_t n, unsigned int* d_err, unsigned int* d_anynull, bool* handled,
+                          int64_t* m_out)
     {
         *handled = false;
         const int64_t tile = (int64_t)FPC_R * FPC_T;
@@ -465,9 +853,10 @@ struct FilterProjectOp : tgpu_op {
         long long n_arg = n;
         {
             DColumns c = cols;
+            StrCols sc = strs_in;
             unsigned char* f_arg = flags.as<unsigned char>();
             unsigned int* cnt_arg = counts.as<unsigned int>();
-            void* params[6] = {&c, &n_arg, &chunk, &f_arg, &cnt_arg, &d_err};
+            void* params[7] = {&c, &sc, &n_arg, &chunk, &f_arg, &cnt_arg, &d_err};
             TG_TRY(jit_launch(ctx, jit_filter_chunks, chunks, FPC_T, 0, params));
         }
         TG_LAUNCH(ctx, fp_chunk_scan_kernel, 1, 256, 0, counts.as<unsigned int>(), chunks, chunk_off.as<long long>(), d_total.as<long long>());
@@ -512,9 +901,10 @@ struct FilterProjectOp : tgpu_op {
         }
         {
             DColumns c = cols;
+            StrCols sc = strs_in;
             const unsigned char* f_arg = flags.as<unsigned char>();
             const long long* off_arg = chunk_off.as<long long>();
-            void* params[8] = {&c, &f_arg, &n_arg, &chunk, &off_arg, &oc, &d_err, &d_anynull};
+            void* params[9] = {&c, &sc, &f_arg, &n_arg, &chunk, &off_arg, &oc, &d_err, &d_anynull};
             TG_TRY(jit_launch(ctx, jit_project_chunks, chunks, FPC_T, 0, params));
         }
         TG_TRY(finish_computed(cc, d_err, &outp));

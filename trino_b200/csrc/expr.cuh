@@ -41,7 +41,22 @@ struct DProgram {
     int32_t in_count[8];
     int64_t in_values[128];
     DInsn insns[TGPU_MAX_INSNS];
+    // VARCHAR operands (FilterAndProject only): the UTF8 channels string operations read (slot k = channel str_channel[k];
+    // str_slot[channel] = its slot or -1), the constant pool and the compiled LIKE patterns
+    int32_t num_str_channels;
+    int32_t str_channel[TGD_MAX_STR_CHANNELS];
+    int8_t str_slot[TGPU_MAX_CHANNELS];
+    int32_t num_strings;
+    int32_t str_off[TGPU_MAX_STRINGS];
+    int32_t str_len[TGPU_MAX_STRINGS];
+    int32_t num_likes;
+    int32_t str_pad;
+    uint8_t str_bytes[TGPU_MAX_STRING_BYTES];
+    DLike likes[TGPU_MAX_LIKE_PATTERNS];
 };
+
+// the program has an instruction over VARCHAR operands (or a LIKE)
+bool expr_uses_strings(const DProgram& prog);
 
 
 #if defined(__CUDACC__)
@@ -87,12 +102,83 @@ __device__ __forceinline__ uint32_t vm_temp_error(uint32_t errs, int t) { return
 // Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
 // [temp][thread] array (stride tstride).  Returns the updated null bitmask; *errs holds the TG_ERR_BIT_* each temp
 // carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.  `split` / `split_row`: see vm_fetch.
+// A VARCHAR operand: a UTF8 channel (through `strs`), a pool constant or NULL
+__device__ __forceinline__ StrRef vm_fetch_str(const DProgram* __restrict__ prog, const DOperand& o, const DColumns& cols, const StrCols& strs, int64_t row,
+                                               bool* is_null)
+{
+    if (o.kind == TGPU_OPND_COLUMN) {
+        *is_null = !tg_valid(cols.cols[o.index].validity, row);
+        if (*is_null) return StrRef{nullptr, 0};
+        return tg_str(strs, prog->str_slot[o.index], row);
+    }
+    if (o.kind == TGPU_OPND_CONST) {
+        *is_null = false;
+        return StrRef{prog->str_bytes + prog->str_off[o.imm], prog->str_len[o.imm]};
+    }
+    *is_null = true;
+    return StrRef{nullptr, 0};
+}
+
+// One string operation: BOOLEAN result, NULL as for the numeric operations, never an error (its operands are never temps)
+__device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog, const DInsn& in, const DColumns& cols, const StrCols& strs, int64_t row)
+{
+    Value r;
+    r.bits = 0;
+    bool an, bn = true, cn = true;
+    const StrRef a = vm_fetch_str(prog, in.a, cols, strs, row, &an);
+    switch (in.op) {
+        case TGPU_EX_IS_NULL: r.is_null = false; r.bits = an ? 1 : 0; return r;
+        case TGPU_EX_IS_NOT_NULL: r.is_null = false; r.bits = an ? 0 : 1; return r;
+        case TGPU_EX_LIKE:
+            r.is_null = an;
+            if (!an) r.bits = tg_like(prog->likes[in.b.imm], a) ? 1 : 0;
+            return r;
+        case TGPU_EX_IN: {
+            r.is_null = an;
+            if (an) return r;
+            const int li = (int)in.b.imm;
+            bool hit = false;
+            for (int k = 0; k < prog->in_count[li] && !hit; k++) {
+                const int64_t sidx = prog->in_values[prog->in_offset[li] + k];
+                hit = tg_str_eq(a, StrRef{prog->str_bytes + prog->str_off[sidx], prog->str_len[sidx]});
+            }
+            r.bits = hit ? 1 : 0;
+            return r;
+        }
+        case TGPU_EX_BETWEEN: {
+            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn);
+            const StrRef c = vm_fetch_str(prog, in.c, cols, strs, row, &cn);
+            const bool n1 = an || bn, n2 = an || cn;
+            const bool f1 = !n1 && tg_str_cmp(a, b) < 0, f2 = !n2 && tg_str_cmp(a, c) > 0;
+            r.is_null = !(f1 || f2) && (n1 || n2);
+            r.bits = (f1 || f2 || r.is_null) ? 0 : 1;
+            return r;
+        }
+        default: {
+            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn);
+            r.is_null = an || bn;
+            if (!r.is_null) r.bits = tg_str_cmp_op(in.op, a, b) ? 1 : 0;
+            return r;
+        }
+    }
+}
+
+// STR: the program may hold string operations (FilterAndProject), read through `strs`
+template <bool STR = false>
 __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
-                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs, int split = 0, int64_t split_row = 0)
+                                           int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs, int split = 0, int64_t split_row = 0,
+                                           const StrCols* strs = nullptr)
 {
     uint32_t te = *errs;
     for (int pc = first; pc < last; pc++) {
         const DInsn& in = prog->insns[pc];
+        if (STR && in.vtype == TGPU_V_VARCHAR) {
+            const Value v = vm_apply_str(prog, in, cols, *strs, row);
+            temps[in.dst * tstride] = v.bits;
+            nullbits = (nullbits & ~(1u << in.dst)) | ((v.is_null ? 1u : 0u) << in.dst);
+            te &= ~(0xFu << (4 * in.dst));
+            continue;
+        }
         Value a = vm_fetch(in.a, cols, row, temps, tstride, nullbits, split, split_row);
         Value b = vm_fetch(in.b, cols, row, temps, tstride, nullbits, split, split_row);
         Value c;

@@ -3462,6 +3462,8 @@ int build_agg_op(tgpu_ctx* ctx, const tgpu_agg_spec* spec, AggOp** out)
             return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a fused pre-stage only makes sense on raw input");
         op->has_pre = true;
         TG_TRY(tg::expr_compile(ctx, spec->pre, &op->host_prog, &op->prog_max_channel));
+        if (tg::expr_uses_strings(op->host_prog))
+            return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "the fused pre-stage does not evaluate VARCHAR operations: put a FilterAndProject in front");
         op->projections.assign(spec->pre->projections, spec->pre->projections + spec->pre->num_projections);
         op->pre_insns.assign(spec->pre->insns, spec->pre->insns + spec->pre->num_insns);
         for (int i = 0; i < spec->pre->num_in_lists; i++)
@@ -3627,6 +3629,7 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
             o->has_pre = true;
             int st = tg::expr_compile(&fake, spec->pre, &o->host_prog, &o->prog_max_channel);
             if (st != TGPU_OK) return st;
+            if (tg::expr_uses_strings(o->host_prog)) return TGPU_ERR_NOT_SUPPORTED;
             o->projections.assign(spec->pre->projections, spec->pre->projections + spec->pre->num_projections);
         }
         op = o.release();

@@ -299,8 +299,14 @@ class Col:
 
 
 class Const:
+    """value: int / float / bool, or str / bytes for V_VARCHAR (a str is taken as its UTF-8 bytes)"""
+
     def __init__(self, value, vtype):
         self.value, self.vtype = value, vtype
+
+
+def _utf8(v):
+    return v.encode() if isinstance(v, str) else bytes(v)
 
 
 class Null:
@@ -309,14 +315,17 @@ class Null:
 
 
 class Call:
-    """op: one of abi.EX_*; args: expressions.  vtype is the OPERAND type (result of comparisons is BOOLEAN)."""
+    """op: one of abi.EX_*; args: expressions.  vtype is the OPERAND type (result of comparisons is BOOLEAN).
+    EX_IN takes in_list (str / bytes values for a VARCHAR operand); EX_LIKE takes the constant pattern and an optional one-character
+    escape (str / bytes): `value LIKE pattern [ESCAPE escape]`."""
 
-    def __init__(self, op, *args, in_list=None):
+    def __init__(self, op, *args, in_list=None, pattern=None, escape=None):
         self.op, self.args, self.in_list = op, list(args), in_list
+        self.pattern, self.escape = pattern, escape
         a0 = args[0]
         self.operand_vtype = a0.vtype if not isinstance(a0, Call) else a0.result_vtype
         boolean_result = op in (abi.EX_EQ, abi.EX_NE, abi.EX_LT, abi.EX_LE, abi.EX_GT, abi.EX_GE, abi.EX_AND, abi.EX_OR, abi.EX_NOT,
-                                abi.EX_IS_NULL, abi.EX_IS_NOT_NULL, abi.EX_BETWEEN, abi.EX_IN)
+                                abi.EX_IS_NULL, abi.EX_IS_NOT_NULL, abi.EX_BETWEEN, abi.EX_IN, abi.EX_LIKE)
         if boolean_result:
             self.result_vtype = abi.V_BOOLEAN
         elif op == abi.EX_CAST_BIGINT_TO_DOUBLE:
@@ -338,6 +347,8 @@ class PageProcessorProgram:
     def __init__(self, filter_expr, projections):
         self.insns = []
         self.in_lists = []
+        self.strings = []          # VARCHAR constants (bytes), indexed by TGPU_OPND_CONST imm and VARCHAR IN-list values
+        self.like_patterns = []    # (pattern bytes, escape bytes)
         self.live = set()
         self.filter_temp = -1
         self.num_filter_insns = 0
@@ -373,9 +384,17 @@ class PageProcessorProgram:
     def _push(self, op, vtype, dst, a, b=None, c=None):
         self.insns.append((op, vtype, dst, a, b or (abi.OPND_NONE, 0, 0), c or (abi.OPND_NONE, 0, 0)))
 
+    def _string(self, v):
+        b = _utf8(v)
+        if b not in self.strings:
+            self.strings.append(b)
+        return self.strings.index(b)
+
     def _emit(self, e):
         if isinstance(e, Col):
             return (abi.OPND_COLUMN, e.channel, 0)
+        if isinstance(e, Const) and e.vtype == abi.V_VARCHAR:
+            return (abi.OPND_CONST, 0, self._string(e.value))
         if isinstance(e, Const):
             imm = abi.Imm()
             if e.vtype == abi.V_DOUBLE:
@@ -387,7 +406,13 @@ class PageProcessorProgram:
             return (abi.OPND_NULL, 0, 0)
         ops = [self._emit(a) for a in e.args]
         b = None
-        if e.op == abi.EX_IN:
+        if e.op == abi.EX_LIKE:
+            self.like_patterns.append((_utf8(e.pattern), b"" if e.escape is None else _utf8(e.escape)))
+            b = (abi.OPND_CONST, 0, len(self.like_patterns) - 1)
+        elif e.op == abi.EX_IN and e.operand_vtype == abi.V_VARCHAR:
+            self.in_lists.append([self._string(v) for v in e.in_list])
+            b = (abi.OPND_CONST, 0, len(self.in_lists) - 1)
+        elif e.op == abi.EX_IN:
             vals = []
             for v in e.in_list:
                 imm = abi.Imm()
@@ -425,9 +450,22 @@ class PageProcessorProgram:
             self._list_bufs.append(buf)
             self._lists[i].count = len(vals)
             self._lists[i].values = C.cast(buf, C.POINTER(C.c_int64))
+        # the pool's and the patterns' bytes stay alive with the program
+        self._str_bufs = [C.create_string_buffer(b, max(1, len(b))) for b in self.strings]
+        self._strs = (abi.Bytes * max(1, len(self.strings)))()
+        for i, b in enumerate(self.strings):
+            self._strs[i].length, self._strs[i].data = len(b), C.cast(self._str_bufs[i], C.c_void_p)
+        self._likes = (abi.LikePattern * max(1, len(self.like_patterns)))()
+        for i, (pat, esc) in enumerate(self.like_patterns):
+            pb, eb = C.create_string_buffer(pat, max(1, len(pat))), C.create_string_buffer(esc, max(1, len(esc)))
+            self._str_bufs += [pb, eb]
+            self._likes[i].pattern.length, self._likes[i].pattern.data = len(pat), C.cast(pb, C.c_void_p)
+            self._likes[i].escape.length, self._likes[i].escape.data = len(esc), C.cast(eb, C.c_void_p)
         self.struct = abi.ExprProgram(n, C.cast(self._insns, C.POINTER(abi.ExprInsn)), self.filter_temp, self.num_filter_insns,
                                       len(self.projections), C.cast(self._projs, C.POINTER(abi.Projection)),
-                                      len(self.in_lists), C.cast(self._lists, C.POINTER(abi.InList)))
+                                      len(self.in_lists), C.cast(self._lists, C.POINTER(abi.InList)),
+                                      len(self.strings), C.cast(self._strs, C.POINTER(abi.Bytes)),
+                                      len(self.like_patterns), C.cast(self._likes, C.POINTER(abi.LikePattern)))
 
 
 class FilterAndProjectOperatorFactory(OperatorFactory):
