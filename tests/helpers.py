@@ -180,6 +180,29 @@ def oracle_agg_rows(pages, key_channels, aggs):
 
 
 
+def kernels_launched(fn, attempts=5):
+    """Names of the kernels `fn` launches, from a profiler session (CUDA activity) in which `fn` runs between two marker kernels
+    (torch's spin_kernel, with device synchronisations around `fn`).  Only kernels that start between this session's own markers count,
+    so a record delivered late from another session cannot be attributed to `fn`.  The profiler can lose the records of a short session;
+    a session without both markers is incomplete and `fn` is observed again.  None: no complete session in `attempts`."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.init()
+    for _ in range(attempts):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
+            fn()
+            torch.cuda.synchronize()
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
+        events = [(e.time_range.start, e.name.replace(" ", "")) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+        marks = sorted(t for t, name in events if "spin_kernel" in name)
+        if len(marks) == 2:
+            return sorted({name for t, name in events if marks[0] < t < marks[1]})
+    return None
+
+
 def aggregation_known_answer_cases():
     """The sequences of the reference's AbstractTestAggregationFunction (:70-127: testNoPositions is omitted - a grouped aggregation
     without rows has no group -, testSinglePosition, testMultiplePositions, testAllPositionsNull, testMixedNullAndNonNullPositions,

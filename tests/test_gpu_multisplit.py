@@ -25,6 +25,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as o
+from helpers import kernels_launched as _kernels_launched
 from trino_b200 import abi
 from trino_b200 import operators as ops
 from trino_b200.page import Block, Page
@@ -604,29 +605,6 @@ def test_next_page_waits_until_every_page_is_taken(ctx, switches):
 
 
 # ---- routing: the table above is what the pages launch -----------------------------------------------------------------------------
-def _kernels_launched(fn, attempts=5):
-    """Names of the kernels `fn` launches, from a profiler session (CUDA activity) in which `fn` runs between two marker kernels
-    (torch's spin_kernel, with device synchronisations around `fn`).  Only kernels that start between this session's own markers count,
-    so a record delivered late from another session cannot be attributed to `fn`.  The profiler can lose the records of a short session;
-    a session without both markers is incomplete and `fn` is observed again.  None: no complete session in `attempts`."""
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.init()
-    for _ in range(attempts):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            torch.cuda._sleep(1000)
-            torch.cuda.synchronize()
-            fn()
-            torch.cuda.synchronize()
-            torch.cuda._sleep(1000)
-            torch.cuda.synchronize()
-        events = [(e.time_range.start, e.name.replace(" ", "")) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        marks = sorted(t for t, name in events if "spin_kernel" in name)
-        if len(marks) == 2:
-            return sorted({name for t, name in events if marks[0] < t < marks[1]})
-    return None
-
-
 def routing_main():
     """Body of the routing test's child process: every form's 8195-row page (checked against the reference) observed by
     _kernels_launched; prints {form: kernel names, or None} as one JSON line."""
