@@ -149,6 +149,10 @@ typedef enum tgpu_expr_op {
     TGPU_EX_BETWEEN = 25,          /* a BETWEEN b AND c: c in operand `c` */
     TGPU_EX_CAST_BIGINT_TO_DOUBLE = 30,
     TGPU_EX_CAST_DOUBLE_TO_BIGINT = 31, /* Math.round semantics, range-checked (M/type/DoubleOperators.java) */
+    TGPU_EX_CAST_TO_DECIMAL = 32,  /* CAST(a AS DECIMAL(result)): vtype BIGINT (M/type/DecimalCasts.java:240-267) or DECIMAL
+                                      (M/type/DecimalToDecimalCasts.java:36-60)                                                    */
+    TGPU_EX_CAST_DECIMAL_TO_BIGINT = 33, /* vtype DECIMAL: HALF_UP (M/type/DecimalCasts.java:219-237)                          */
+    TGPU_EX_CAST_DECIMAL_TO_DOUBLE = 34, /* vtype DECIMAL: the reference's rounding (M/type/DecimalCasts.java:439-448)         */
     TGPU_EX_IN = 40,               /* a IN (const list): b.imm = index into in_lists, all operands of `vtype`.  Under
                                       TGPU_V_VARCHAR the list's values are indices into `strings`                      */
     TGPU_EX_LIKE = 41              /* a LIKE like_patterns[b.imm] (LikeFunctions.likeVarchar, M/type/LikeFunctions.java:49-56, over
@@ -160,7 +164,14 @@ typedef enum tgpu_expr_op {
  * and offsets[i+1]), a TGPU_OPND_CONST whose imm indexes `strings`, or TGPU_OPND_NULL; a VARCHAR TGPU_OPND_TEMP is INVALID_ARGUMENT.
  * Equality is bytewise; order is Slice.compareTo (unsigned bytes, a proper prefix first: S/type/AbstractVariableWidthType.java:403-410).
  * CHAR(n) (padded comparison and LIKE) is not covered: keep Java for it. */
-typedef enum tgpu_vtype { TGPU_V_BIGINT = 0, TGPU_V_DOUBLE = 1, TGPU_V_BOOLEAN = 2, TGPU_V_VARCHAR = 3 } tgpu_vtype;
+/* TGPU_V_DECIMAL: DECIMAL(p, s) as its unscaled value; precision <= 18 is a short decimal (one BIGINT word: a TGPU_INT64 channel or a
+ * 64-bit immediate), precision 19..38 a long one (a TGPU_INT128 channel, or a (high, low) pair of `decimal_constants`).  The caller gives
+ * the resolved types of every decimal instruction in `decimal_signatures` (a, b, c: the operands that are DECIMAL; result: the DECIMAL
+ * result), and the library picks the reference's method for them (M/type/DecimalOperators.java): +, -, *, /, unary -, the six
+ * comparisons, BETWEEN, IN, IS [NOT] NULL, MOV and the three casts.  Results outside +-(10^38 - 1) raise NUMERIC_VALUE_OUT_OF_RANGE
+ * ("Decimal overflow"), a zero divisor DIVISION_BY_ZERO, a cast that does not fit INVALID_CAST_ARGUMENT.  DECIMAL % and
+ * casts from DOUBLE answer TGPU_ERR_NOT_SUPPORTED at create.  Only tgpu_filter_project_create evaluates DECIMAL. */
+typedef enum tgpu_vtype { TGPU_V_BIGINT = 0, TGPU_V_DOUBLE = 1, TGPU_V_BOOLEAN = 2, TGPU_V_VARCHAR = 3, TGPU_V_DECIMAL = 4 } tgpu_vtype;
 typedef enum tgpu_operand_kind { TGPU_OPND_NONE = 0, TGPU_OPND_COLUMN = 1, TGPU_OPND_TEMP = 2, TGPU_OPND_CONST = 3, TGPU_OPND_NULL = 4 } tgpu_operand_kind;
 
 typedef struct tgpu_operand {
@@ -205,8 +216,12 @@ typedef struct tgpu_projection {
     int32_t kind;        /* 0 = pass an input channel through (any type incl. UTF8/DICT/RLE, like InputPageProjection);
                             1 = computed: value of temp `index` after the program ran */
     int32_t index;       /* channel or temp */
-    int32_t vtype;       /* computed only: result type (BIGINT->INT64, DOUBLE->FLOAT64, BOOLEAN->INT8) */
+    int32_t vtype;       /* computed only: result type (BIGINT->INT64, DOUBLE->FLOAT64, BOOLEAN->INT8, DECIMAL->INT64 for a short and
+                            INT128 for a long result of the instruction that defines the temp) */
 } tgpu_projection;
+
+typedef struct tgpu_decimal_type { int8_t precision, scale; } tgpu_decimal_type;     /* 1 <= precision <= 38, 0 <= scale <= precision */
+typedef struct tgpu_decimal_signature { tgpu_decimal_type a, b, c, result; } tgpu_decimal_signature;   /* zero where not DECIMAL */
 
 typedef struct tgpu_expr_program {
     int32_t num_insns;
@@ -228,6 +243,11 @@ typedef struct tgpu_expr_program {
     const tgpu_bytes* strings;
     int32_t num_like_patterns;
     const tgpu_like_pattern* like_patterns;
+    /* DECIMAL (see TGPU_V_DECIMAL): one signature per instruction, or NULL for a program without DECIMAL; the long constants, as
+       (high, low) pairs, that a long TGPU_OPND_CONST's imm and a long DECIMAL IN-list value index.  A zeroed tail means no decimals. */
+    const tgpu_decimal_signature* decimal_signatures;
+    int32_t num_decimal_constants;
+    const int64_t* decimal_constants;
 } tgpu_expr_program;
 
 /* FilterAndProjectOperator (M/operator/FilterAndProjectOperator.java:60-95) over a PageProcessor

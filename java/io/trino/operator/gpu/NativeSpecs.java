@@ -16,6 +16,7 @@ import java.lang.foreign.StructLayout;
 import java.util.List;
 
 import static java.lang.foreign.ValueLayout.ADDRESS;
+import static java.lang.foreign.ValueLayout.JAVA_BYTE;
 import static java.lang.foreign.ValueLayout.JAVA_INT;
 import static java.lang.foreign.ValueLayout.JAVA_LONG;
 
@@ -52,13 +53,26 @@ public final class NativeSpecs
     static final StructLayout LIKE_PATTERN = MemoryLayout.structLayout(BYTES.withName("pattern"), BYTES.withName("escape"));
     // tgpu_expr_program { int32 num_insns; (pad); tgpu_expr_insn* insns; int32 filter_temp; int32 num_filter_insns; int32 num_projections; (pad);
     //                     tgpu_projection* projections; int32 num_in_lists; (pad); tgpu_in_list* in_lists; int32 num_strings; (pad); tgpu_bytes* strings;
-    //                     int32 num_like_patterns; (pad); tgpu_like_pattern* like_patterns }  (88 bytes; the last four fields zero = no strings)
+    //                     int32 num_like_patterns; (pad); tgpu_like_pattern* like_patterns; tgpu_decimal_signature* decimal_signatures;
+    //                     int32 num_decimal_constants; (pad); int64* decimal_constants }  (112 bytes; a zeroed tail = no strings, no decimals)
     static final StructLayout EXPR_PROGRAM = MemoryLayout.structLayout(
             JAVA_INT.withName("num_insns"), MemoryLayout.paddingLayout(4), ADDRESS.withName("insns"),
             JAVA_INT.withName("filter_temp"), JAVA_INT.withName("num_filter_insns"), JAVA_INT.withName("num_projections"), MemoryLayout.paddingLayout(4),
             ADDRESS.withName("projections"), JAVA_INT.withName("num_in_lists"), MemoryLayout.paddingLayout(4), ADDRESS.withName("in_lists"),
             JAVA_INT.withName("num_strings"), MemoryLayout.paddingLayout(4), ADDRESS.withName("strings"),
-            JAVA_INT.withName("num_like_patterns"), MemoryLayout.paddingLayout(4), ADDRESS.withName("like_patterns"));
+            JAVA_INT.withName("num_like_patterns"), MemoryLayout.paddingLayout(4), ADDRESS.withName("like_patterns"),
+            ADDRESS.withName("decimal_signatures"), JAVA_INT.withName("num_decimal_constants"), MemoryLayout.paddingLayout(4),
+            ADDRESS.withName("decimal_constants"));
+    // DECIMAL operands: TGPU_V_DECIMAL = 4; casts TGPU_EX_CAST_TO_DECIMAL = 32, _DECIMAL_TO_BIGINT = 33, _DECIMAL_TO_DOUBLE = 34.
+    // tgpu_decimal_type { int8 precision, scale }; tgpu_decimal_signature { a, b, c, result } (8 bytes): the bound types of the resolved
+    // function ($operator$add(decimal(p1,s1), decimal(p2,s2)):decimal(p,s) and the like), one per instruction
+    public static final int V_DECIMAL = 4;
+    public static final int EX_CAST_TO_DECIMAL = 32;
+    public static final int EX_CAST_DECIMAL_TO_BIGINT = 33;
+    public static final int EX_CAST_DECIMAL_TO_DOUBLE = 34;
+    static final StructLayout DECIMAL_TYPE = MemoryLayout.structLayout(JAVA_BYTE.withName("precision"), JAVA_BYTE.withName("scale"));
+    static final StructLayout DECIMAL_SIGNATURE = MemoryLayout.structLayout(DECIMAL_TYPE.withName("a"), DECIMAL_TYPE.withName("b"),
+            DECIMAL_TYPE.withName("c"), DECIMAL_TYPE.withName("result"));
     public static final int PARTITION_HASH_BUCKET = 0;    // HashBucketFunction (M/sql/planner/HashBucketFunction.java:43-46)
     public static final int PARTITION_LOCAL = 1;          // LocalPartitionGenerator (M/operator/exchange/LocalPartitionGenerator.java:45-77)
 

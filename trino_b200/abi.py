@@ -24,7 +24,9 @@ EX_MOV, EX_ADD, EX_SUB, EX_MUL, EX_DIV, EX_MOD, EX_NEG = 0, 1, 2, 3, 4, 5, 6
 EX_EQ, EX_NE, EX_LT, EX_LE, EX_GT, EX_GE = 10, 11, 12, 13, 14, 15
 EX_AND, EX_OR, EX_NOT, EX_IS_NULL, EX_IS_NOT_NULL, EX_BETWEEN = 20, 21, 22, 23, 24, 25
 EX_CAST_BIGINT_TO_DOUBLE, EX_CAST_DOUBLE_TO_BIGINT, EX_IN, EX_LIKE = 30, 31, 40, 41
-V_BIGINT, V_DOUBLE, V_BOOLEAN, V_VARCHAR = 0, 1, 2, 3
+# DECIMAL casts: EX_CAST_TO_DECIMAL reads BIGINT or DECIMAL (its vtype), the other two read DECIMAL
+EX_CAST_TO_DECIMAL, EX_CAST_DECIMAL_TO_BIGINT, EX_CAST_DECIMAL_TO_DOUBLE = 32, 33, 34
+V_BIGINT, V_DOUBLE, V_BOOLEAN, V_VARCHAR, V_DECIMAL = 0, 1, 2, 3, 4
 MAX_STRINGS, MAX_STRING_BYTES, MAX_LIKE_PATTERNS = 128, 4096, 8
 OPND_NONE, OPND_COLUMN, OPND_TEMP, OPND_CONST, OPND_NULL = 0, 1, 2, 3, 4
 
@@ -89,6 +91,15 @@ class Projection(C.Structure):
     _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("vtype", C.c_int32)]
 
 
+class DecimalType(C.Structure):
+    _fields_ = [("precision", C.c_int8), ("scale", C.c_int8)]
+
+
+class DecimalSignature(C.Structure):
+    """the resolved DECIMAL types of one instruction's operands a, b, c and its result (zero where not DECIMAL)"""
+    _fields_ = [("a", DecimalType), ("b", DecimalType), ("c", DecimalType), ("result", DecimalType)]
+
+
 class ExprProgram(C.Structure):
     _fields_ = [
         ("num_insns", C.c_int32),
@@ -103,6 +114,9 @@ class ExprProgram(C.Structure):
         ("strings", C.POINTER(Bytes)),
         ("num_like_patterns", C.c_int32),
         ("like_patterns", C.POINTER(LikePattern)),
+        ("decimal_signatures", C.POINTER(DecimalSignature)),
+        ("num_decimal_constants", C.c_int32),
+        ("decimal_constants", C.POINTER(C.c_int64)),
     ]
 
 

@@ -39,10 +39,22 @@ enum {
     TGD_EX_MOV = 0, TGD_EX_ADD = 1, TGD_EX_SUB = 2, TGD_EX_MUL = 3, TGD_EX_DIV = 4, TGD_EX_MOD = 5, TGD_EX_NEG = 6,
     TGD_EX_EQ = 10, TGD_EX_NE = 11, TGD_EX_LT = 12, TGD_EX_LE = 13, TGD_EX_GT = 14, TGD_EX_GE = 15,
     TGD_EX_AND = 20, TGD_EX_OR = 21, TGD_EX_NOT = 22, TGD_EX_IS_NULL = 23, TGD_EX_IS_NOT_NULL = 24, TGD_EX_BETWEEN = 25,
-    TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_IN = 40, TGD_EX_LIKE = 41
+    TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_CAST_TO_DECIMAL = 32, TGD_EX_CAST_DECIMAL_TO_BIGINT = 33,
+    TGD_EX_CAST_DECIMAL_TO_DOUBLE = 34, TGD_EX_IN = 40, TGD_EX_LIKE = 41
 };
-enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2, TGD_V_VARCHAR = 3 };
-enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4 };
+// TGD_V_DECIMAL_LONG is internal: the output-column type of a long DECIMAL projection (16-byte cells: high word, low word)
+enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2, TGD_V_VARCHAR = 3, TGD_V_DECIMAL = 4, TGD_V_DECIMAL_LONG = 5 };
+enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4, TG_ERR_BIT_DECIMAL_OVERFLOW = 8 };
+
+// The reference's method for one DECIMAL instruction, fixed at create from its signature (expr.cu decimal_method).  la / lb / lc / lr:
+// operand a / b / c and the result are long decimals (a BIGINT operand or a non-DECIMAL result: 0).  k0..k2, m0, m1: see vm_apply_dec.
+// hi: the high words of long constant operands a, b, c.
+struct DDec {
+    int8_t is_dec, la, lb, lc, lr, pad0, pad1, pad2;
+    int32_t k0, k1, k2, pad3;
+    long long m0, m1;
+    long long hi[3];
+};
 
 enum AccKind {
     ACC_ROWS = 0, ACC_NONNULL = 1, ACC_SUM_F64 = 2, ACC_SUM_I64_LO = 3, ACC_SUM_I64_HI = 4,
@@ -473,6 +485,452 @@ __device__ __forceinline__ uint32_t vm_error(int op, int vtype, Value a, uint32_
             if (a.is_null) return 0;
             return eb ? eb : own;
         default: return own;   // one operand
+    }
+}
+
+#endif  // __CUDACC__
+
+// ---- DECIMAL: 128-bit two's-complement arithmetic over (high, low) 64-bit words --------------------------------------------------------
+// Int128Math (S/type/Int128Math.java) and Decimals.overflows (S/type/Decimals.java:314-335) restated.  Written over word pairs so that NVRTC
+// needs no 128-bit integer type; host and device share them (the host computes the constants of a program with them).
+#if defined(__CUDACC__)
+#define TGD_HD __host__ __device__ __forceinline__
+#else
+#define TGD_HD inline
+#endif
+
+struct U128 {
+    unsigned long long hi, lo;
+};
+
+TGD_HD unsigned long long tgd_umulhi(unsigned long long a, unsigned long long b)
+{
+#if defined(__CUDA_ARCH__)
+    return __umul64hi(a, b);
+#else
+    return (unsigned long long)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+
+TGD_HD int tgd_clz64(unsigned long long x)
+{
+#if defined(__CUDA_ARCH__)
+    return __clzll((long long)x);
+#else
+    return x ? __builtin_clzll(x) : 64;
+#endif
+}
+
+TGD_HD U128 u128_sx(long long v) { return U128{(unsigned long long)(v >> 63), (unsigned long long)v}; }
+TGD_HD bool u128_is_neg(U128 x) { return (long long)x.hi < 0; }
+TGD_HD bool u128_is_zero(U128 x) { return (x.hi | x.lo) == 0; }
+TGD_HD U128 u128_negate(U128 x) { return U128{~x.hi + (x.lo == 0 ? 1ULL : 0ULL), 0ULL - x.lo}; }
+TGD_HD U128 u128_add(U128 a, U128 b)
+{
+    const unsigned long long lo = a.lo + b.lo;
+    return U128{a.hi + b.hi + (lo < a.lo ? 1ULL : 0ULL), lo};
+}
+TGD_HD U128 u128_sub(U128 a, U128 b) { return U128{a.hi - b.hi - (a.lo < b.lo ? 1ULL : 0ULL), a.lo - b.lo}; }
+TGD_HD int u128_cmp(U128 a, U128 b)     // signed
+{
+    if (a.hi != b.hi) return (long long)a.hi < (long long)b.hi ? -1 : 1;
+    return a.lo < b.lo ? -1 : a.lo > b.lo ? 1 : 0;
+}
+TGD_HD int u128_ucmp(U128 a, U128 b)
+{
+    if (a.hi != b.hi) return a.hi < b.hi ? -1 : 1;
+    return a.lo < b.lo ? -1 : a.lo > b.lo ? 1 : 0;
+}
+TGD_HD U128 u128_abs(U128 x) { return u128_is_neg(x) ? u128_negate(x) : x; }    // the magnitude, as an unsigned value
+TGD_HD int u128_bits(U128 x) { return x.hi ? 128 - tgd_clz64(x.hi) : 64 - tgd_clz64(x.lo); }
+TGD_HD U128 u128_shr(U128 x, int s)     // logical, 0 <= s < 128
+{
+    if (s == 0) return x;
+    if (s >= 64) return U128{0ULL, x.hi >> (s - 64)};
+    return U128{x.hi >> s, (x.lo >> s) | (x.hi << (64 - s))};
+}
+TGD_HD U128 u128_shl(U128 x, int s)     // 0 <= s < 128
+{
+    if (s == 0) return x;
+    if (s >= 64) return U128{x.lo << (s - 64), 0ULL};
+    return U128{(x.hi << s) | (x.lo >> (64 - s)), x.lo << s};
+}
+TGD_HD bool u128_bit(U128 x, int i) { return i >= 64 ? ((x.hi >> (i - 64)) & 1ULL) != 0 : ((x.lo >> i) & 1ULL) != 0; }
+TGD_HD U128 u128_low_bits(U128 x, int n)     // bits [0, n), 0 <= n < 128
+{
+    if (n >= 64) return U128{n == 64 ? 0ULL : x.hi & ((1ULL << (n - 64)) - 1ULL), x.lo};
+    return U128{0ULL, n == 0 ? 0ULL : x.lo & ((1ULL << n) - 1ULL)};
+}
+// x << s over 256 bits (hi:lo), 0 <= s < 256
+TGD_HD void u128_shl_wide(U128 x, int s, U128* hi, U128* lo)
+{
+    if (s >= 128) { *hi = u128_shl(x, s - 128); *lo = U128{0ULL, 0ULL}; return; }
+    *lo = u128_shl(x, s);
+    *hi = s == 0 ? U128{0ULL, 0ULL} : u128_shr(x, 128 - s);
+}
+
+// 10^k, 0 <= k <= 38 (folds to immediates when k is a constant)
+TGD_HD U128 tgd_pow10(int k)
+{
+    U128 r{0ULL, 1ULL};
+    for (int i = 0; i < k; i++) r = U128{r.hi * 10ULL + tgd_umulhi(r.lo, 10ULL), r.lo * 10ULL};
+    return r;
+}
+
+// magnitudes a * b; true when the product is 2^127 or more (Int128Math.multiply's overflow rule: the signed result would not fit)
+TGD_HD bool u128_umul_ovf(U128 a, U128 b, U128* r)
+{
+    const unsigned long long h0 = tgd_umulhi(a.lo, b.lo);
+    bool ovf = (a.hi != 0 && b.hi != 0) || tgd_umulhi(a.lo, b.hi) != 0 || tgd_umulhi(a.hi, b.lo) != 0;
+    const unsigned long long s1 = h0 + a.lo * b.hi;
+    ovf = ovf || s1 < h0;
+    const unsigned long long s2 = s1 + a.hi * b.lo;
+    ovf = ovf || s2 < s1 || (s2 >> 63) != 0;
+    *r = U128{s2, a.lo * b.lo};
+    return ovf;
+}
+
+// checked signed multiply (Int128Math.multiply)
+TGD_HD bool u128_mul_ovf(U128 a, U128 b, U128* r)
+{
+    const bool neg = u128_is_neg(a) != u128_is_neg(b);
+    U128 m;
+    const bool ovf = u128_umul_ovf(u128_abs(a), u128_abs(b), &m);
+    *r = neg ? u128_negate(m) : m;
+    return ovf;
+}
+
+// x * 10^k, checked (Int128Math.shiftLeftBy10: overflow past 127 bits, or k > 38)
+TGD_HD bool u128_scale_up_ovf(U128 x, int k, U128* r)
+{
+    if (k > 38) { *r = x; return true; }
+    return u128_mul_ovf(x, tgd_pow10(k), r);
+}
+
+// unsigned (nh:nl) / d, 256 by 128 bits; false when the quotient does not fit 128 bits (Int128Math.pack).  A 128-bit dividend over a
+// divisor below 2^32 takes four digit steps; anything else shift-and-subtract from the dividend's top bit.
+TGD_HD bool u256_divmod(U128 nh, U128 nl, U128 d, U128* q, U128* rem)
+{
+    if ((nh.hi | nh.lo) == 0 && d.hi == 0 && (d.lo >> 32) == 0) {
+        // a 128-bit dividend and a divisor below 2^32 (decimal(12,2) / decimal(12,2) and the like): four 64-by-32-bit digit steps
+        const unsigned long long dv = d.lo;
+        const unsigned long long n3 = nl.hi >> 32, n2 = nl.hi & 0xFFFFFFFFULL, n1 = nl.lo >> 32, n0 = nl.lo & 0xFFFFFFFFULL;
+        const unsigned long long q3 = n3 / dv, r3 = n3 % dv;
+        const unsigned long long t2 = (r3 << 32) | n2, q2 = t2 / dv, r2 = t2 % dv;
+        const unsigned long long t1 = (r2 << 32) | n1, q1 = t1 / dv, r1 = t1 % dv;
+        const unsigned long long t0 = (r1 << 32) | n0, q0 = t0 / dv, r0 = t0 % dv;
+        *q = U128{(q3 << 32) | q2, (q1 << 32) | q0};
+        *rem = U128{0ULL, r0};
+        return true;
+    }
+    const int nb = nh.hi | nh.lo ? 128 + u128_bits(nh) : u128_bits(nl);
+    U128 r{0ULL, 0ULL}, qt{0ULL, 0ULL};
+    bool fits = true;
+    for (int i = nb - 1; i >= 0; i--) {
+        const U128& w = i >= 128 ? nh : nl;
+        const int j = i & 127;
+        const unsigned long long bit = j >= 64 ? (w.hi >> (j - 64)) & 1ULL : (w.lo >> j) & 1ULL;
+        const bool carry = (r.hi >> 63) != 0;
+        r = U128{(r.hi << 1) | (r.lo >> 63), (r.lo << 1) | bit};
+        if (carry || u128_ucmp(r, d) >= 0) {
+            r = u128_sub(r, d);
+            if (i >= 128) fits = false;
+            else if (j >= 64) qt.hi |= 1ULL << (j - 64);
+            else qt.lo |= 1ULL << j;
+        }
+    }
+    *q = qt;
+    *rem = r;
+    return fits;
+}
+
+// full unsigned 128 x 128 -> 256 product (hi:lo)
+TGD_HD void u128_umul_full(U128 a, U128 b, U128* hi, U128* lo)
+{
+    // 64-bit limbs: a = a1:a0, b = b1:b0
+    const unsigned long long p00l = a.lo * b.lo, p00h = tgd_umulhi(a.lo, b.lo);
+    const unsigned long long p01l = a.lo * b.hi, p01h = tgd_umulhi(a.lo, b.hi);
+    const unsigned long long p10l = a.hi * b.lo, p10h = tgd_umulhi(a.hi, b.lo);
+    const unsigned long long p11l = a.hi * b.hi, p11h = tgd_umulhi(a.hi, b.hi);
+    unsigned long long w1 = p00h, c1 = 0;
+    w1 += p01l; c1 += w1 < p01l;
+    w1 += p10l; c1 += w1 < p10l;
+    unsigned long long w2 = p11l, c2 = 0;
+    w2 += p01h; c2 += w2 < p01h;
+    w2 += p10h; c2 += w2 < p10h;
+    w2 += c1; c2 += w2 < c1;
+    *lo = U128{w1, p00l};
+    *hi = U128{p11h + c2, w2};
+}
+
+// x / 10^k rounded HALF_UP on the magnitude (Int128Math.scaleDownRoundUp), 0 <= k
+TGD_HD U128 u128_scale_down_round_up(U128 x, int k)
+{
+    if (k == 0) return x;
+    if (k > 38) return U128{0ULL, 0ULL};     // |x| < 2^127 < 10^39 / 2
+    const bool neg = u128_is_neg(x);
+    const U128 d = tgd_pow10(k);
+    U128 q, r;
+    u256_divmod(U128{0ULL, 0ULL}, u128_abs(x), d, &q, &r);
+    if (u128_ucmp(r, u128_sub(d, r)) >= 0) q = u128_add(q, U128{0ULL, 1ULL});
+    return neg ? u128_negate(q) : q;
+}
+
+// Int128Math.rescale: k > 0 scales up (checked), k < 0 scales down HALF_UP
+TGD_HD bool u128_rescale_ovf(U128 x, int k, U128* r)
+{
+    if (k >= 0) return k == 0 ? (*r = x, false) : u128_scale_up_ovf(x, k, r);
+    *r = u128_scale_down_round_up(x, -k);
+    return false;
+}
+
+// Decimals.overflows: outside +-(10^38 - 1)
+TGD_HD bool u128_dec_overflows(U128 x)
+{
+    const U128 max{0x4b3b4ca85a86c47aULL, 0x098a223fffffffffULL};
+    return u128_cmp(x, max) > 0 || u128_cmp(x, u128_negate(max)) < 0;
+}
+
+// |x| >= 10^p (Decimals.overflows(Int128, precision))
+TGD_HD bool u128_exceeds_precision(U128 x, int p) { return u128_ucmp(u128_abs(x), tgd_pow10(p)) >= 0; }
+
+// Int128Math.divideRoundUp(dividend, k, divisor, 0): |dividend| * 10^k / |divisor| HALF_UP, the sign restored; true on overflow
+// (k >= 38 or a quotient past 128 bits).  The increment and the negation wrap as the reference's do.
+TGD_HD bool u128_divide_round_up_ovf(U128 a, int k, U128 b, U128* r)
+{
+    if (k >= 38) return true;
+    const bool neg = u128_is_neg(a) != u128_is_neg(b);
+    const U128 d = u128_abs(b);
+    U128 nh, nl, q, rem;
+    u128_umul_full(u128_abs(a), tgd_pow10(k), &nh, &nl);
+    if (!u256_divmod(nh, nl, d, &q, &rem)) return true;
+    const U128 rem2{(rem.hi << 1) | (rem.lo >> 63), rem.lo << 1};
+    if (u128_ucmp(rem2, d) >= 0) q = u128_add(q, U128{0ULL, 1ULL});
+    *r = neg ? u128_negate(q) : q;
+    return false;
+}
+
+#if defined(__CUDACC__)
+
+// x / 10^s correctly rounded to the nearest double (DecimalConversions.longDecimalToDouble: its fast path and its parseDouble fallback
+// both give the double nearest the exact value).  The magnitude is shifted left until the quotient holds at least 66 bits; the quotient
+// rounds to 53 bits half-even with the remainder as sticky bit.
+__device__ __forceinline__ double tgd_u128_div_pow10_to_double(U128 x, int s)
+{
+    if (u128_is_zero(x)) return 0.0;
+    const bool neg = u128_is_neg(x);
+    const U128 n = u128_abs(x), d = tgd_pow10(s);
+    int sh = 66 + u128_bits(d) - u128_bits(n);     // <= 66 + 127 - 1
+    if (sh < 0) sh = 0;
+    U128 th, tl;     // n << sh over 256 bits
+    u128_shl_wide(n, sh, &th, &tl);
+    U128 q, rem;
+    u256_divmod(th, tl, d, &q, &rem);     // q has 66..128 bits
+    const int drop = u128_bits(q) - 53;
+    unsigned long long mant = u128_shr(q, drop).lo;
+    const bool round_bit = u128_bit(q, drop - 1);
+    const bool sticky = !u128_is_zero(rem) || !u128_is_zero(u128_low_bits(q, drop - 1));
+    int e = drop - sh;
+    if (round_bit && (sticky || (mant & 1ULL))) {
+        mant++;
+        if (mant == (1ULL << 53)) { mant >>= 1; e++; }
+    }
+    const double v = scalbn((double)mant, e);
+    return neg ? -v : v;
+}
+
+struct DVal {
+    U128 v;
+    bool is_null;
+};
+
+__device__ __forceinline__ long long tgd_mulhi_s(long long a, long long b) { return __mul64hi(a, b); }
+
+// One DECIMAL instruction (d.is_dec) except IN: the operands as 128-bit values (a short decimal or a BIGINT sign-extended).  The
+// result's low word is a short decimal, BIGINT, DOUBLE (bits) or BOOLEAN result; a long decimal uses both words.  The method is the
+// reference's for the signature, fixed in `d` (expr.cu decimal_method):
+//   ADD / SUB   short: a * m0 +- b * m1 (unchecked); long: k0 = rescale, k1 = rescale the left operand, k2 = result rescale
+//   MUL         short: a * b (unchecked); short x short -> long: exact; long: checked, then rescale by k2
+//   DIV         k0 = rescale factor; short / short -> short: divideShortShortShort with m0 = 10^k0; otherwise divideRoundUp
+//   CAST_TO_DECIMAL      k0 = result precision, k1 = result scale - operand scale (DECIMAL operand) or the result scale (BIGINT),
+//                        k2 = 1 when the types are identical; m0 = 10^|k1| and m1 = 10^|k1| / 2 for the short paths
+//   CAST_DECIMAL_TO_*    k1 = the operand's scale, m0 = 10^k1 (short)
+__device__ __forceinline__ DVal vm_apply_dec(int op, int vtype, const DDec& d, DVal a, DVal b, DVal c, uint32_t* err)
+{
+    DVal r;
+    r.v = U128{0ULL, 0ULL};
+    r.is_null = false;
+    const bool shortest = !d.la && !d.lb && !d.lr;
+    switch (op) {
+        case TGD_EX_MOV: r = a; break;
+        case TGD_EX_ADD: case TGD_EX_SUB: {
+            r.is_null = a.is_null || b.is_null;
+            if (r.is_null) break;
+            if (shortest) {
+                const unsigned long long x = a.v.lo * (unsigned long long)d.m0, y = b.v.lo * (unsigned long long)d.m1;
+                r.v = u128_sx((long long)(op == TGD_EX_ADD ? x + y : x - y));
+                break;
+            }
+            U128 x = a.v, y = b.v, s;
+            bool ovf = false;
+            if (d.k0) ovf = d.k1 ? u128_scale_up_ovf(a.v, d.k0, &x) : u128_scale_up_ovf(b.v, d.k0, &y);
+            if (op == TGD_EX_ADD) {
+                s = u128_add(x, y);
+                ovf = ovf || (((s.hi ^ x.hi) & (s.hi ^ y.hi)) >> 63) != 0;
+            }
+            else {
+                s = u128_sub(x, y);
+                ovf = ovf || (((x.hi ^ y.hi) & (x.hi ^ s.hi)) >> 63) != 0;
+            }
+            if (!ovf) ovf = u128_rescale_ovf(s, d.k2, &r.v);
+            if (ovf || u128_dec_overflows(r.v)) *err |= TG_ERR_BIT_DECIMAL_OVERFLOW;
+            break;
+        }
+        case TGD_EX_MUL: {
+            r.is_null = a.is_null || b.is_null;
+            if (r.is_null) break;
+            if (shortest) { r.v = u128_sx((long long)(a.v.lo * b.v.lo)); break; }
+            if (!d.la && !d.lb) {
+                r.v = U128{(unsigned long long)tgd_mulhi_s((long long)a.v.lo, (long long)b.v.lo), a.v.lo * b.v.lo};
+                break;
+            }
+            U128 p;
+            bool ovf = u128_mul_ovf(a.v, b.v, &p);
+            if (!ovf) ovf = u128_rescale_ovf(p, d.k2, &r.v);
+            if (ovf || u128_dec_overflows(r.v)) *err |= TG_ERR_BIT_DECIMAL_OVERFLOW;
+            break;
+        }
+        case TGD_EX_DIV: {
+            r.is_null = a.is_null || b.is_null;
+            if (r.is_null) break;
+            if (u128_is_zero(b.v)) { *err |= TG_ERR_BIT_DIV_ZERO; break; }
+            if (shortest) {
+                // divideShortShortShort, 64-bit wraparound included
+                const long long x = (long long)a.v.lo, y = (long long)b.v.lo;
+                if (x == 0) break;
+                const long long sg = (x > 0 ? 1 : -1) * (y > 0 ? 1 : -1);
+                const long long ux = x < 0 ? (long long)(0ULL - (unsigned long long)x) : x, uy = y < 0 ? (long long)(0ULL - (unsigned long long)y) : y;
+                const long long rs = (long long)((unsigned long long)ux * (unsigned long long)d.m0);
+                const long long q = rs / uy;     // (uy is never -1)
+                const long long rem = (long long)((unsigned long long)rs - (unsigned long long)q * (unsigned long long)uy);
+                const long long q2 = (unsigned long long)rem * 2ULL >= (unsigned long long)uy ? (long long)((unsigned long long)q + 1ULL) : q;
+                r.v = u128_sx((long long)((unsigned long long)sg * (unsigned long long)q2));
+                break;
+            }
+            U128 q;
+            bool ovf = u128_divide_round_up_ovf(a.v, d.k0, b.v, &q);
+            if (!ovf) ovf = d.lr ? u128_dec_overflows(q) : q.hi != (unsigned long long)((long long)q.lo >> 63);
+            if (ovf) *err |= TG_ERR_BIT_DECIMAL_OVERFLOW;
+            else r.v = q;
+            break;
+        }
+        case TGD_EX_NEG:
+            r.is_null = a.is_null;
+            if (r.is_null) break;
+            if (!d.la) r.v = u128_sx((long long)(0ULL - a.v.lo));
+            else {
+                if (a.v.hi == 0x8000000000000000ULL && a.v.lo == 0ULL) *err |= TG_ERR_BIT_DECIMAL_OVERFLOW;
+                r.v = u128_negate(a.v);
+            }
+            break;
+        case TGD_EX_EQ: case TGD_EX_NE: case TGD_EX_LT: case TGD_EX_LE: case TGD_EX_GT: case TGD_EX_GE: {
+            r.is_null = a.is_null || b.is_null;
+            if (r.is_null) break;
+            const int k = d.la ? u128_cmp(a.v, b.v) : ((long long)a.v.lo < (long long)b.v.lo ? -1 : (long long)a.v.lo > (long long)b.v.lo ? 1 : 0);
+            const bool t = op == TGD_EX_EQ ? k == 0 : op == TGD_EX_NE ? k != 0 : op == TGD_EX_LT ? k < 0 : op == TGD_EX_LE ? k <= 0 : op == TGD_EX_GT ? k > 0 : k >= 0;
+            r.v.lo = t ? 1ULL : 0ULL;
+            break;
+        }
+        case TGD_EX_BETWEEN: {
+            const bool n1 = a.is_null || b.is_null, n2 = a.is_null || c.is_null;
+            const bool f1 = !n1 && u128_cmp(a.v, b.v) < 0, f2 = !n2 && u128_cmp(a.v, c.v) > 0;
+            r.is_null = !(f1 || f2) && (n1 || n2);
+            r.v.lo = (f1 || f2 || r.is_null) ? 0ULL : 1ULL;
+            break;
+        }
+        case TGD_EX_IS_NULL: r.v.lo = a.is_null ? 1ULL : 0ULL; break;
+        case TGD_EX_IS_NOT_NULL: r.v.lo = a.is_null ? 0ULL : 1ULL; break;
+        case TGD_EX_CAST_TO_DECIMAL: {
+            r.is_null = a.is_null;
+            if (r.is_null) break;
+            bool bad = false;
+            if (vtype != TGD_V_DECIMAL) {
+                if (!d.lr) {
+                    // bigintToShortDecimal: multiplyExact, then |v| >= 10^p (Math.abs wraps at Long.MIN_VALUE as the reference's does)
+                    const long long x = (long long)a.v.lo, v = (long long)((unsigned long long)x * (unsigned long long)d.m0);
+                    bad = tgd_mulhi_s(x, d.m0) != (v >> 63);
+                    const long long av = v < 0 ? (long long)(0ULL - (unsigned long long)v) : v;
+                    bad = bad || av >= (long long)tgd_pow10(d.k0).lo;
+                    r.v = u128_sx(v);
+                }
+                else {
+                    bad = u128_mul_ovf(tgd_pow10(d.k1), a.v, &r.v);
+                    bad = bad || u128_exceeds_precision(r.v, d.k0);
+                }
+            }
+            else if (d.k2) r = a;
+            else if (!d.la && !d.lr) {
+                // shortToShortCast
+                const long long x = (long long)a.v.lo;
+                long long v;
+                if (d.k1 >= 0) v = (long long)((unsigned long long)x * (unsigned long long)d.m0);
+                else {
+                    v = x / d.m0;
+                    const long long rm = x % d.m0;
+                    if (x >= 0) { if (rm >= d.m1) v++; }
+                    else if (rm <= -d.m1) v--;
+                }
+                const long long av = v < 0 ? (long long)(0ULL - (unsigned long long)v) : v;
+                bad = av >= (long long)tgd_pow10(d.k0).lo;
+                r.v = u128_sx(v);
+            }
+            else {
+                bad = u128_rescale_ovf(a.v, d.k1, &r.v) || u128_exceeds_precision(r.v, d.k0);
+                if (!d.lr) r.v = u128_sx((long long)r.v.lo);
+            }
+            if (bad) { *err |= TG_ERR_BIT_INVALID_CAST; r.v = U128{0ULL, 0ULL}; }
+            break;
+        }
+        case TGD_EX_CAST_DECIMAL_TO_BIGINT:
+            r.is_null = a.is_null;
+            if (r.is_null) break;
+            if (!d.la) {
+                const unsigned long long x = a.v.lo, h = (unsigned long long)d.m0 / 2ULL;
+                r.v = u128_sx((long long)x >= 0 ? (long long)(x + h) / d.m0 : (long long)(0ULL - (unsigned long long)((long long)(0ULL - x + h) / d.m0)));
+            }
+            else {
+                const U128 q = u128_scale_down_round_up(a.v, d.k1);
+                if (q.hi != (unsigned long long)((long long)q.lo >> 63)) *err |= TG_ERR_BIT_INVALID_CAST;
+                else r.v = q;
+            }
+            break;
+        case TGD_EX_CAST_DECIMAL_TO_DOUBLE:
+            r.is_null = a.is_null;
+            if (r.is_null) break;
+            r.v.lo = (unsigned long long)__double_as_longlong(d.la ? tgd_u128_div_pow10_to_double(a.v, d.k1)
+                                                                   : __ddiv_rn((double)(long long)a.v.lo, (double)d.m0));
+            break;
+        default: break;
+    }
+    if (!d.lr && op != TGD_EX_MOV) r.v.hi = (unsigned long long)((long long)r.v.lo >> 63);
+    return r;
+}
+
+// vm_error for a DECIMAL instruction: the same rules, BETWEEN's "min <= value" compared as 128-bit values
+__device__ __forceinline__ uint32_t vm_error_dec(int op, DVal a, uint32_t ea, DVal b, uint32_t eb, uint32_t ec, uint32_t own)
+{
+    if (ea) return ea;
+    switch (op) {
+        case TGD_EX_BETWEEN:
+            if (a.is_null) return 0;
+            if (eb) return eb;
+            if (!b.is_null && u128_cmp(b.v, a.v) > 0) return 0;
+            return ec;
+        case TGD_EX_ADD: case TGD_EX_SUB: case TGD_EX_MUL: case TGD_EX_DIV:
+        case TGD_EX_EQ: case TGD_EX_NE: case TGD_EX_LT: case TGD_EX_LE: case TGD_EX_GT: case TGD_EX_GE:
+            if (a.is_null) return 0;
+            return eb ? eb : own;
+        default: return own;
     }
 }
 

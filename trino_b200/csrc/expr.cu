@@ -235,6 +235,213 @@ static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i
     return TGPU_OK;
 }
 
+// ---- DECIMAL ------------------------------------------------------------------------------------------------------------------------
+struct DecType {
+    int p = 0, s = 0;     // p == 0: not a DECIMAL
+    bool operator==(const DecType& o) const { return p == o.p && s == o.s; }
+    bool lng() const { return p > 18; }
+};
+
+static bool dec_insn(const tgpu_expr_insn& s)
+{
+    return s.vtype == TGPU_V_DECIMAL || s.op == TGPU_EX_CAST_TO_DECIMAL || s.op == TGPU_EX_CAST_DECIMAL_TO_BIGINT || s.op == TGPU_EX_CAST_DECIMAL_TO_DOUBLE;
+}
+
+static long long pow10_i64(int k)
+{
+    long long r = 1;
+    for (int i = 0; i < k; i++) r *= 10;
+    return r;
+}
+
+// the DECIMAL instructions of `p`: every type checked against the rules of the signatures, and the reference's method of each
+// (DecimalOperators.java's specialisers: calculateShortRescaleParameters, calculateLongRescaleParameters,
+// calculateMultiplicativeResultRescale, divideRescaleFactor; DecimalCasts / DecimalToDecimalCasts) fixed in out->dec
+static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out)
+{
+    bool any = false;
+    for (int i = 0; i < p->num_insns; i++) any = any || dec_insn(p->insns[i]);
+    if (!any) return TGPU_OK;
+    if (!p->decimal_signatures) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "a program with DECIMAL instructions needs decimal_signatures");
+    if (p->num_decimal_constants < 0 || (p->num_decimal_constants > 0 && !p->decimal_constants))
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "bad decimal constants");
+    out->has_dec = 1;
+    DecType temp_t[TGPU_MAX_TEMPS], col_t[TGPU_MAX_CHANNELS];
+    bool temp_written[TGPU_MAX_TEMPS] = {false};
+    int8_t col_seen[TGPU_MAX_CHANNELS] = {0};     // 1 read as a DECIMAL, 2 as something else
+    auto valid = [](const tgpu_decimal_type& t) { return t.precision >= 1 && t.precision <= 38 && t.scale >= 0 && t.scale <= t.precision; };
+    // does a value fit DECIMAL(t)?  (hi, lo) two's complement
+    auto fits = [](const DecType& t, long long hi, long long lo) {
+        const U128 v{(unsigned long long)hi, (unsigned long long)lo};
+        return !u128_exceeds_precision(v, t.p);
+    };
+    for (int i = 0; i < p->num_insns; i++) {
+        const tgpu_expr_insn& s = p->insns[i];
+        DInsn& d = out->insns[i];
+        const tgpu_operand* ops[3] = {&s.a, &s.b, &s.c};
+        DOperand* dops[3] = {&d.a, &d.b, &d.c};
+        const bool unary = s.op == TGPU_EX_MOV || s.op == TGPU_EX_NEG || s.op == TGPU_EX_IS_NULL || s.op == TGPU_EX_IS_NOT_NULL || s.op == TGPU_EX_IN ||
+                           s.op == TGPU_EX_CAST_TO_DECIMAL || s.op == TGPU_EX_CAST_DECIMAL_TO_BIGINT || s.op == TGPU_EX_CAST_DECIMAL_TO_DOUBLE ||
+                           s.op == TGPU_EX_NOT;
+        const int used = unary ? 1 : s.op == TGPU_EX_BETWEEN ? 3 : 2;
+        if (!dec_insn(s)) {
+            // a numeric instruction never reads a DECIMAL temp or a channel read as DECIMAL
+            for (int k = 0; k < used && k < 3; k++) {
+                if (s.op == TGPU_EX_IN && k > 0) break;
+                if (ops[k]->kind == TGPU_OPND_TEMP && temp_t[ops[k]->index].p)
+                    return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads DECIMAL temp %d as another type", i, ops[k]->index);
+                if (ops[k]->kind == TGPU_OPND_COLUMN && s.vtype != TGPU_V_VARCHAR && s.op != TGPU_EX_LIKE) {
+                    if (col_seen[ops[k]->index] == 1) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads DECIMAL channel %d as another type", i, ops[k]->index);
+                    col_seen[ops[k]->index] = 2;
+                }
+            }
+            temp_t[s.dst] = DecType{};
+            temp_written[s.dst] = true;
+            continue;
+        }
+        const tgpu_decimal_signature& sig = p->decimal_signatures[i];
+        DDec& x = out->dec[i];
+        memset(&x, 0, sizeof(x));
+        x.is_dec = 1;
+        // which operands and result are DECIMAL
+        bool opnd_dec = s.vtype == TGPU_V_DECIMAL;
+        bool res_dec = false;
+        switch (s.op) {
+            case TGPU_EX_MOV: case TGPU_EX_ADD: case TGPU_EX_SUB: case TGPU_EX_MUL: case TGPU_EX_DIV: case TGPU_EX_NEG: res_dec = true; break;
+            case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE: case TGPU_EX_BETWEEN:
+            case TGPU_EX_IN: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: break;
+            case TGPU_EX_CAST_TO_DECIMAL:
+                if (s.vtype == TGPU_V_DOUBLE) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: CAST(DOUBLE AS DECIMAL) is not evaluated on the GPU", i);
+                if (s.vtype != TGPU_V_BIGINT && s.vtype != TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: CAST to DECIMAL reads BIGINT or DECIMAL", i);
+                res_dec = true;
+                break;
+            case TGPU_EX_CAST_DECIMAL_TO_BIGINT: case TGPU_EX_CAST_DECIMAL_TO_DOUBLE:
+                if (s.vtype != TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: this cast reads a DECIMAL operand", i);
+                break;
+            case TGPU_EX_MOD: return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: DECIMAL %% is not evaluated on the GPU", i);
+            default: return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: op %d does not take DECIMAL operands", i, s.op);
+        }
+        DecType ot[3], rt;
+        const tgpu_decimal_type* st[3] = {&sig.a, &sig.b, &sig.c};
+        const int nopnd = s.op == TGPU_EX_IN ? 1 : used;
+        for (int k = 0; k < nopnd; k++) {
+            if (!opnd_dec) continue;
+            if (!valid(*st[k])) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad DECIMAL type of operand %d", i, k);
+            ot[k] = DecType{st[k]->precision, st[k]->scale};
+        }
+        if (res_dec) {
+            if (!valid(sig.result)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad DECIMAL result type", i);
+            rt = DecType{sig.result.precision, sig.result.scale};
+        }
+        // operands: temps carry their writer's type, a channel one type throughout, constants fit their type
+        for (int k = 0; k < nopnd; k++) {
+            const tgpu_operand& o = *ops[k];
+            if (o.kind == TGPU_OPND_TEMP) {
+                if (!temp_written[o.index] || !(temp_t[o.index] == ot[k]))
+                    return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: temp %d does not hold the operand's type", i, o.index);
+            }
+            else if (o.kind == TGPU_OPND_COLUMN) {
+                if (!opnd_dec) {
+                    if (col_seen[o.index] == 1) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads DECIMAL channel %d as another type", i, o.index);
+                    col_seen[o.index] = 2;
+                }
+                else {
+                    if (col_seen[o.index] == 2 || (col_seen[o.index] == 1 && !(col_t[o.index] == ot[k])))
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d with another type", i, o.index);
+                    col_seen[o.index] = 1;
+                    col_t[o.index] = ot[k];
+                }
+            }
+            else if (o.kind == TGPU_OPND_CONST && opnd_dec) {
+                long long hi = o.imm.i64 >> 63, lo = o.imm.i64;
+                if (ot[k].lng()) {
+                    if (o.imm.i64 < 0 || o.imm.i64 >= p->num_decimal_constants)
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: decimal constant index out of range", i);
+                    hi = p->decimal_constants[2 * o.imm.i64];
+                    lo = p->decimal_constants[2 * o.imm.i64 + 1];
+                    x.hi[k] = hi;
+                    dops[k]->imm = lo;
+                }
+                if (!fits(ot[k], hi, lo)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: constant does not fit DECIMAL(%d, %d)", i, ot[k].p, ot[k].s);
+            }
+        }
+        if (s.op == TGPU_EX_IN) {
+            const tgpu_in_list& l = p->in_lists[s.b.imm.i64];
+            const int off = out->in_offset[s.b.imm.i64];
+            for (int k = 0; k < l.count; k++) {
+                long long hi = l.values[k] >> 63, lo = l.values[k];
+                if (ot[0].lng()) {
+                    if (l.values[k] < 0 || l.values[k] >= p->num_decimal_constants)
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: decimal constant index out of range", i);
+                    hi = p->decimal_constants[2 * l.values[k]];
+                    lo = p->decimal_constants[2 * l.values[k] + 1];
+                }
+                if (!fits(ot[0], hi, lo)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: IN value does not fit DECIMAL(%d, %d)", i, ot[0].p, ot[0].s);
+                out->in_values[off + k] = lo;
+                out->in_hi[off + k] = hi;
+            }
+        }
+        const bool cmp = s.op == TGPU_EX_EQ || s.op == TGPU_EX_NE || s.op == TGPU_EX_LT || s.op == TGPU_EX_LE || s.op == TGPU_EX_GT || s.op == TGPU_EX_GE ||
+                         s.op == TGPU_EX_BETWEEN;
+        if (cmp && !(ot[0] == ot[1] && (s.op != TGPU_EX_BETWEEN || ot[0] == ot[2])))
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: compared DECIMAL operands have different types", i);
+        if ((s.op == TGPU_EX_MOV || s.op == TGPU_EX_NEG) && !(rt == ot[0]))
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: the result has another type than the operand", i);
+        x.la = ot[0].lng();
+        x.lb = ot[1].lng();
+        x.lc = ot[2].lng();
+        x.lr = rt.lng();
+        const bool any_long = x.la || x.lb;
+        switch (s.op) {
+            case TGPU_EX_ADD: case TGPU_EX_SUB: {
+                const int ar = std::max(0, ot[1].s - ot[0].s), br = std::max(0, ot[0].s - ot[1].s);
+                if (!any_long && !x.lr) { x.m0 = pow10_i64(ar); x.m1 = pow10_i64(br); }
+                else {
+                    if (!x.lr) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a long operand needs a long result", i);
+                    x.k0 = ar == 0 ? br : ar;
+                    x.k1 = ar == 0 ? 0 : 1;
+                    x.k2 = rt.s - std::max(ot[0].s, ot[1].s);
+                }
+                break;
+            }
+            case TGPU_EX_MUL:
+                if (any_long && !x.lr) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a long operand needs a long result", i);
+                x.k2 = rt.s - (ot[0].s + ot[1].s);
+                break;
+            case TGPU_EX_DIV:
+                x.k0 = rt.s - ot[0].s + ot[1].s;
+                if (x.la && x.lb && !x.lr) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: DECIMAL long / long -> short has no method", i);
+                if (!any_long && !x.lr) {
+                    if (x.k0 < 0 || x.k0 > 18) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: short DECIMAL division rescales by 10^%d", i, x.k0);
+                    x.m0 = pow10_i64(x.k0);
+                }
+                break;
+            case TGPU_EX_CAST_TO_DECIMAL:
+                x.k0 = rt.p;
+                if (s.vtype == TGPU_V_BIGINT) {
+                    x.k1 = rt.s;
+                    if (!x.lr) x.m0 = pow10_i64(rt.s);
+                }
+                else {
+                    x.k1 = rt.s - ot[0].s;
+                    x.k2 = rt == ot[0] ? 1 : 0;
+                    if (!x.la && !x.lr) { x.m0 = pow10_i64(std::abs(x.k1)); x.m1 = x.m0 / 2; }
+                }
+                break;
+            case TGPU_EX_CAST_DECIMAL_TO_BIGINT: case TGPU_EX_CAST_DECIMAL_TO_DOUBLE:
+                x.k1 = ot[0].s;
+                if (!x.la) x.m0 = pow10_i64(ot[0].s);
+                break;
+            default: break;
+        }
+        temp_t[s.dst] = res_dec ? rt : DecType{};
+        temp_written[s.dst] = true;
+        if (res_dec && rt.lng()) out->long_temps |= 1u << s.dst;
+    }
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) out->temp_dec[t] = temp_t[t].p == 0 ? 0 : temp_t[t].lng() ? 2 : 1;
+    return TGPU_OK;
+}
+
 bool expr_uses_strings(const DProgram& prog)
 {
     for (int i = 0; i < prog.num_insns; i++)
@@ -299,7 +506,7 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         const tgpu_expr_insn& s = p->insns[i];
         DInsn& d = out->insns[i];
         if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
-        if (s.vtype < 0 || s.vtype > TGPU_V_VARCHAR) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
+        if (s.vtype < 0 || s.vtype > TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
         if (s.vtype == TGPU_V_VARCHAR || s.op == TGPU_EX_LIKE) {
             TG_TRY(compile_varchar_insn(ctx, p, i, out, max_channel));
             continue;
@@ -309,6 +516,7 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
             case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE:
             case TGPU_EX_AND: case TGPU_EX_OR: case TGPU_EX_NOT: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: case TGPU_EX_BETWEEN:
             case TGPU_EX_CAST_BIGINT_TO_DOUBLE: case TGPU_EX_CAST_DOUBLE_TO_BIGINT:
+            case TGPU_EX_CAST_TO_DECIMAL: case TGPU_EX_CAST_DECIMAL_TO_BIGINT: case TGPU_EX_CAST_DECIMAL_TO_DOUBLE:
                 break;
             case TGPU_EX_IN:
                 if (s.b.imm.i64 < 0 || s.b.imm.i64 >= p->num_in_lists) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: IN list index out of range", i);
@@ -324,13 +532,14 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         TG_TRY(conv(s.c, &d.c));
         if (s.op == TGPU_EX_IN) d.b.kind = TGPU_OPND_CONST;
     }
-    return TGPU_OK;
+    return compile_decimals(ctx, p, out);
 }
 
 int expr_raise(tgpu_ctx* ctx, int64_t errbits)
 {
     if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
     if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
+    if (errbits & TG_ERR_BIT_DECIMAL_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "Decimal overflow");
     if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
     return TGPU_OK;
 }
@@ -483,11 +692,64 @@ static std::string fp_string_decls(const DProgram& prog)
     return s;
 }
 
+// a DECIMAL operand of generated code as a DVal (`lng`: a long decimal: locals ch<k> / th<i> hold the high words)
+static std::string fp_dec_operand(const DOperand& o, bool lng, long long khi)
+{
+    char buf[160];
+    switch (o.kind) {
+        case TGPU_OPND_COLUMN:
+            if (lng) snprintf(buf, sizeof(buf), "DVal{U128{(unsigned long long)ch%d, (unsigned long long)c%d}, c%dn}", o.index, o.index, o.index);
+            else snprintf(buf, sizeof(buf), "DVal{u128_sx(c%d), c%dn}", o.index, o.index);
+            break;
+        case TGPU_OPND_TEMP:
+            if (lng) snprintf(buf, sizeof(buf), "DVal{U128{(unsigned long long)th%d, (unsigned long long)t%d}, tn%d}", o.index, o.index, o.index);
+            else snprintf(buf, sizeof(buf), "DVal{u128_sx(t%d), tn%d}", o.index, o.index);
+            break;
+        case TGPU_OPND_CONST:
+            snprintf(buf, sizeof(buf), "DVal{U128{0x%llxULL, 0x%llxULL}, false}", lng ? (unsigned long long)khi : (unsigned long long)(o.imm >> 63),
+                     (unsigned long long)o.imm);
+            break;
+        default: snprintf(buf, sizeof(buf), "DVal{U128{0ULL, 0ULL}, true}"); break;
+    }
+    return buf;
+}
+
+// straight-line code of one DECIMAL instruction: vm_apply_dec with the instruction's method as constants, so that the compiler keeps only
+// that method's path (a short one stays 64-bit code with 10^k as immediates); the high word is kept for long results only
+static void fp_emit_dec_insn(std::string& s, const DProgram& prog, int i)
+{
+    const DInsn& in = prog.insns[i];
+    const DDec& d = prog.dec[i];
+    const bool long_dst = (prog.long_temps >> in.dst) & 1;
+    if (in.op == TGPU_EX_IN) {
+        const int li = (int)in.b.imm;
+        fp_appendf(s, "    { DVal a = %s; bool hit = false;\n", fp_dec_operand(in.a, d.la, 0).c_str());
+        for (int k = 0; k < prog.in_count[li]; k++) {
+            const int at = prog.in_offset[li] + k;
+            const unsigned long long lo = (unsigned long long)prog.in_values[at], hi = d.la ? (unsigned long long)prog.in_hi[at] : (unsigned long long)(prog.in_values[at] >> 63);
+            fp_appendf(s, "      hit |= a.v.hi == 0x%llxULL && a.v.lo == 0x%llxULL;\n", hi, lo);
+        }
+        fp_appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s;%s }\n", in.dst, in.dst, in.dst, fp_operand_error(in.a).c_str(),
+                   long_dst ? (" th" + std::to_string(in.dst) + " = 0;").c_str() : "");
+        return;
+    }
+    fp_appendf(s, "    { DVal a = %s, b = %s, c = %s; unsigned int e = 0;\n", fp_dec_operand(in.a, d.la, d.hi[0]).c_str(), fp_dec_operand(in.b, d.lb, d.hi[1]).c_str(),
+               fp_dec_operand(in.c, d.lc, d.hi[2]).c_str());
+    fp_appendf(s, "      const DDec dd = {1, %d, %d, %d, %d, 0, 0, 0, %d, %d, %d, 0, %lldLL, %lldLL, {0, 0, 0}};\n", d.la, d.lb, d.lc, d.lr, d.k0, d.k1, d.k2,
+               d.m0, d.m1);
+    fp_appendf(s, "      DVal x = vm_apply_dec(%d, %d, dd, a, b, c, &e);\n", in.op, in.vtype);
+    fp_appendf(s, "      e = vm_error_dec(%d, a, %s, b, %s, %s, e); t%d = (long long)x.v.lo; tn%d = x.is_null; te%d = e;", in.op, fp_operand_error(in.a).c_str(),
+               fp_operand_error(in.b).c_str(), fp_operand_error(in.c).c_str(), in.dst, in.dst, in.dst);
+    if (long_dst) fp_appendf(s, " th%d = (long long)x.v.hi;", in.dst);
+    s += " }\n";
+}
+
 void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
 {
     for (int i = first; i < last; i++) {
         const DInsn& in = prog.insns[i];
-        if (in.vtype == TGPU_V_VARCHAR) fp_emit_str_insn(s, prog, in);
+        if (prog.has_dec && prog.dec[i].is_dec) fp_emit_dec_insn(s, prog, i);
+        else if (in.vtype == TGPU_V_VARCHAR) fp_emit_str_insn(s, prog, in);
         else if (in.op == TGPU_EX_IN) {
             int li = (int)in.b.imm;
             fp_appendf(s, "    { Value a = %s; bool hit = false;\n", fp_operand(in.a).c_str());
@@ -518,17 +780,21 @@ constexpr int FP_THREADS = 256;
 
 // ---- NVRTC specialisation of the two PageProcessor kernels ----------------------------------------------------------
 
-// filter pass: one row per thread, writes 1/0 selection flags
+// filter pass: one row per thread, writes 1/0 selection flags.  DEC: the program holds DECIMAL operations, whose temps keep a high word
+// in a second shared lane (programs without DECIMAL keep the shared memory and occupancy they had)
+template <bool DEC>
 __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* __restrict__ prog, DColumns cols, StrCols strs, int64_t n, uint8_t* __restrict__ flags,
                                                               unsigned int* __restrict__ err_out)
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
+    __shared__ int64_t temps_hi[DEC ? TGPU_MAX_TEMPS * FP_THREADS : 1];
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t err = 0;
     for (; i < n; i += stride) {
         uint32_t te = 0;
-        uint32_t nb = vm_run<true>(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te, 0, 0, &strs);
+        uint32_t nb = vm_run<true, DEC>(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te, 0, 0, &strs,
+                                        DEC ? temps_hi + threadIdx.x : nullptr);
         int ft = prog->filter_temp;
         err |= vm_temp_error(te, ft);
         bool sel = !((nb >> ft) & 1) && temps[ft * FP_THREADS + threadIdx.x] != 0;
@@ -538,24 +804,31 @@ __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* _
 }
 
 // projection pass: output row j <- input row sel[j] (sel == nullptr: identity)
+template <bool DEC>
 __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* __restrict__ prog, DColumns cols, StrCols strs, const int32_t* __restrict__ sel, int64_t m,
                                                                OutCols out, unsigned int* __restrict__ err_out, unsigned int* __restrict__ any_null)
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
+    __shared__ int64_t temps_hi[DEC ? TGPU_MAX_TEMPS * FP_THREADS : 1];
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t err = 0, nulls_seen = 0;
     for (; j < m; j += stride) {
         int64_t row = sel ? sel[j] : j;
         int64_t* t = temps + threadIdx.x;
+        int64_t* th = DEC ? temps_hi + threadIdx.x : nullptr;
         uint32_t te = 0;
-        uint32_t nb = vm_run<true>(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te, 0, 0, &strs);
+        uint32_t nb = vm_run<true, DEC>(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te, 0, 0, &strs, th);
         for (int c = 0; c < out.count; c++) {
             int tp = out.temp[c];
             err |= vm_temp_error(te, tp);
             bool isn = (nb >> tp) & 1;
             int64_t v = isn ? 0 : t[tp * FP_THREADS];
-            if (out.vtype[c] == TGPU_V_BOOLEAN) ((int8_t*)out.data[c])[j] = (int8_t)v;
+            if (DEC && out.vtype[c] == TGD_V_DECIMAL_LONG) {
+                ((int64_t*)out.data[c])[2 * j] = isn ? 0 : th[tp * FP_THREADS];
+                ((int64_t*)out.data[c])[2 * j + 1] = v;
+            }
+            else if (out.vtype[c] == TGPU_V_BOOLEAN) ((int8_t*)out.data[c])[j] = (int8_t)v;
             else ((int64_t*)out.data[c])[j] = v;
             out.nullmap[c][j] = isn ? 1 : 0;
             if (isn) nulls_seen |= 1u << c;
@@ -571,24 +844,43 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
 {
     std::string s = fp_string_decls(prog);
     bool used[TGPU_MAX_CHANNELS] = {false}, str_used[TGPU_MAX_CHANNELS] = {false};     // read as a number / as a string
+    bool wide_used[TGPU_MAX_CHANNELS] = {false};                                      // read as a long DECIMAL
     for (int i = 0; i < prog.num_insns; i++) {
         const DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
-        for (auto* o : ops)
-            if (o->kind == TGPU_OPND_COLUMN) (prog.insns[i].vtype == TGPU_V_VARCHAR ? str_used : used)[o->index] = true;
+        const DDec& d = prog.dec[i];
+        const bool lng[3] = {d.la != 0, d.lb != 0, d.lc != 0};
+        for (int k = 0; k < 3; k++)
+            if (ops[k]->kind == TGPU_OPND_COLUMN) (prog.insns[i].vtype == TGPU_V_VARCHAR ? str_used : lng[k] ? wide_used : used)[ops[k]->index] = true;
     }
     std::string loads, temps;
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        if (!used[c] && !str_used[c]) continue;
-        if (used[c]) fp_appendf(loads, "    const long long c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
+        if (!used[c] && !str_used[c] && !wide_used[c]) continue;
+        if (wide_used[c])
+            fp_appendf(loads, "    const longlong2 c%dw = ((const longlong2*)cols.cols[%d].data)[row]; const long long ch%d = c%dw.x, c%d = c%dw.y;", c, c, c, c, c, c);
+        else if (used[c]) fp_appendf(loads, "    const long long c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
         if ((nullable_mask >> c) & 1) fp_appendf(loads, " const bool c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
         else fp_appendf(loads, " const bool c%dn = false;\n", c);
         if (str_used[c]) fp_appendf(loads, "    const StrRef s%d = tg_str(strs, %d, row);\n", c, prog.str_slot[c]);
     }
     for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    // high words of the temps that hold a long DECIMAL
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++)
+        if ((prog.long_temps >> t) & 1) fp_appendf(temps, "    long long th%d = 0;\n", t);
+    const bool wide_out = prog.long_temps != 0;
     // value, NULL flag and carried error of the temp behind each computed output column (the only errors a projection raises)
-    std::string output_switch = "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true; unsigned int e = 0;\n      switch (out.temp[c]) {\n";
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(output_switch, "        case %d: v = t%d; isn = tn%d; e = te%d; break;\n", t, t, t, t);
+    std::string output_switch = "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true; unsigned int e = 0;\n";
+    if (wide_out) output_switch += "      long long hv = 0;\n";
+    output_switch += "      switch (out.temp[c]) {\n";
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) {
+        if ((prog.long_temps >> t) & 1) fp_appendf(output_switch, "        case %d: v = t%d; hv = th%d; isn = tn%d; e = te%d; break;\n", t, t, t, t, t);
+        else fp_appendf(output_switch, "        case %d: v = t%d; isn = tn%d; e = te%d; break;\n", t, t, t, t);
+    }
     output_switch += "      }\n      err |= e;\n      if (isn) v = 0;\n";
+    // the store of one computed output cell: a long DECIMAL writes a 16-byte (high, low) cell
+    std::string store = "      if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
+    if (wide_out)
+        store = "      if (isn) hv = 0;\n      if (out.vtype[c] == TGD_V_DECIMAL_LONG) ((longlong2*)out.data[c])[j] = make_longlong2(hv, v);\n"
+                "      else if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
     // filter kernel
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_jit(DColumns cols, StrCols strs, long long n, unsigned char* flags, unsigned int* err_out) {\n";
     s += "  unsigned int err = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
@@ -606,7 +898,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     s += loads + temps;
     fp_emit_insns(s, prog, 0, prog.num_insns);
     s += output_switch;
-    s += "      if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
+    s += store;
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
     s += "  }\n  if (err) atomicOr(err_out, err);\n  if (nulls_seen) atomicOr(any_null, nulls_seen);\n}\n";
     // chunked two-pass form (no selection vector): per-row functors + the two kernels around the bodies of device_lib.cuh
@@ -624,7 +916,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     s += loads + temps;
     fp_emit_insns(s, prog, 0, prog.num_insns);
     s += output_switch;
-    s += "      if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
+    s += store;
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
     for (size_t k = 0; k < pass_channels.size(); k++) {
         int ch = pass_channels[k];
@@ -703,6 +995,19 @@ struct FilterProjectOp : tgpu_op {
         for (int i = 0; i < host_prog.num_insns; i++) {
             const DOperand* ops[3] = {&host_prog.insns[i].a, &host_prog.insns[i].b, &host_prog.insns[i].c};
             const bool str = host_prog.insns[i].vtype == TGPU_V_VARCHAR;
+            const DDec& dd = host_prog.dec[i];
+            if (dd.is_dec && host_prog.insns[i].vtype == TGPU_V_DECIMAL) {
+                // a short DECIMAL channel is TGPU_INT64, a long one TGPU_INT128
+                const bool lng[3] = {dd.la != 0, dd.lb != 0, dd.lc != 0};
+                for (int k = 0; k < 3; k++) {
+                    if (ops[k]->kind != TGPU_OPND_COLUMN) continue;
+                    const int want = lng[k] ? TGPU_INT128 : TGPU_INT64;
+                    if (in.cols[ops[k]->index].type != want)
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d as a %s DECIMAL, the page's channel is not %s", i, ops[k]->index,
+                                       lng[k] ? "long" : "short", lng[k] ? "INT128" : "INT64");
+                }
+                continue;
+            }
             for (auto* o : ops) {
                 if (o->kind != TGPU_OPND_COLUMN) continue;
                 if (str && in.cols[o->index].type != TGPU_UTF8)
@@ -745,7 +1050,8 @@ struct FilterProjectOp : tgpu_op {
                 void* params[5] = {&cols, &strs, &n_arg, &f_arg, &d_err};
                 TG_TRY(jit_launch(ctx, jit_filter, tg_grid(ctx, n, FP_THREADS, jit_blocks_per_sm(jit_filter, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
-            else TG_LAUNCH(ctx, fp_filter_kernel, grid, FP_THREADS, 0, dp, cols, strs, n, flags.as<uint8_t>(), d_err);
+            else if (host_prog.has_dec) TG_LAUNCH(ctx, fp_filter_kernel<true>, grid, FP_THREADS, 0, dp, cols, strs, n, flags.as<uint8_t>(), d_err);
+            else TG_LAUNCH(ctx, fp_filter_kernel<false>, grid, FP_THREADS, 0, dp, cols, strs, n, flags.as<uint8_t>(), d_err);
             long long* d_count = &ctx->d_scratch->fp_count;
             TG_TRY(tg_flagged_positions(ctx, flags.as<uint8_t>(), n, &sel, d_count));
             TG_TRY(tg_read_i64(ctx, d_count, &m));
@@ -777,7 +1083,8 @@ struct FilterProjectOp : tgpu_op {
                 void* params[7] = {&cols, &strs, &d_sel, &m_arg, &cc.oc, &d_err, &d_anynull};
                 TG_TRY(jit_launch(ctx, jit_project, tg_grid(ctx, m, FP_THREADS, jit_blocks_per_sm(jit_project, FP_THREADS, 0)), FP_THREADS, 0, params));
             }
-            else TG_LAUNCH(ctx, fp_project_kernel, pgrid, FP_THREADS, 0, dp, cols, strs, d_sel, m, cc.oc, d_err, d_anynull);
+            else if (host_prog.has_dec) TG_LAUNCH(ctx, fp_project_kernel<true>, pgrid, FP_THREADS, 0, dp, cols, strs, d_sel, m, cc.oc, d_err, d_anynull);
+            else TG_LAUNCH(ctx, fp_project_kernel<false>, pgrid, FP_THREADS, 0, dp, cols, strs, d_sel, m, cc.oc, d_err, d_anynull);
             TG_TRY(finish_computed(cc, d_err, &outp));
         }
         pending.push_back(tg_make_owned_page(std::move(outp)));
@@ -796,7 +1103,8 @@ struct FilterProjectOp : tgpu_op {
     int add_computed(const tgpu_projection& pr, int64_t m, int pi, DevPage* outp, ComputedCols* cc)
     {
         DevColumn& c = outp->cols[pi];
-        c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : TGPU_INT64;
+        const bool wide = pr.vtype == TGPU_V_DECIMAL && host_prog.temp_dec[pr.index] == 2;     // a long DECIMAL: 16-byte cells
+        c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : wide ? TGPU_INT128 : TGPU_INT64;
         c.length = m;
         c.own_data = std::make_shared<DevBuf>();
         TG_TRY(c.own_data->alloc(ctx, (size_t)m * c.elem_size()));
@@ -805,7 +1113,7 @@ struct FilterProjectOp : tgpu_op {
         TG_TRY(nm->alloc(ctx, (size_t)m));
         int k = cc->oc.count++;
         cc->oc.temp[k] = pr.index;
-        cc->oc.vtype[k] = pr.vtype;
+        cc->oc.vtype[k] = wide ? TGD_V_DECIMAL_LONG : pr.vtype == TGPU_V_DECIMAL ? TGPU_V_BIGINT : pr.vtype;
         cc->oc.data[k] = c.own_data->p;
         cc->oc.nullmap[k] = nm->as<uint8_t>();
         cc->nullmaps.push_back(std::move(nm));
@@ -953,7 +1261,13 @@ struct FilterProjectOp : tgpu_op {
         return TGPU_OK;
     }
 
-    int raise(int64_t errbits) { return expr_raise(ctx, errbits); }
+    int raise(int64_t errbits)
+    {
+        // in a program with DECIMAL the invalid-cast bit may come from a DECIMAL cast as well as from CAST(DOUBLE AS BIGINT)
+        if (host_prog.has_dec && !(errbits & (TG_ERR_BIT_DIV_ZERO | TG_ERR_BIT_OVERFLOW)) && (errbits & TG_ERR_BIT_INVALID_CAST))
+            return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Cannot cast value: it does not fit the target type");
+        return expr_raise(ctx, errbits);
+    }
 
     int get_output(OwnedPage** out) override
     {
@@ -977,6 +1291,10 @@ extern "C" int tgpu_filter_project_create(tgpu_ctx* ctx, const tgpu_expr_program
     for (int i = 0; i < program->num_projections; i++) {
         const tgpu_projection& p = program->projections[i];
         if (p.kind == 1 && (p.index < 0 || p.index >= TGPU_MAX_TEMPS)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "projection temp out of range");
+        if (p.kind == 1 && p.vtype == TGPU_V_DECIMAL && op->host_prog.temp_dec[p.index] == 0)
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "projection %d: temp %d does not hold a DECIMAL", i, p.index);
+        if (p.kind == 1 && p.vtype != TGPU_V_DECIMAL && op->host_prog.temp_dec[p.index] != 0)
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "projection %d: temp %d holds a DECIMAL, the projection's type is %d", i, p.index, p.vtype);
         op->projections.push_back(p);
     }
     TG_TRY(op->d_prog.alloc(ctx, sizeof(tg::DProgram)));

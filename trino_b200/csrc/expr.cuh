@@ -53,10 +53,20 @@ struct DProgram {
     int32_t str_pad;
     uint8_t str_bytes[TGPU_MAX_STRING_BYTES];
     DLike likes[TGPU_MAX_LIKE_PATTERNS];
+    // DECIMAL operands (FilterAndProject only): the reference's method of each DECIMAL instruction (dec[i].is_dec), the high words of
+    // long DECIMAL IN-list values, and what each temp holds after the program ran (temp_dec: 0 not a decimal, 1 short, 2 long).
+    // long_temps: the temps that ever hold a long decimal (they get a high word)
+    int32_t has_dec;
+    uint32_t long_temps;
+    int8_t temp_dec[TGPU_MAX_TEMPS];
+    DDec dec[TGPU_MAX_INSNS];
+    int64_t in_hi[128];
 };
 
 // the program has an instruction over VARCHAR operands (or a LIKE)
 bool expr_uses_strings(const DProgram& prog);
+// the program has an instruction over DECIMAL operands or with a DECIMAL result
+inline bool expr_uses_decimals(const DProgram& prog) { return prog.has_dec != 0; }
 
 
 #if defined(__CUDACC__)
@@ -163,15 +173,82 @@ __device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog,
     }
 }
 
-// STR: the program may hold string operations (FilterAndProject), read through `strs`
-template <bool STR = false>
+// A DECIMAL operand (or the BIGINT operand of a cast to DECIMAL) as a 128-bit value: `lng` = a long decimal (a TGPU_INT128 channel's
+// (high, low) cell, a temp's high-word lane `thi`, or a constant whose high word is `khi`); anything else is sign-extended
+__device__ __forceinline__ DVal vm_fetch_dec(const DOperand& o, bool lng, long long khi, const DColumns& cols, int64_t row, const int64_t* temps,
+                                             const int64_t* thi, int tstride, uint32_t nullbits)
+{
+    DVal v;
+    v.v = U128{0ULL, 0ULL};
+    v.is_null = true;
+    switch (o.kind) {
+        case TGPU_OPND_COLUMN: {
+            const ColRef& c = cols.cols[o.index];
+            v.is_null = !tg_valid(c.validity, row);
+            if (lng) v.v = U128{(unsigned long long)((const int64_t*)c.data)[2 * row], (unsigned long long)((const int64_t*)c.data)[2 * row + 1]};
+            else v.v = u128_sx(tg_load_i64(c, row));
+            break;
+        }
+        case TGPU_OPND_TEMP:
+            v.is_null = (nullbits >> o.index) & 1;
+            v.v = lng ? U128{(unsigned long long)thi[o.index * tstride], (unsigned long long)temps[o.index * tstride]} : u128_sx(temps[o.index * tstride]);
+            break;
+        case TGPU_OPND_CONST:
+            v.is_null = false;
+            v.v = lng ? U128{(unsigned long long)khi, (unsigned long long)o.imm} : u128_sx(o.imm);
+            break;
+        default: break;
+    }
+    return v;
+}
+
+// One DECIMAL instruction of the interpreter: result value in temps / thi, NULL flag and error as the numeric ones
+__device__ __forceinline__ void vm_step_dec(const DProgram* __restrict__ prog, const DInsn& in, const DDec& d, const DColumns& cols, int64_t row,
+                                            int64_t* temps, int64_t* thi, int tstride, uint32_t* nullbits, uint32_t* te)
+{
+    const DVal a = vm_fetch_dec(in.a, d.la, d.hi[0], cols, row, temps, thi, tstride, *nullbits);
+    DVal r;
+    uint32_t e;
+    if (in.op == TGPU_EX_IN) {
+        r.is_null = a.is_null;
+        r.v = U128{0ULL, 0ULL};
+        const int li = (int)in.b.imm;
+        bool hit = false;
+        for (int k = 0; k < prog->in_count[li]; k++) {
+            const int at = prog->in_offset[li] + k;
+            const U128 x = d.la ? U128{(unsigned long long)prog->in_hi[at], (unsigned long long)prog->in_values[at]} : u128_sx(prog->in_values[at]);
+            hit |= x.hi == a.v.hi && x.lo == a.v.lo;
+        }
+        r.v.lo = hit && !a.is_null ? 1ULL : 0ULL;
+        e = vm_carried(in.a, *te);
+    }
+    else {
+        const DVal b = vm_fetch_dec(in.b, d.lb, d.hi[1], cols, row, temps, thi, tstride, *nullbits);
+        const DVal c = vm_fetch_dec(in.c, d.lc, d.hi[2], cols, row, temps, thi, tstride, *nullbits);
+        uint32_t own = 0;
+        r = vm_apply_dec(in.op, in.vtype, d, a, b, c, &own);
+        e = vm_error_dec(in.op, a, vm_carried(in.a, *te), b, vm_carried(in.b, *te), vm_carried(in.c, *te), own);
+    }
+    temps[in.dst * tstride] = (int64_t)r.v.lo;
+    thi[in.dst * tstride] = (int64_t)r.v.hi;
+    *nullbits = (*nullbits & ~(1u << in.dst)) | ((r.is_null ? 1u : 0u) << in.dst);
+    *te = (*te & ~(0xFu << (4 * in.dst))) | (e << (4 * in.dst));
+}
+
+// STR: the program may hold string operations (FilterAndProject), read through `strs`.  DEC: the program may hold DECIMAL operations
+// (FilterAndProject), whose temps keep their high words in `thi` (same layout as `temps`)
+template <bool STR = false, bool DEC = false>
 __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
                                            int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs, int split = 0, int64_t split_row = 0,
-                                           const StrCols* strs = nullptr)
+                                           const StrCols* strs = nullptr, int64_t* thi = nullptr)
 {
     uint32_t te = *errs;
     for (int pc = first; pc < last; pc++) {
         const DInsn& in = prog->insns[pc];
+        if (DEC && prog->dec[pc].is_dec) {
+            vm_step_dec(prog, in, prog->dec[pc], cols, row, temps, thi, tstride, &nullbits, &te);
+            continue;
+        }
         if (STR && in.vtype == TGPU_V_VARCHAR) {
             const Value v = vm_apply_str(prog, in, cols, *strs, row);
             temps[in.dst * tstride] = v.bits;

@@ -3464,6 +3464,8 @@ int build_agg_op(tgpu_ctx* ctx, const tgpu_agg_spec* spec, AggOp** out)
         TG_TRY(tg::expr_compile(ctx, spec->pre, &op->host_prog, &op->prog_max_channel));
         if (tg::expr_uses_strings(op->host_prog))
             return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "the fused pre-stage does not evaluate VARCHAR operations: put a FilterAndProject in front");
+        if (tg::expr_uses_decimals(op->host_prog))
+            return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "the fused pre-stage does not evaluate DECIMAL operations: put a FilterAndProject in front");
         op->projections.assign(spec->pre->projections, spec->pre->projections + spec->pre->num_projections);
         op->pre_insns.assign(spec->pre->insns, spec->pre->insns + spec->pre->num_insns);
         for (int i = 0; i < spec->pre->num_in_lists; i++)
@@ -3630,6 +3632,7 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
             int st = tg::expr_compile(&fake, spec->pre, &o->host_prog, &o->prog_max_channel);
             if (st != TGPU_OK) return st;
             if (tg::expr_uses_strings(o->host_prog)) return TGPU_ERR_NOT_SUPPORTED;
+            if (tg::expr_uses_decimals(o->host_prog)) return TGPU_ERR_NOT_SUPPORTED;
             o->projections.assign(spec->pre->projections, spec->pre->projections + spec->pre->num_projections);
         }
         op = o.release();

@@ -1524,6 +1524,7 @@ int join_filter_compile(tgpu_ctx* ctx, const tgpu_expr_program* program, int32_t
     int32_t max_channel = -1;
     TG_TRY(tg::expr_compile(ctx, program, out, &max_channel));
     if (tg::expr_uses_strings(*out)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters do not evaluate VARCHAR operations");
+    if (tg::expr_uses_decimals(*out)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters do not evaluate DECIMAL operations");
     return TGPU_OK;
 }
 

@@ -294,15 +294,18 @@ class OperatorFactory:
 
 # ---- expressions ----------------------------------------------------------------------------------
 class Col:
-    def __init__(self, channel, vtype):
-        self.channel, self.vtype = channel, vtype
+    """dtype: (precision, scale) of a V_DECIMAL channel (a short decimal is an INT64 channel, a long one INT128)"""
+
+    def __init__(self, channel, vtype, dtype=None):
+        self.channel, self.vtype, self.dtype = channel, vtype, dtype
 
 
 class Const:
-    """value: int / float / bool, or str / bytes for V_VARCHAR (a str is taken as its UTF-8 bytes)"""
+    """value: int / float / bool, or str / bytes for V_VARCHAR (a str is taken as its UTF-8 bytes), or the unscaled int of a V_DECIMAL
+    of type dtype = (precision, scale)"""
 
-    def __init__(self, value, vtype):
-        self.value, self.vtype = value, vtype
+    def __init__(self, value, vtype, dtype=None):
+        self.value, self.vtype, self.dtype = value, vtype, dtype
 
 
 def _utf8(v):
@@ -310,30 +313,69 @@ def _utf8(v):
 
 
 class Null:
-    def __init__(self, vtype):
-        self.vtype = vtype
+    def __init__(self, vtype, dtype=None):
+        self.vtype, self.dtype = vtype, dtype
+
+
+def decimal_result_type(op, a, b=None, legacy=False):
+    """the result DECIMAL(p, s) of a decimal operator under the reference's type rules (M/type/DecimalOperators.java: the default rules,
+    or deprecated.legacy-arithmetic-decimal-operators with legacy=True)"""
+    (ap, as_), (bp, bs) = a, (b if b is not None else (0, 0))
+    if op in (abi.EX_MOV, abi.EX_NEG):
+        return a
+    if op in (abi.EX_ADD, abi.EX_SUB):
+        if legacy:
+            return min(38, max(ap - as_, bp - bs) + max(as_, bs) + 1), max(as_, bs)
+        integral, raw = max(ap - as_, bp - bs), max(as_, bs)
+        p = min(raw + integral + 1, 38)
+        return p, min(raw, p - integral)
+    if op == abi.EX_MUL:
+        if legacy:
+            return min(38, ap + bp), as_ + bs
+        rp, rs = ap + bp + 1, as_ + bs
+        integral = rp - rs
+        return min(rp, 38), min(rs, 6 if integral > 32 else 38 - integral)
+    if op == abi.EX_DIV:
+        if legacy:
+            return min(38, ap + bs + max(bs - as_, 0)), max(as_, bs)
+        rs = max(6, as_ + bp + 1)
+        rp = ap - as_ + bs + rs
+        integral = rp - rs
+        return min(rp, 38), min(rs, 6 if integral > 32 else 38 - integral)
+    raise ValueError("no DECIMAL result type for op %d" % op)
 
 
 class Call:
     """op: one of abi.EX_*; args: expressions.  vtype is the OPERAND type (result of comparisons is BOOLEAN).
-    EX_IN takes in_list (str / bytes values for a VARCHAR operand); EX_LIKE takes the constant pattern and an optional one-character
-    escape (str / bytes): `value LIKE pattern [ESCAPE escape]`."""
+    EX_IN takes in_list (str / bytes values for a VARCHAR operand, unscaled ints for a DECIMAL one); EX_LIKE takes the constant pattern
+    and an optional one-character escape (str / bytes): `value LIKE pattern [ESCAPE escape]`.
+    DECIMAL: the result type of +, -, *, / follows the reference's default rules (legacy=True: the legacy ones) unless result_dtype gives
+    it; EX_CAST_TO_DECIMAL needs result_dtype."""
 
-    def __init__(self, op, *args, in_list=None, pattern=None, escape=None):
+    def __init__(self, op, *args, in_list=None, pattern=None, escape=None, result_dtype=None, legacy=False):
         self.op, self.args, self.in_list = op, list(args), in_list
         self.pattern, self.escape = pattern, escape
         a0 = args[0]
         self.operand_vtype = a0.vtype if not isinstance(a0, Call) else a0.result_vtype
+        self.operand_dtypes = [getattr(x, "dtype", None) for x in args]
+        self.dtype = None
         boolean_result = op in (abi.EX_EQ, abi.EX_NE, abi.EX_LT, abi.EX_LE, abi.EX_GT, abi.EX_GE, abi.EX_AND, abi.EX_OR, abi.EX_NOT,
                                 abi.EX_IS_NULL, abi.EX_IS_NOT_NULL, abi.EX_BETWEEN, abi.EX_IN, abi.EX_LIKE)
         if boolean_result:
             self.result_vtype = abi.V_BOOLEAN
-        elif op == abi.EX_CAST_BIGINT_TO_DOUBLE:
+        elif op in (abi.EX_CAST_BIGINT_TO_DOUBLE, abi.EX_CAST_DECIMAL_TO_DOUBLE):
             self.result_vtype = abi.V_DOUBLE
-        elif op == abi.EX_CAST_DOUBLE_TO_BIGINT:
+        elif op in (abi.EX_CAST_DOUBLE_TO_BIGINT, abi.EX_CAST_DECIMAL_TO_BIGINT):
             self.result_vtype = abi.V_BIGINT
+        elif op == abi.EX_CAST_TO_DECIMAL:
+            if result_dtype is None:
+                raise ValueError("a cast to DECIMAL needs result_dtype")
+            self.result_vtype, self.dtype = abi.V_DECIMAL, tuple(result_dtype)
         else:
             self.result_vtype = self.operand_vtype
+            if self.operand_vtype == abi.V_DECIMAL:
+                self.dtype = tuple(result_dtype) if result_dtype is not None else decimal_result_type(
+                    op, self.operand_dtypes[0], self.operand_dtypes[1] if len(args) > 1 else None, legacy)
 
     @property
     def vtype(self):
@@ -349,6 +391,8 @@ class PageProcessorProgram:
         self.in_lists = []
         self.strings = []          # VARCHAR constants (bytes), indexed by TGPU_OPND_CONST imm and VARCHAR IN-list values
         self.like_patterns = []    # (pattern bytes, escape bytes)
+        self.signatures = []       # per instruction: ((p, s) of a, b, c, result) or None
+        self.decimal_constants = []   # long DECIMAL constants (python ints), indexed by a long constant's imm and long IN-list values
         self.live = set()
         self.filter_temp = -1
         self.num_filter_insns = 0
@@ -369,7 +413,8 @@ class PageProcessorProgram:
             opnd = self._emit(p)
             if opnd[0] != abi.OPND_TEMP or opnd[1] == self.filter_temp:
                 t = self._alloc()
-                self._push(abi.EX_MOV, vt, t, opnd)
+                dt = p.dtype if vt == abi.V_DECIMAL else None
+                self._push(abi.EX_MOV, vt, t, opnd, sig=(dt, None, None, dt) if dt else None)
                 opnd = (abi.OPND_TEMP, t, 0)
             self.projections.append((1, opnd[1], vt))
         self._build()
@@ -381,8 +426,17 @@ class PageProcessorProgram:
                 return t
         raise ValueError("expression needs more than 8 temporaries")
 
-    def _push(self, op, vtype, dst, a, b=None, c=None):
+    def _push(self, op, vtype, dst, a, b=None, c=None, sig=None):
         self.insns.append((op, vtype, dst, a, b or (abi.OPND_NONE, 0, 0), c or (abi.OPND_NONE, 0, 0)))
+        self.signatures.append(sig)
+
+    def _decimal(self, value, dtype):
+        """a DECIMAL constant: a short one is its unscaled value, a long one an index into decimal_constants"""
+        if dtype[0] <= 18:
+            return int(value)
+        if value not in self.decimal_constants:
+            self.decimal_constants.append(int(value))
+        return self.decimal_constants.index(value)
 
     def _string(self, v):
         b = _utf8(v)
@@ -395,6 +449,8 @@ class PageProcessorProgram:
             return (abi.OPND_COLUMN, e.channel, 0)
         if isinstance(e, Const) and e.vtype == abi.V_VARCHAR:
             return (abi.OPND_CONST, 0, self._string(e.value))
+        if isinstance(e, Const) and e.vtype == abi.V_DECIMAL:
+            return (abi.OPND_CONST, 0, self._decimal(e.value, e.dtype))
         if isinstance(e, Const):
             imm = abi.Imm()
             if e.vtype == abi.V_DOUBLE:
@@ -409,6 +465,9 @@ class PageProcessorProgram:
         if e.op == abi.EX_LIKE:
             self.like_patterns.append((_utf8(e.pattern), b"" if e.escape is None else _utf8(e.escape)))
             b = (abi.OPND_CONST, 0, len(self.like_patterns) - 1)
+        elif e.op == abi.EX_IN and e.operand_vtype == abi.V_DECIMAL:
+            self.in_lists.append([self._decimal(v, e.operand_dtypes[0]) for v in e.in_list])
+            b = (abi.OPND_CONST, 0, len(self.in_lists) - 1)
         elif e.op == abi.EX_IN and e.operand_vtype == abi.V_VARCHAR:
             self.in_lists.append([self._string(v) for v in e.in_list])
             b = (abi.OPND_CONST, 0, len(self.in_lists) - 1)
@@ -427,7 +486,13 @@ class PageProcessorProgram:
             if o[0] == abi.OPND_TEMP and o[1] != self.filter_temp:
                 self.live.discard(o[1])
         dst = self._alloc()
-        self._push(e.op, e.operand_vtype, dst, ops[0], b if b else (ops[1] if len(ops) > 1 else None), ops[2] if len(ops) > 2 else None)
+        sig = None
+        if e.operand_vtype == abi.V_DECIMAL or e.dtype is not None:
+            dts = (e.operand_dtypes + [None, None, None])[:3] if e.operand_vtype == abi.V_DECIMAL else [None, None, None]
+            if e.op == abi.EX_IN:
+                dts = [dts[0], None, None]
+            sig = (dts[0], dts[1], dts[2], e.dtype)
+        self._push(e.op, e.operand_vtype, dst, ops[0], b if b else (ops[1] if len(ops) > 1 else None), ops[2] if len(ops) > 2 else None, sig=sig)
         return (abi.OPND_TEMP, dst, 0)
 
     def _build(self):
@@ -466,6 +531,20 @@ class PageProcessorProgram:
                                       len(self.in_lists), C.cast(self._lists, C.POINTER(abi.InList)),
                                       len(self.strings), C.cast(self._strs, C.POINTER(abi.Bytes)),
                                       len(self.like_patterns), C.cast(self._likes, C.POINTER(abi.LikePattern)))
+        if any(sig is not None for sig in self.signatures):
+            self._sigs = (abi.DecimalSignature * max(1, n))()
+            for i, sig in enumerate(self.signatures):
+                for fld, dt in zip(("a", "b", "c", "result"), sig or ()):
+                    if dt is not None:
+                        getattr(self._sigs[i], fld).precision, getattr(self._sigs[i], fld).scale = dt
+            words = []
+            for v in self.decimal_constants:
+                u = v & ((1 << 128) - 1)
+                words += [u >> 64, u & ((1 << 64) - 1)]
+            self._dec_consts = (C.c_int64 * max(1, len(words)))(*[w - (1 << 64) if w >= (1 << 63) else w for w in words])
+            self.struct.decimal_signatures = C.cast(self._sigs, C.POINTER(abi.DecimalSignature))
+            self.struct.num_decimal_constants = len(self.decimal_constants)
+            self.struct.decimal_constants = C.cast(self._dec_consts, C.POINTER(C.c_int64))
 
 
 class FilterAndProjectOperatorFactory(OperatorFactory):
