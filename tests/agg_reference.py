@@ -7,6 +7,8 @@ channel) triple (channel -1: none).
 Group ids follow first appearance over the whole stream (GroupByHash.java:118-125).  A NULL key is an ordinary group.  DOUBLE keys
 group by IDENTICAL (DoubleType.java:218-229: NaN = NaN, -0.0 = +0.0) and the output key is the first raw value seen for the group, bit
 for bit (NaN payload and zero sign included).  A multi-column key is equal only when every field is, NULL included.
+VARCHAR keys are bytes, INT128 (long DECIMAL) keys Python ints, REAL keys their float value (no rule is stated here for a REAL NaN or
+-0.0 key).
 
 A row counts for an aggregate only if its mask is non-NULL and non-zero; NULL inputs are skipped (count(*) counts the row).
 
@@ -57,7 +59,9 @@ def _column(page, channel):
     nulls = blk.nulls if blk.nulls is not None else np.zeros(n, dtype=bool)
     if blk.type == abi.FLOAT64:
         vals = [_float_of_bits(b) for b in blk.values.view(np.int64).tolist()]
-    elif blk.type == abi.UTF8:
+    elif blk.type == abi.FLOAT32:
+        vals = [float(x) for x in blk.values.tolist()]
+    elif blk.type in (abi.UTF8, abi.INT128):
         vals = [blk.get(i) if not nulls[i] else None for i in range(n)]
     else:
         vals = blk.values.astype(np.int64).tolist()

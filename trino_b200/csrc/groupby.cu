@@ -3311,6 +3311,16 @@ struct AggOp : tgpu_op {
         fused_general = false;
         f_recs.release();
         f_cap = f_used = f_specials = rows_seen = 0;
+        // the string dictionaries go with the builder (FlatHash's variable-width data): the flushed output is decoded already, so no id
+        // of theirs is alive.  Kept, they would count against max_partial_bytes forever and flush every later page.  Keys that read the
+        // same channel share one dictionary, and share the fresh one.
+        std::map<StringDict*, std::shared_ptr<StringDict>> fresh;
+        for (auto& d : key_dicts) {
+            if (!d) continue;
+            auto& f = fresh[d.get()];
+            if (!f) f = std::make_shared<StringDict>(ctx);
+            d = f;
+        }
         TG_TRY(init_state());
         // once the pre-stage was un-fused (inner_fp exists, the plan's sources point at projection OUTPUT channels) the
         // shared-memory path must never see a raw input page again: stay on the general path across flushes
