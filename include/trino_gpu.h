@@ -46,7 +46,8 @@ typedef enum tgpu_status {
     TGPU_ERR_DIVISION_BY_ZERO = -5,       /* DIVISION_BY_ZERO (M/type/BigintOperators.java:96-106) */
     TGPU_ERR_NOT_SUPPORTED = -6,          /* NOT_SUPPORTED: caller keeps the Java operator */
     TGPU_ERR_ILLEGAL_STATE = -7,          /* IllegalStateException / checkState (protocol misuse) */
-    TGPU_ERR_INVALID_CAST_ARGUMENT = -8   /* INVALID_CAST_ARGUMENT (M/type/DoubleOperators.java:159-167: CAST(DOUBLE AS BIGINT) of NaN, +-Infinity, |x| >= 2^63) */
+    TGPU_ERR_INVALID_CAST_ARGUMENT = -8,  /* INVALID_CAST_ARGUMENT (M/type/DoubleOperators.java:159-167: CAST(DOUBLE AS BIGINT) of NaN, +-Infinity, |x| >= 2^63) */
+    TGPU_ERR_INVALID_FUNCTION_ARGUMENT = -9 /* INVALID_FUNCTION_ARGUMENT (M/operator/scalar/ConcatFunction.java:82-88: "Concatenated string is too large") */
 } tgpu_status;
 
 /* ------------------------------------------------------------------ columnar data model
@@ -155,13 +156,28 @@ typedef enum tgpu_expr_op {
     TGPU_EX_CAST_DECIMAL_TO_DOUBLE = 34, /* vtype DECIMAL: the reference's rounding (M/type/DecimalCasts.java:439-448)         */
     TGPU_EX_IN = 40,               /* a IN (const list): b.imm = index into in_lists, all operands of `vtype`.  Under
                                       TGPU_V_VARCHAR the list's values are indices into `strings`                      */
-    TGPU_EX_LIKE = 41              /* a LIKE like_patterns[b.imm] (LikeFunctions.likeVarchar, M/type/LikeFunctions.java:49-56, over
+    TGPU_EX_LIKE = 41,             /* a LIKE like_patterns[b.imm] (LikeFunctions.likeVarchar, M/type/LikeFunctions.java:49-56, over
                                       LikeMatcher.compile(pattern, escape) with optimize = true): BOOLEAN, vtype TGPU_V_VARCHAR */
+    /* string functions (vtype TGPU_V_VARCHAR, the type of operand a; FilterAndProject only; M/operator/scalar/StringFunctions.java) */
+    TGPU_EX_LENGTH = 50,           /* length(a): BIGINT, code points (:95-102)                                                    */
+    TGPU_EX_SUBSTR = 51,           /* substr(a, b) / substr(a, b, c): b, c BIGINT, c TGPU_OPND_NONE for the two-argument form
+                                      (:284-320, :331-378): VARCHAR                                                                */
+    TGPU_EX_LTRIM = 52, TGPU_EX_RTRIM = 53, TGPU_EX_TRIM = 54, /* one-argument whitespace trims (:484-527): VARCHAR               */
+    TGPU_EX_CONCAT = 55            /* a || b (ConcatFunction.java:78-95): VARCHAR.  Lower concat(x1, ..., xn) to a left-deep chain of
+                                      binary CONCATs: the same value and the same error                                            */
 } tgpu_expr_op;
 
-/* TGPU_V_VARCHAR is an OPERAND type only: =, <>, <, <=, >, >=, BETWEEN, IN, IS [NOT] NULL and LIKE read it and give BOOLEAN; no
- * instruction produces a string.  A VARCHAR operand is a TGPU_OPND_COLUMN naming a TGPU_UTF8 channel (the bytes between offsets[i]
- * and offsets[i+1]), a TGPU_OPND_CONST whose imm indexes `strings`, or TGPU_OPND_NULL; a VARCHAR TGPU_OPND_TEMP is INVALID_ARGUMENT.
+/* TGPU_V_VARCHAR: =, <>, <, <=, >, >=, BETWEEN, IN, IS [NOT] NULL and LIKE read it and give BOOLEAN; LENGTH gives BIGINT; SUBSTR, the
+ * trims and CONCAT give VARCHAR.  A VARCHAR operand is a TGPU_OPND_COLUMN naming a TGPU_UTF8 channel (the bytes between offsets[i]
+ * and offsets[i+1]), a TGPU_OPND_CONST whose imm indexes `strings`, TGPU_OPND_NULL, or a TGPU_OPND_TEMP that an earlier instruction
+ * wrote a VARCHAR to (otherwise INVALID_ARGUMENT).  The result of SUBSTR or a trim is a view of the bytes of one channel or constant;
+ * every VARCHAR reader takes it.  A CONCAT result (at most 8 pieces in all, else NOT_SUPPORTED) may be read only by another CONCAT
+ * or by a computed projection; any other reader answers NOT_SUPPORTED at create.  A computed projection with vtype TGPU_V_VARCHAR
+ * gives a TGPU_UTF8 column.
+ * Code points are counted as airlift's SliceUtf8 counts them (bytes that are not 10xxxxxx); on bytes that are not UTF-8 the functions
+ * claim no parity but never read outside the row's bytes.  The trims remove the code points Character.isWhitespace accepts.  A NULL
+ * argument gives NULL.  CONCAT raises INVALID_FUNCTION_ARGUMENT "Concatenated string is too large" when its total passes 1 MiB
+ * (DEFAULT_MAX_PAGE_SIZE_IN_BYTES, S/block/PageBuilderStatus.java:22), never when a piece is NULL.
  * Equality is bytewise; order is Slice.compareTo (unsigned bytes, a proper prefix first: S/type/AbstractVariableWidthType.java:403-410).
  * CHAR(n) (padded comparison and LIKE) is not covered: keep Java for it. */
 /* TGPU_V_DECIMAL: DECIMAL(p, s) as its unscaled value; precision <= 18 is a short decimal (one BIGINT word: a TGPU_INT64 channel or a
@@ -217,7 +233,8 @@ typedef struct tgpu_projection {
                             1 = computed: value of temp `index` after the program ran */
     int32_t index;       /* channel or temp */
     int32_t vtype;       /* computed only: result type (BIGINT->INT64, DOUBLE->FLOAT64, BOOLEAN->INT8, DECIMAL->INT64 for a short and
-                            INT128 for a long result of the instruction that defines the temp) */
+                            INT128 for a long result of the instruction that defines the temp, VARCHAR->UTF8; at most 8 VARCHAR
+                            projections, and a column of more than INT32_MAX bytes fails with TGPU_ERR_INSUFFICIENT_RESOURCES) */
 } tgpu_projection;
 
 typedef struct tgpu_decimal_type { int8_t precision, scale; } tgpu_decimal_type;     /* 1 <= precision <= 38, 0 <= scale <= precision */

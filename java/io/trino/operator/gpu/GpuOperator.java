@@ -30,6 +30,7 @@ import static io.trino.spi.StandardErrorCode.DIVISION_BY_ZERO;
 import static io.trino.spi.StandardErrorCode.GENERIC_INSUFFICIENT_RESOURCES;
 import static io.trino.spi.StandardErrorCode.GENERIC_INTERNAL_ERROR;
 import static io.trino.spi.StandardErrorCode.INVALID_CAST_ARGUMENT;
+import static io.trino.spi.StandardErrorCode.INVALID_FUNCTION_ARGUMENT;
 import static io.trino.spi.StandardErrorCode.NOT_SUPPORTED;
 import static io.trino.spi.StandardErrorCode.NUMERIC_VALUE_OUT_OF_RANGE;
 import static java.lang.foreign.ValueLayout.ADDRESS;
@@ -255,6 +256,7 @@ public class GpuOperator
             case -4 -> new TrinoException(NUMERIC_VALUE_OUT_OF_RANGE, message);
             case -5 -> new TrinoException(DIVISION_BY_ZERO, message);
             case -8 -> new TrinoException(INVALID_CAST_ARGUMENT, message);
+            case -9 -> new TrinoException(INVALID_FUNCTION_ARGUMENT, message);   // "Concatenated string is too large"
             case -6 -> new TrinoException(NOT_SUPPORTED, message);   // shapes the planner-side check (GpuSupport) should have kept on the Java operator
             case -1 -> new IllegalArgumentException(message);
             case -7 -> new IllegalStateException(message);

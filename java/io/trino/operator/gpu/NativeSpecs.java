@@ -73,6 +73,34 @@ public final class NativeSpecs
     static final StructLayout DECIMAL_TYPE = MemoryLayout.structLayout(JAVA_BYTE.withName("precision"), JAVA_BYTE.withName("scale"));
     static final StructLayout DECIMAL_SIGNATURE = MemoryLayout.structLayout(DECIMAL_TYPE.withName("a"), DECIMAL_TYPE.withName("b"),
             DECIMAL_TYPE.withName("c"), DECIMAL_TYPE.withName("result"));
+    // String functions (operand type TGPU_V_VARCHAR = 3): the resolved function of a call maps to one opcode.  length(varchar) -> EX_LENGTH;
+    // substr / substring(varchar, bigint[, bigint]) -> EX_SUBSTR (the two-argument form leaves operand c TGPU_OPND_NONE); ltrim / rtrim /
+    // trim(varchar) with one argument -> EX_LTRIM / EX_RTRIM / EX_TRIM; concat(varchar, ...) and `||` -> a left-deep chain of binary
+    // EX_CONCATs, at most 8 pieces.  A computed projection of vtype 3 yields a UTF8 column.  CHAR(n) arguments and the trims with a
+    // character list keep the Java operator.
+    public static final int V_VARCHAR = 3;
+    public static final int EX_LENGTH = 50;
+    public static final int EX_SUBSTR = 51;
+    public static final int EX_LTRIM = 52;
+    public static final int EX_RTRIM = 53;
+    public static final int EX_TRIM = 54;
+    public static final int EX_CONCAT = 55;
+    public static final int MAX_CONCAT_PIECES = 8;
+
+    /** the opcode of a one-call string function (by its resolved name and argument count), or -1 when it keeps the Java operator */
+    public static int stringFunctionOpcode(String name, int arity)
+    {
+        return switch (name) {
+            case "length" -> arity == 1 ? EX_LENGTH : -1;
+            case "substr", "substring" -> arity == 2 || arity == 3 ? EX_SUBSTR : -1;
+            case "ltrim" -> arity == 1 ? EX_LTRIM : -1;
+            case "rtrim" -> arity == 1 ? EX_RTRIM : -1;
+            case "trim" -> arity == 1 ? EX_TRIM : -1;
+            case "concat", "$operator$concat" -> arity >= 2 && arity <= MAX_CONCAT_PIECES ? EX_CONCAT : -1;
+            default -> -1;
+        };
+    }
+
     public static final int PARTITION_HASH_BUCKET = 0;    // HashBucketFunction (M/sql/planner/HashBucketFunction.java:43-46)
     public static final int PARTITION_LOCAL = 1;          // LocalPartitionGenerator (M/operator/exchange/LocalPartitionGenerator.java:45-77)
 

@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtrino_gpu.so")
 TGPU_OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_INSUFFICIENT_RESOURCES, ERR_NUMERIC_VALUE_OUT_OF_RANGE = -1, -2, -3, -4
 ERR_DIVISION_BY_ZERO, ERR_NOT_SUPPORTED, ERR_ILLEGAL_STATE, ERR_INVALID_CAST_ARGUMENT = -5, -6, -7, -8
+ERR_INVALID_FUNCTION_ARGUMENT = -9
 
 INT64, INT32, INT16, INT8, FLOAT64, UTF8, DICT32, RLE, INT128, FLOAT32 = 1, 2, 3, 4, 5, 7, 8, 9, 10, 11
 COL_NULLS_BYTEMAP = 1
@@ -26,6 +27,9 @@ EX_AND, EX_OR, EX_NOT, EX_IS_NULL, EX_IS_NOT_NULL, EX_BETWEEN = 20, 21, 22, 23, 
 EX_CAST_BIGINT_TO_DOUBLE, EX_CAST_DOUBLE_TO_BIGINT, EX_IN, EX_LIKE = 30, 31, 40, 41
 # DECIMAL casts: EX_CAST_TO_DECIMAL reads BIGINT or DECIMAL (its vtype), the other two read DECIMAL
 EX_CAST_TO_DECIMAL, EX_CAST_DECIMAL_TO_BIGINT, EX_CAST_DECIMAL_TO_DOUBLE = 32, 33, 34
+# string functions over a VARCHAR operand a: LENGTH gives BIGINT, the others VARCHAR; SUBSTR reads BIGINT b (and c, or OPND_NONE)
+EX_LENGTH, EX_SUBSTR, EX_LTRIM, EX_RTRIM, EX_TRIM, EX_CONCAT = 50, 51, 52, 53, 54, 55
+MAX_CONCAT_PIECES, MAX_VARCHAR_PROJECTIONS = 8, 8
 V_BIGINT, V_DOUBLE, V_BOOLEAN, V_VARCHAR, V_DECIMAL = 0, 1, 2, 3, 4
 MAX_STRINGS, MAX_STRING_BYTES, MAX_LIKE_PATTERNS = 128, 4096, 8
 OPND_NONE, OPND_COLUMN, OPND_TEMP, OPND_CONST, OPND_NULL = 0, 1, 2, 3, 4

@@ -41,6 +41,7 @@ extern "C" const char* tgpu_status_name(int status)
         case TGPU_ERR_NOT_SUPPORTED: return "NOT_SUPPORTED";
         case TGPU_ERR_ILLEGAL_STATE: return "ILLEGAL_STATE";
         case TGPU_ERR_INVALID_CAST_ARGUMENT: return "INVALID_CAST_ARGUMENT";
+        case TGPU_ERR_INVALID_FUNCTION_ARGUMENT: return "INVALID_FUNCTION_ARGUMENT";
         default: return "UNKNOWN";
     }
 }

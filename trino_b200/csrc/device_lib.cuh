@@ -40,11 +40,16 @@ enum {
     TGD_EX_EQ = 10, TGD_EX_NE = 11, TGD_EX_LT = 12, TGD_EX_LE = 13, TGD_EX_GT = 14, TGD_EX_GE = 15,
     TGD_EX_AND = 20, TGD_EX_OR = 21, TGD_EX_NOT = 22, TGD_EX_IS_NULL = 23, TGD_EX_IS_NOT_NULL = 24, TGD_EX_BETWEEN = 25,
     TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_CAST_TO_DECIMAL = 32, TGD_EX_CAST_DECIMAL_TO_BIGINT = 33,
-    TGD_EX_CAST_DECIMAL_TO_DOUBLE = 34, TGD_EX_IN = 40, TGD_EX_LIKE = 41
+    TGD_EX_CAST_DECIMAL_TO_DOUBLE = 34, TGD_EX_IN = 40, TGD_EX_LIKE = 41,
+    TGD_EX_LENGTH = 50, TGD_EX_SUBSTR = 51, TGD_EX_LTRIM = 52, TGD_EX_RTRIM = 53, TGD_EX_TRIM = 54, TGD_EX_CONCAT = 55
 };
 // TGD_V_DECIMAL_LONG is internal: the output-column type of a long DECIMAL projection (16-byte cells: high word, low word)
 enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2, TGD_V_VARCHAR = 3, TGD_V_DECIMAL = 4, TGD_V_DECIMAL_LONG = 5 };
-enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4, TG_ERR_BIT_DECIMAL_OVERFLOW = 8 };
+// TG_ERR_BIT_CONCAT_TOO_LARGE: a concatenation past 1 MiB (INVALID_FUNCTION_ARGUMENT).  The interpreter keeps 4 bits of error per temp and
+// holds it there as TG_ERR_CODE_CONCAT (15, never a single bit); vm_temp_error turns it back into the bit.
+enum { TG_ERR_BIT_OVERFLOW = 1, TG_ERR_BIT_DIV_ZERO = 2, TG_ERR_BIT_INVALID_CAST = 4, TG_ERR_BIT_DECIMAL_OVERFLOW = 8, TG_ERR_BIT_CONCAT_TOO_LARGE = 16 };
+#define TG_ERR_CODE_CONCAT 15u
+#define TGD_MAX_CONCAT_BYTES (1 << 20)    // DEFAULT_MAX_PAGE_SIZE_IN_BYTES (S/block/PageBuilderStatus.java:22)
 
 // The reference's method for one DECIMAL instruction, fixed at create from its signature (expr.cu decimal_method).  la / lb / lc / lr:
 // operand a / b / c and the result are long decimals (a BIGINT operand or a non-DECIMAL result: 0).  k0..k2, m0, m1: see vm_apply_dec.
@@ -74,6 +79,11 @@ struct SmallOut {
     unsigned int* err;
 };
 
+#define TGD_MAX_STR_OUTS 8
+#define TGD_MAX_PIECES 8          // pieces of one concatenation
+#define TGD_MAX_PIECE_SLOTS 16    // captured pieces of one program
+#define TGD_SRC_NONE (-2147483647 - 1)
+
 // computed projection outputs of the filter/project kernels
 struct OutCols {
     int32_t count;
@@ -85,6 +95,11 @@ struct OutCols {
     int32_t pass_count;
     void* pass_data[TGD_MAX_CHANNELS];
     uint8_t* pass_nullmap[TGD_MAX_CHANNELS];
+    // VARCHAR projections (DProgram::str_out[k]): per output row and piece an (int32 begin, int32 len) descriptor into the piece's
+    // source, [row][piece]; the byte assembly kernel turns them into a UTF8 column
+    int32_t str_count;
+    void* str_desc[TGD_MAX_STR_OUTS];
+    uint8_t* str_nullmap[TGD_MAX_STR_OUTS];
 };
 
 // ---- VARCHAR operands of FilterAndProject programs ------------------------------------------------------------------------
@@ -185,6 +200,135 @@ __device__ __forceinline__ bool tg_str_cmp_op(int op, StrRef a, StrRef b)
         case TGD_EX_GT: return c > 0;
         default: return c >= 0;
     }
+}
+
+// ---- string functions (M/operator/scalar/StringFunctions.java over airlift's SliceUtf8) -----------------------------------------------
+// Code points are counted as SliceUtf8.countCodePoints counts them: every byte that is not a continuation byte (10xxxxxx).  On bytes that
+// are not UTF-8 the results are deterministic and stay inside the string, with no parity claimed.
+__device__ __forceinline__ bool tg_utf8_cont(uint8_t b) { return (b & 0xC0) == 0x80; }
+
+__device__ __forceinline__ long long tg_utf8_count(StrRef s)
+{
+    long long n = 0;
+    int i = 0;
+    for (; i + 8 <= s.len; i += 8) {
+        const unsigned long long w = tg_ld_bytes(s.p + i, 8);
+        // a continuation byte has bit 7 set and bit 6 clear
+        n += 8 - __popcll(w & ~(w << 1) & 0x8080808080808080ULL);
+    }
+    for (; i < s.len; i++) n += tg_utf8_cont(s.p[i]) ? 0 : 1;
+    return n;
+}
+
+// SliceUtf8.offsetOfCodePoint(s, position, count): the byte offset of the count-th code point after `position`, or -1 when the string ends
+// first.  A code point starts at a byte that is not a continuation byte.
+__device__ __forceinline__ int tg_utf8_offset(StrRef s, int position, int count)
+{
+    if ((long long)s.len - position <= count) return -1;
+    int i = position;
+    for (int k = 0; k < count; k++) {
+        i++;
+        while (i < s.len && tg_utf8_cont(s.p[i])) i++;
+        if (i >= s.len) return -1;
+    }
+    return i;
+}
+
+__device__ __forceinline__ int tg_sat_int(long long v) { return v > 2147483647LL ? 2147483647 : v < -2147483648LL ? (-2147483647 - 1) : (int)v; }
+
+// StringFunctions.substring(utf8, start) (has_len = false, :284-320) and substring(utf8, start, length) (:331-378).  Where Java's
+// startCodePoint + lengthCodePoints wraps (a negative start with a length near INT_MAX) the reference fails inside Slice.slice; this
+// returns the suffix, as the unwrapped sum would.
+__device__ __forceinline__ StrRef tg_substr(StrRef s, long long start, bool has_len, long long length)
+{
+    const StrRef empty{s.p, 0};
+    if (start == 0 || (has_len && length <= 0) || s.len == 0) return empty;
+    int sc = tg_sat_int(start);
+    const int lc = has_len ? tg_sat_int(length) : 0;
+    int b, e = s.len;
+    if (sc > 0) {
+        b = tg_utf8_offset(s, 0, sc - 1);
+        if (b < 0) return empty;
+        if (has_len) {
+            e = tg_utf8_offset(s, b, lc);
+            if (e < 0) e = s.len;
+        }
+    }
+    else {
+        const long long cps = tg_utf8_count(s);
+        const long long st = (long long)sc + cps;
+        if (st < 0) return empty;
+        b = tg_utf8_offset(s, 0, (int)st);
+        if (b < 0) return empty;
+        if (has_len && st + lc < cps) {
+            e = tg_utf8_offset(s, b, lc);
+            if (e < 0) e = s.len;
+        }
+    }
+    return StrRef{s.p + b, e - b};
+}
+
+// Character.isWhitespace: the space separators but U+00A0, U+2007 and U+202F, the line and paragraph separators, U+0009-U+000D and
+// U+001C-U+001F
+__device__ __forceinline__ bool tg_is_whitespace(unsigned int c)
+{
+    if (c <= 0x20) return c == 0x20 || (c >= 0x09 && c <= 0x0D) || (c >= 0x1C && c <= 0x1F);
+    if (c < 0x1680) return false;
+    return c == 0x1680 || (c >= 0x2000 && c <= 0x200A && c != 0x2007) || c == 0x2028 || c == 0x2029 || c == 0x205F || c == 0x3000;
+}
+
+// the code point of the well-formed sequence of n bytes at p (n = 1..4), or -1 when it is not one
+__device__ __forceinline__ int tg_utf8_decode(const uint8_t* p, int n)
+{
+    const unsigned int h = p[0];
+    if (n == 1) return h < 0x80 ? (int)h : -1;
+    const unsigned int want = n == 2 ? 0xC0u : n == 3 ? 0xE0u : 0xF0u, mask = n == 2 ? 0xE0u : n == 3 ? 0xF0u : 0xF8u;
+    if ((h & mask) != want) return -1;
+    unsigned int c = h & (0x7Fu >> n);
+    for (int k = 1; k < n; k++) {
+        if (!tg_utf8_cont(p[k])) return -1;
+        c = (c << 6) | (p[k] & 0x3Fu);
+    }
+    return (int)c;
+}
+
+__device__ __forceinline__ int tg_utf8_lead_len(uint8_t h) { return h < 0x80 ? 1 : (h & 0xE0) == 0xC0 ? 2 : (h & 0xF0) == 0xE0 ? 3 : (h & 0xF8) == 0xF0 ? 4 : 0; }
+
+// SliceUtf8.leftTrim / rightTrim / trim: whitespace code points off either end; a sequence that is not UTF-8 stops the trim
+__device__ __forceinline__ StrRef tg_trim(StrRef s, bool left, bool right)
+{
+    int b = 0, e = s.len;
+    if (left) {
+        while (b < e) {
+            const int n = tg_utf8_lead_len(s.p[b]);
+            if (n == 0 || b + n > e) break;
+            const int c = tg_utf8_decode(s.p + b, n);
+            if (c < 0 || !tg_is_whitespace((unsigned int)c)) break;
+            b += n;
+        }
+    }
+    if (right) {
+        while (e > b) {
+            int q = e - 1;
+            while (q > b && q > e - 4 && tg_utf8_cont(s.p[q])) q--;
+            const int n = e - q;
+            if (tg_utf8_lead_len(s.p[q]) != n) break;
+            const int c = tg_utf8_decode(s.p + q, n);
+            if (c < 0 || !tg_is_whitespace((unsigned int)c)) break;
+            e = q;
+        }
+    }
+    return StrRef{s.p + b, e - b};
+}
+
+// The error of a call over operands a, b, c (BytecodeUtils.java:303-306): the operands' errors in order, stopping at the first NULL one,
+// then its own
+__device__ __forceinline__ uint32_t vm_error_call(bool an, uint32_t ea, bool bn, uint32_t eb, uint32_t ec, bool any_null, uint32_t own)
+{
+    if (ea || an) return ea;
+    if (eb || bn) return eb;
+    if (ec) return ec;
+    return any_null ? 0u : own;
 }
 
 __device__ __forceinline__ bool tg_bytes_eq(const uint8_t* p, const uint8_t* q, int n)

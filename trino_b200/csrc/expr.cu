@@ -180,23 +180,51 @@ static bool varchar_op(int op)
     switch (op) {
         case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE: case TGPU_EX_BETWEEN:
         case TGPU_EX_IN: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: case TGPU_EX_LIKE:
+        case TGPU_EX_LENGTH: case TGPU_EX_SUBSTR: case TGPU_EX_LTRIM: case TGPU_EX_RTRIM: case TGPU_EX_TRIM: case TGPU_EX_CONCAT:
             return true;
         default: return false;
     }
 }
 
-// one instruction over VARCHAR operands: operands are UTF8 channels (given a string slot), pool constants or NULL
-static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i, DProgram* out, int32_t* max_channel)
+static bool string_function(int op) { return op >= TGPU_EX_LENGTH && op <= TGPU_EX_CONCAT; }
+
+// the vtype of what instruction `s` writes to its temp
+static int result_vtype(const tgpu_expr_insn& s)
+{
+    switch (s.op) {
+        case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE: case TGPU_EX_AND: case TGPU_EX_OR:
+        case TGPU_EX_NOT: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: case TGPU_EX_BETWEEN: case TGPU_EX_IN: case TGPU_EX_LIKE:
+            return TGPU_V_BOOLEAN;
+        case TGPU_EX_CAST_BIGINT_TO_DOUBLE: case TGPU_EX_CAST_DECIMAL_TO_DOUBLE: return TGPU_V_DOUBLE;
+        case TGPU_EX_CAST_DOUBLE_TO_BIGINT: case TGPU_EX_CAST_DECIMAL_TO_BIGINT: case TGPU_EX_LENGTH: return TGPU_V_BIGINT;
+        case TGPU_EX_CAST_TO_DECIMAL: return TGPU_V_DECIMAL;
+        default: return s.vtype;
+    }
+}
+
+// What each temp holds while the instructions are compiled in order
+struct TempState {
+    int vt[TGPU_MAX_TEMPS];         // vtype of the value, -1 never written
+    int kind[TGPU_MAX_TEMPS];       // VARCHAR temps: 1 a view, 2 a CONCAT result
+    int32_t src[TGPU_MAX_TEMPS];    // a view's source
+    int cat[TGPU_MAX_TEMPS];        // a CONCAT result's instruction
+    TempState() { for (int t = 0; t < TGPU_MAX_TEMPS; t++) { vt[t] = -1; kind[t] = 0; src[t] = TGD_SRC_NONE; cat[t] = -1; } }
+};
+
+// one instruction with VARCHAR operands: operands are UTF8 channels (given a string slot), pool constants, NULL, or temps holding a
+// VARCHAR (a view, or a CONCAT result that only CONCAT reads).  SUBSTR's start and length are BIGINT operands.
+static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i, DProgram* out, int32_t* max_channel, TempState* ts)
 {
     const tgpu_expr_insn& s = p->insns[i];
     DInsn& d = out->insns[i];
     if (s.vtype != TGPU_V_VARCHAR) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: LIKE needs VARCHAR operands", i);
     if (!varchar_op(s.op)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: op %d does not take VARCHAR operands", i, s.op);
     if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
-    const bool unary = s.op == TGPU_EX_IS_NULL || s.op == TGPU_EX_IS_NOT_NULL || s.op == TGPU_EX_IN || s.op == TGPU_EX_LIKE;
+    const bool unary = s.op == TGPU_EX_IS_NULL || s.op == TGPU_EX_IS_NOT_NULL || s.op == TGPU_EX_IN || s.op == TGPU_EX_LIKE || s.op == TGPU_EX_LENGTH ||
+                       s.op == TGPU_EX_LTRIM || s.op == TGPU_EX_RTRIM || s.op == TGPU_EX_TRIM;
     const tgpu_operand* ops[3] = {&s.a, &s.b, &s.c};
     DOperand* dops[3] = {&d.a, &d.b, &d.c};
-    const int used = unary ? 1 : s.op == TGPU_EX_BETWEEN ? 3 : 2;
+    const int used = unary ? 1 : (s.op == TGPU_EX_BETWEEN || (s.op == TGPU_EX_SUBSTR && s.c.kind != TGPU_OPND_NONE)) ? 3 : 2;
     for (int k = 0; k < 3; k++) {
         const tgpu_operand& o = *ops[k];
         DOperand& x = *dops[k];
@@ -204,8 +232,27 @@ static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i
         x.index = o.index;
         x.imm = o.imm.i64;
         if (k >= used) continue;
-        if (o.kind == TGPU_OPND_TEMP) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a VARCHAR operand cannot be a temp", i);
-        if (o.kind == TGPU_OPND_CONST) {
+        if (s.op == TGPU_EX_SUBSTR && k > 0) {
+            // the BIGINT start and length
+            if (o.kind == TGPU_OPND_TEMP) {
+                if (o.index < 0 || o.index >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "operand temp %d out of range", o.index);
+                if (ts->vt[o.index] != TGPU_V_BIGINT) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: substr's start and length are BIGINT", i);
+            }
+            else if (o.kind == TGPU_OPND_COLUMN) {
+                if (o.index < 0 || o.index >= TGPU_MAX_CHANNELS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "operand channel %d out of range", o.index);
+                if (o.index > *max_channel) *max_channel = o.index;
+            }
+            else if (o.kind != TGPU_OPND_CONST && o.kind != TGPU_OPND_NULL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad BIGINT operand kind %d", i, o.kind);
+            continue;
+        }
+        if (o.kind == TGPU_OPND_TEMP) {
+            if (o.index < 0 || o.index >= TGPU_MAX_TEMPS || ts->vt[o.index] != TGPU_V_VARCHAR)
+                return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a VARCHAR temp operand must be written by an earlier VARCHAR instruction", i);
+            if (ts->kind[o.index] == 2 && s.op != TGPU_EX_CONCAT)
+                return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: a concatenation is read only by another concatenation or a projection", i);
+            x.imm = ts->src[o.index];
+        }
+        else if (o.kind == TGPU_OPND_CONST) {
             if (o.imm.i64 < 0 || o.imm.i64 >= p->num_strings) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: pool string index out of range", i);
         }
         else if (o.kind == TGPU_OPND_COLUMN) {
@@ -232,6 +279,52 @@ static int compile_varchar_insn(tgpu_ctx* ctx, const tgpu_expr_program* p, int i
     d.op = s.op;
     d.vtype = s.vtype;
     d.dst = s.dst;
+    if (string_function(s.op)) out->has_strfn = 1;
+    // the source of a VARCHAR operand's bytes
+    auto src_of = [&](const DOperand& o) -> int32_t {
+        if (o.kind == TGPU_OPND_COLUMN) return o.index;
+        if (o.kind == TGPU_OPND_CONST) return (int32_t)(-(o.imm + 1));
+        if (o.kind == TGPU_OPND_TEMP) return (int32_t)o.imm;
+        return TGD_SRC_NONE;
+    };
+    int kind = 0, cat = -1;
+    int32_t src = TGD_SRC_NONE;
+    if (s.op == TGPU_EX_SUBSTR || s.op == TGPU_EX_LTRIM || s.op == TGPU_EX_RTRIM || s.op == TGPU_EX_TRIM) {
+        kind = 1;
+        src = src_of(d.a);
+    }
+    else if (s.op == TGPU_EX_CONCAT) {
+        DCat& c = out->cat[i];
+        memset(&c, 0, sizeof(c));
+        c.a_slot = c.b_slot = -1;
+        const DOperand* cops[2] = {&d.a, &d.b};
+        int8_t* capture[2] = {&c.a_slot, &c.b_slot};
+        for (int k = 0; k < 2; k++) {
+            const DOperand& o = *cops[k];
+            if (o.kind == TGPU_OPND_TEMP && ts->kind[o.index] == 2) {
+                DCat& inner = out->cat[ts->cat[o.index]];
+                inner.inner = 1;
+                for (int q = 0; q < inner.n; q++) {
+                    if (c.n >= TGD_MAX_PIECES) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: a concatenation of more than %d pieces", i, TGD_MAX_PIECES);
+                    c.slot[c.n] = inner.slot[q];
+                    c.src[c.n++] = inner.src[q];
+                }
+                continue;
+            }
+            if (c.n >= TGD_MAX_PIECES) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: a concatenation of more than %d pieces", i, TGD_MAX_PIECES);
+            if (out->num_piece_slots >= TGD_MAX_PIECE_SLOTS)
+                return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "concatenations capture more than %d pieces", TGD_MAX_PIECE_SLOTS);
+            *capture[k] = (int8_t)out->num_piece_slots;
+            c.slot[c.n] = (int8_t)out->num_piece_slots++;
+            c.src[c.n++] = src_of(o);
+        }
+        kind = 2;
+        cat = i;
+    }
+    ts->vt[s.dst] = result_vtype(s);
+    ts->kind[s.dst] = kind;
+    ts->src[s.dst] = src;
+    ts->cat[s.dst] = cat;
     return TGPU_OK;
 }
 
@@ -502,15 +595,22 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         else if (o.kind < 0 || o.kind > TGPU_OPND_NULL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "bad operand kind %d", o.kind);
         return TGPU_OK;
     };
+    TempState ts;
     for (int i = 0; i < p->num_insns; i++) {
         const tgpu_expr_insn& s = p->insns[i];
         DInsn& d = out->insns[i];
         if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
         if (s.vtype < 0 || s.vtype > TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
         if (s.vtype == TGPU_V_VARCHAR || s.op == TGPU_EX_LIKE) {
-            TG_TRY(compile_varchar_insn(ctx, p, i, out, max_channel));
+            TG_TRY(compile_varchar_insn(ctx, p, i, out, max_channel, &ts));
             continue;
         }
+        if (string_function(s.op)) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: a string function needs VARCHAR operands", i);
+        for (const tgpu_operand* o : {&s.a, &s.b, &s.c})
+            if (o->kind == TGPU_OPND_TEMP && o->index >= 0 && o->index < TGPU_MAX_TEMPS && ts.vt[o->index] == TGPU_V_VARCHAR && !(s.op == TGPU_EX_IN && o != &s.a))
+                return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads VARCHAR temp %d as another type", i, o->index);
+        ts.vt[s.dst] = result_vtype(s);
+        ts.kind[s.dst] = 0;
         switch (s.op) {
             case TGPU_EX_MOV: case TGPU_EX_ADD: case TGPU_EX_SUB: case TGPU_EX_MUL: case TGPU_EX_DIV: case TGPU_EX_MOD: case TGPU_EX_NEG:
             case TGPU_EX_EQ: case TGPU_EX_NE: case TGPU_EX_LT: case TGPU_EX_LE: case TGPU_EX_GT: case TGPU_EX_GE:
@@ -532,6 +632,31 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         TG_TRY(conv(s.c, &d.c));
         if (s.op == TGPU_EX_IN) d.b.kind = TGPU_OPND_CONST;
     }
+    // VARCHAR projections: the view or the pieces the output is assembled from
+    for (int k = 0; k < p->num_projections && p->projections; k++) {
+        const tgpu_projection& pr = p->projections[k];
+        if (pr.kind != 1 || pr.index < 0 || pr.index >= TGPU_MAX_TEMPS) continue;
+        const int t = pr.index;
+        if ((pr.vtype == TGPU_V_VARCHAR) != (ts.vt[t] == TGPU_V_VARCHAR && p->num_insns > 0))
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "projection %d: the projection's type and what temp %d holds differ", k, t);
+        if (pr.vtype != TGPU_V_VARCHAR) continue;
+        if (out->num_str_outs >= TGD_MAX_STR_OUTS) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "more than %d VARCHAR projections", TGD_MAX_STR_OUTS);
+        DStrOut& so = out->str_out[out->num_str_outs++];
+        memset(&so, 0, sizeof(so));
+        so.temp = t;
+        if (ts.kind[t] == 2) {
+            const DCat& c = out->cat[ts.cat[t]];
+            if (c.inner) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "projection %d: temp %d is also read by a later concatenation", k, t);
+            so.n = c.n;
+            for (int q = 0; q < c.n; q++) { so.slot[q] = c.slot[q]; so.src[q] = c.src[q]; }
+        }
+        else {
+            so.n = 1;
+            so.slot[0] = -1;
+            so.src[0] = ts.src[t];
+        }
+        out->has_strfn = 1;
+    }
     return compile_decimals(ctx, p, out);
 }
 
@@ -541,6 +666,7 @@ int expr_raise(tgpu_ctx* ctx, int64_t errbits)
     if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
     if (errbits & TG_ERR_BIT_DECIMAL_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "Decimal overflow");
     if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
+    if (errbits & TG_ERR_BIT_CONCAT_TOO_LARGE) return tg_fail(ctx, TGPU_ERR_INVALID_FUNCTION_ARGUMENT, "Concatenated string is too large");
     return TGPU_OK;
 }
 
@@ -586,7 +712,66 @@ static void fp_str_operand(const DProgram& prog, const DOperand& o, std::string*
         snprintf(buf, sizeof(buf), "StrRef{(const uint8_t*)tg_pool + %d, %d}", prog.str_off[o.imm], prog.str_len[o.imm]);
         *ref = buf;
     }
+    else if (o.kind == TGPU_OPND_TEMP) {
+        snprintf(buf, sizeof(buf), "tn%d", o.index); *isnull = buf;
+        snprintf(buf, sizeof(buf), "v%d", o.index); *ref = buf;
+    }
     else { *isnull = "true"; *ref = "StrRef{nullptr, 0}"; }
+}
+
+// the first byte of a VARCHAR source in generated code (see DCat): the channel's byte buffer or the constant in tg_pool; `ref` for none
+static std::string fp_src_base(const DProgram& prog, int32_t src, const std::string& ref)
+{
+    if (src == TGD_SRC_NONE) return ref + ".p";
+    if (src >= 0) return "strs.bytes[" + std::to_string(prog.str_slot[src]) + "]";
+    return "((const uint8_t*)tg_pool + " + std::to_string(prog.str_off[-(src + 1)]) + ")";
+}
+
+// straight-line code of one string function: LENGTH (BIGINT t<d>), the views SUBSTR and the trims write (StrRef v<d>), CONCAT (its total
+// length in t<d>, its new pieces in StrRef q<slot>).  Errors as vm_step_str.
+static void fp_emit_strfn_insn(std::string& s, const DProgram& prog, int i)
+{
+    const DInsn& in = prog.insns[i];
+    const int d = in.dst;
+    std::string an, a, bn, b;
+    fp_str_operand(prog, in.a, &an, &a);
+    const std::string ea = fp_operand_error(in.a);
+    if (in.op == TGPU_EX_CONCAT) {
+        const DCat& k = prog.cat[i];
+        fp_str_operand(prog, in.b, &bn, &b);
+        fp_appendf(s, "    { const bool an = %s, bn = %s; const bool rn = an || bn; long long tot = 0;\n", an.c_str(), bn.c_str());
+        if (k.a_slot >= 0 || k.b_slot >= 0) {
+            s += "      if (!rn) {";
+            if (k.a_slot >= 0) fp_appendf(s, " q%d = %s;", k.a_slot, a.c_str());
+            if (k.b_slot >= 0) fp_appendf(s, " q%d = %s;", k.b_slot, b.c_str());
+            s += " }\n";
+        }
+        s += "      if (!rn) tot = 0";
+        for (int q = 0; q < k.n; q++) fp_appendf(s, " + (long long)q%d.len", k.slot[q]);
+        s += ";\n";
+        fp_appendf(s, "      t%d = tot; tn%d = rn; te%d = vm_error_call(an, %s, bn, %s, 0u, rn, %s); }\n", d, d, d, ea.c_str(), fp_operand_error(in.b).c_str(),
+                   k.inner ? "0u" : "tot > TGD_MAX_CONCAT_BYTES ? (unsigned int)TG_ERR_BIT_CONCAT_TOO_LARGE : 0u");
+        return;
+    }
+    fp_appendf(s, "    { const bool an = %s; const StrRef a = %s;\n", an.c_str(), a.c_str());
+    switch (in.op) {
+        case TGPU_EX_LENGTH:
+            fp_appendf(s, "      t%d = an ? 0LL : tg_utf8_count(a); tn%d = an; te%d = %s; }\n", d, d, d, ea.c_str());
+            break;
+        case TGPU_EX_SUBSTR: {
+            const bool has_len = in.c.kind != TGPU_OPND_NONE;
+            fp_appendf(s, "      const Value b = %s, c = %s; const bool rn = an || b.is_null || c.is_null;\n", fp_operand(in.b).c_str(),
+                       has_len ? fp_operand(in.c).c_str() : "Value{0, false}");
+            fp_appendf(s, "      te%d = vm_error_call(an, %s, b.is_null, %s, %s, rn, 0u);\n", d, ea.c_str(), fp_operand_error(in.b).c_str(),
+                       has_len ? fp_operand_error(in.c).c_str() : "0u");
+            fp_appendf(s, "      v%d = rn ? StrRef{nullptr, 0} : tg_substr(a, b.bits, %s, c.bits); tn%d = rn; }\n", d, has_len ? "true" : "false", d);
+            break;
+        }
+        default:
+            fp_appendf(s, "      v%d = an ? StrRef{nullptr, 0} : tg_trim(a, %s, %s); tn%d = an; te%d = %s; }\n", d, in.op != TGPU_EX_RTRIM ? "true" : "false",
+                       in.op != TGPU_EX_LTRIM ? "true" : "false", d, d, ea.c_str());
+            break;
+    }
 }
 
 // `x` (a StrRef) equals pool string k: the length decides first, then packed 8-byte words against immediates (a constant of more than
@@ -611,6 +796,10 @@ static std::string fp_str_eq_const(const std::string& x, const DProgram& prog, i
 // straight-line code of one instruction over VARCHAR operands (result BOOLEAN, never an error)
 static void fp_emit_str_insn(std::string& s, const DProgram& prog, const DInsn& in)
 {
+    if (string_function(in.op)) {
+        fp_emit_strfn_insn(s, prog, (int)(&in - prog.insns));
+        return;
+    }
     std::string an, a, bn, b, cn, c;
     fp_str_operand(prog, in.a, &an, &a);
     fp_appendf(s, "    { const bool an = %s; const StrRef a = %s; bool r = false, rn = an;\n", an.c_str(), a.c_str());
@@ -643,7 +832,18 @@ static void fp_emit_str_insn(std::string& s, const DProgram& prog, const DInsn& 
             else fp_appendf(s, "      if (!rn) r = tg_str_cmp_op(%d, a, %s);\n", in.op, b.c_str());
             break;
     }
-    fp_appendf(s, "      t%d = r ? 1 : 0; tn%d = rn; te%d = 0u; }\n", in.dst, in.dst, in.dst);
+    // the error a view temp operand carries (vm_error_str_pred); none without temp operands
+    std::string e = "0u";
+    if (in.a.kind == TGPU_OPND_TEMP || in.b.kind == TGPU_OPND_TEMP || in.c.kind == TGPU_OPND_TEMP) {
+        const std::string ea = fp_operand_error(in.a), eb = fp_operand_error(in.b), ec = fp_operand_error(in.c);
+        if (in.op == TGPU_EX_IS_NULL || in.op == TGPU_EX_IS_NOT_NULL || in.op == TGPU_EX_LIKE || in.op == TGPU_EX_IN) e = ea;
+        else if (in.op == TGPU_EX_BETWEEN) {
+            fp_str_operand(prog, in.b, &bn, &b);
+            e = "((" + ea + ") || an ? (" + ea + ") : (" + eb + ") ? (" + eb + ") : (!(" + bn + ") && tg_str_cmp(" + b + ", a) > 0) ? 0u : (" + ec + "))";
+        }
+        else e = "((" + ea + ") || an ? (" + ea + ") : (" + eb + "))";
+    }
+    fp_appendf(s, "      t%d = r ? 1 : 0; tn%d = rn; te%d = %s; }\n", in.dst, in.dst, in.dst, e.c_str());
 }
 
 // module-scope data and functions the string operations of `prog` use: the constant pool and one matcher per LIKE pattern, whose
@@ -788,13 +988,14 @@ __global__ void __launch_bounds__(FP_THREADS) fp_filter_kernel(const DProgram* _
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
     __shared__ int64_t temps_hi[DEC ? TGPU_MAX_TEMPS * FP_THREADS : 1];
+    int64_t pieces[TGD_MAX_PIECE_SLOTS];
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t err = 0;
     for (; i < n; i += stride) {
         uint32_t te = 0;
         uint32_t nb = vm_run<true, DEC>(prog, 0, prog->num_filter_insns, cols, i, temps + threadIdx.x, FP_THREADS, 0, &te, 0, 0, &strs,
-                                        DEC ? temps_hi + threadIdx.x : nullptr);
+                                        DEC ? temps_hi + threadIdx.x : nullptr, pieces);
         int ft = prog->filter_temp;
         err |= vm_temp_error(te, ft);
         bool sel = !((nb >> ft) & 1) && temps[ft * FP_THREADS + threadIdx.x] != 0;
@@ -810,6 +1011,7 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
 {
     __shared__ int64_t temps[TGPU_MAX_TEMPS * FP_THREADS];
     __shared__ int64_t temps_hi[DEC ? TGPU_MAX_TEMPS * FP_THREADS : 1];
+    int64_t pieces[TGD_MAX_PIECE_SLOTS];
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t err = 0, nulls_seen = 0;
@@ -818,7 +1020,19 @@ __global__ void __launch_bounds__(FP_THREADS) fp_project_kernel(const DProgram* 
         int64_t* t = temps + threadIdx.x;
         int64_t* th = DEC ? temps_hi + threadIdx.x : nullptr;
         uint32_t te = 0;
-        uint32_t nb = vm_run<true, DEC>(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te, 0, 0, &strs, th);
+        uint32_t nb = vm_run<true, DEC>(prog, 0, prog->num_insns, cols, row, t, FP_THREADS, 0, &te, 0, 0, &strs, th, pieces);
+        // VARCHAR projections: the view in the temp or the concatenation's pieces, as (begin - source base, length) descriptors
+        for (int k = 0; k < out.str_count; k++) {
+            const DStrOut& so = prog->str_out[k];
+            const bool isn = (nb >> so.temp) & 1;
+            err |= vm_temp_error(te, so.temp);
+            int2* d = (int2*)out.str_desc[k] + j * so.n;
+            for (int q = 0; q < so.n; q++) {
+                const int64_t v = so.slot[q] < 0 ? t[so.temp * FP_THREADS] : pieces[so.slot[q]];
+                d[q] = isn ? make_int2(0, 0) : make_int2((int)(uint32_t)v, (int)(v >> 32));
+            }
+            out.str_nullmap[k][j] = isn ? 1 : 0;
+        }
         for (int c = 0; c < out.count; c++) {
             int tp = out.temp[c];
             err |= vm_temp_error(te, tp);
@@ -849,8 +1063,11 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         const DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
         const DDec& d = prog.dec[i];
         const bool lng[3] = {d.la != 0, d.lb != 0, d.lc != 0};
-        for (int k = 0; k < 3; k++)
-            if (ops[k]->kind == TGPU_OPND_COLUMN) (prog.insns[i].vtype == TGPU_V_VARCHAR ? str_used : lng[k] ? wide_used : used)[ops[k]->index] = true;
+        for (int k = 0; k < 3; k++) {
+            // substr's start and length are BIGINT operands
+            const bool str = prog.insns[i].vtype == TGPU_V_VARCHAR && !(prog.insns[i].op == TGPU_EX_SUBSTR && k > 0);
+            if (ops[k]->kind == TGPU_OPND_COLUMN) (str ? str_used : lng[k] ? wide_used : used)[ops[k]->index] = true;
+        }
     }
     std::string loads, temps;
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
@@ -866,6 +1083,11 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     // high words of the temps that hold a long DECIMAL
     for (int t = 0; t < TGPU_MAX_TEMPS; t++)
         if ((prog.long_temps >> t) & 1) fp_appendf(temps, "    long long th%d = 0;\n", t);
+    // string functions: the views temps hold and the captured concatenation pieces
+    if (prog.has_strfn) {
+        for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    StrRef v%d = {nullptr, 0};\n", t);
+        for (int q = 0; q < prog.num_piece_slots; q++) fp_appendf(temps, "    StrRef q%d = {nullptr, 0};\n", q);
+    }
     const bool wide_out = prog.long_temps != 0;
     // value, NULL flag and carried error of the temp behind each computed output column (the only errors a projection raises)
     std::string output_switch = "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true; unsigned int e = 0;\n";
@@ -881,6 +1103,18 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     if (wide_out)
         store = "      if (isn) hv = 0;\n      if (out.vtype[c] == TGD_V_DECIMAL_LONG) ((longlong2*)out.data[c])[j] = make_longlong2(hv, v);\n"
                 "      else if (out.vtype[c] == TGD_V_BOOLEAN) ((signed char*)out.data[c])[j] = (signed char)v; else ((long long*)out.data[c])[j] = v;\n";
+    // VARCHAR projections: one (begin, length) descriptor per piece into the piece's source, and the NULL byte
+    std::string str_store;
+    for (int k = 0; k < prog.num_str_outs; k++) {
+        const DStrOut& so = prog.str_out[k];
+        fp_appendf(str_store, "    { const bool isn = tn%d; err |= te%d; int2* d = (int2*)out.str_desc[%d] + j * %d;\n", so.temp, so.temp, k, so.n);
+        for (int q = 0; q < so.n; q++) {
+            const std::string ref = so.slot[q] < 0 ? "v" + std::to_string(so.temp) : "q" + std::to_string(so.slot[q]);
+            fp_appendf(str_store, "      d[%d] = isn ? make_int2(0, 0) : make_int2((int)(%s.p - %s), %s.len);\n", q, ref.c_str(),
+                       fp_src_base(prog, so.src[q], ref).c_str(), ref.c_str());
+        }
+        fp_appendf(str_store, "      out.str_nullmap[%d][j] = isn ? 1 : 0; }\n", k);
+    }
     // filter kernel
     s += "extern \"C\" __global__ void __launch_bounds__(256) tg_fp_filter_jit(DColumns cols, StrCols strs, long long n, unsigned char* flags, unsigned int* err_out) {\n";
     s += "  unsigned int err = 0;\n  long long stride = (long long)gridDim.x * blockDim.x;\n";
@@ -900,6 +1134,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     s += output_switch;
     s += store;
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
+    s += str_store;
     s += "  }\n  if (err) atomicOr(err_out, err);\n  if (nulls_seen) atomicOr(any_null, nulls_seen);\n}\n";
     // chunked two-pass form (no selection vector): per-row functors + the two kernels around the bodies of device_lib.cuh
     bool chunkable = prog.filter_temp >= 0;
@@ -918,6 +1153,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
     s += output_switch;
     s += store;
     s += "      out.nullmap[c][j] = isn ? 1 : 0;\n      if (isn) nulls_seen |= 1u << c;\n    }\n";
+    s += str_store;
     for (size_t k = 0; k < pass_channels.size(); k++) {
         int ch = pass_channels[k];
         const char* ty = elems[ch] == 16 ? "int4" : elems[ch] == 8 ? "long long" : elems[ch] == 4 ? "int" : elems[ch] == 2 ? "short" : "signed char";
@@ -959,11 +1195,108 @@ __global__ void __launch_bounds__(256) fp_chunk_scan_kernel(const unsigned int* 
     if (t == 255) *total = part[255];
 }
 
+// ---- VARCHAR projection columns ------------------------------------------------------------------------------------------------
+// row length = the sum of the row's piece lengths (0 for a NULL row); len[m] = 0 so that the exclusive scan ends in the total
+__global__ void __launch_bounds__(256) fp_str_lengths_kernel(const int2* __restrict__ desc, int np, const uint8_t* __restrict__ nullmap, int64_t m,
+                                                            long long* __restrict__ len, unsigned int* __restrict__ any_null)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    unsigned int seen = 0;
+    for (; i < m; i += stride) {
+        long long l = 0;
+        for (int q = 0; q < np; q++) l += desc[i * np + q].y;
+        len[i] = l;
+        seen |= nullmap[i];
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) len[m] = 0;
+    if (seen) atomicOr(any_null, 1u);
+}
+
+__global__ void __launch_bounds__(256) fp_str_narrow_kernel(const long long* __restrict__ off64, int64_t n, int32_t* __restrict__ off)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) off[i] = (int32_t)off64[i];
+}
+
+// the sources of one VARCHAR projection's pieces
+struct StrSrcs {
+    const uint8_t* base[TGD_MAX_PIECES];
+};
+
+constexpr int FPS_WARPS = 8;      // warps per CTA of the assembly kernel; a warp owns 32 consecutive output rows at a time
+
+// Byte assembly: a warp owns the contiguous destination range of 32 consecutive output rows.  Its lanes note where each (row, piece)
+// segment starts in the destination and in its source, then store the range as aligned 8-byte words: a lane finds the segment of its
+// word's first byte by binary search and reads the word's bytes with at most one aligned-word load pair per segment it crosses.  Words
+// shared with the neighbouring tiles are stored byte by byte.
+__global__ void __launch_bounds__(FPS_WARPS * 32) fp_str_assemble_kernel(const int2* __restrict__ desc, int np, StrSrcs srcs, const int32_t* __restrict__ off,
+                                                                        int64_t m, uint8_t* __restrict__ dst)
+{
+    __shared__ int32_t seg_dst[FPS_WARPS][32 * TGD_MAX_PIECES + 1];
+    __shared__ int32_t seg_src[FPS_WARPS][32 * TGD_MAX_PIECES];
+    __shared__ const uint8_t* base[TGD_MAX_PIECES];
+#pragma unroll
+    for (int q = 0; q < TGD_MAX_PIECES; q++)      // constant indices: the parameter is read in place, not copied to the stack
+        if (threadIdx.x == q) base[q] = srcs.base[q];
+    __syncthreads();
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int32_t* sd = seg_dst[w];
+    int32_t* ss = seg_src[w];
+    const int nseg = 32 * np;
+    const int64_t tiles = (m + 31) / 32;
+    for (int64_t tile = (int64_t)blockIdx.x * FPS_WARPS + w; tile < tiles; tile += (int64_t)gridDim.x * FPS_WARPS) {
+        const int64_t r0 = tile * 32;
+        const int64_t r = r0 + lane;
+        const int32_t t1 = off[r0 + 32 < m ? r0 + 32 : m];
+        int32_t d = r < m ? off[r] : t1;
+        for (int q = 0; q < np; q++) {
+            const int2 x = r < m ? desc[r * np + q] : make_int2(0, 0);
+            sd[lane * np + q] = d;
+            ss[lane * np + q] = x.x;
+            d += x.y;
+        }
+        if (lane == 0) sd[nseg] = t1;
+        __syncwarp();
+        const int32_t t0 = sd[0];
+        if (t1 > t0) {
+            for (int64_t word = (t0 >> 3) + lane; word <= (int64_t)((t1 - 1) >> 3); word += 32) {
+                const int32_t wb = (int32_t)(word * 8);
+                const int32_t b0 = wb > t0 ? wb : t0, b1 = wb + 8 < t1 ? wb + 8 : t1;
+                // the last segment that starts at or before b0 holds it (empty segments share their start with the next one)
+                int lo = 0, hi = nseg - 1;
+                while (lo < hi) {
+                    const int mid = (lo + hi + 1) >> 1;
+                    if (sd[mid] <= b0) lo = mid;
+                    else hi = mid - 1;
+                }
+                int sg = lo;
+                unsigned long long v = 0;
+                int32_t b = b0;
+                while (b < b1) {
+                    while (sd[sg + 1] <= b) sg++;
+                    const int32_t e = sd[sg + 1] < b1 ? sd[sg + 1] : b1;
+                    const uint8_t* src = base[sg % np] + ss[sg] + (b - sd[sg]);
+                    v |= tg_ld_bytes(src, e - b) << (8 * (b - wb));
+                    b = e;
+                }
+                if (b0 == wb && b1 == wb + 8) *(unsigned long long*)(dst + wb) = v;
+                else
+                    for (int32_t k = b0; k < b1; k++) dst[k] = (uint8_t)(v >> (8 * (k - wb)));
+            }
+        }
+        __syncwarp();
+    }
+}
+
 struct FilterProjectOp : tgpu_op {
     DProgram host_prog;
     DevBuf d_prog;
     std::vector<tgpu_projection> projections;
     int32_t max_channel = -1;
+    StrCols cur_strs;                    // the UTF8 channels of the page in flight (sources of VARCHAR projections)
+    int64_t utf8_limit = INT32_MAX;      // the most bytes a VARCHAR projection column holds (int32 offsets)
     std::vector<OwnedPage*> pending;
     size_t next_out = 0;
     bool finishing = false;
@@ -1010,6 +1343,13 @@ struct FilterProjectOp : tgpu_op {
             }
             for (auto* o : ops) {
                 if (o->kind != TGPU_OPND_COLUMN) continue;
+                if (str && host_prog.insns[i].op == TGPU_EX_SUBSTR && o != ops[0]) {
+                    // substr's start and length: an integer channel
+                    const int t = in.cols[o->index].type;
+                    if (t != TGPU_INT64 && t != TGPU_INT32 && t != TGPU_INT16 && t != TGPU_INT8)
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d as BIGINT, the page's channel is not an integer", i, o->index);
+                    continue;
+                }
                 if (str && in.cols[o->index].type != TGPU_UTF8)
                     return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d as VARCHAR, the page's channel is not UTF8", i, o->index);
                 if (!str && (in.cols[o->index].elem_size() == 0 || in.cols[o->index].elem_size() == 16 || in.cols[o->index].type == TGPU_FLOAT32))
@@ -1022,6 +1362,7 @@ struct FilterProjectOp : tgpu_op {
             strs.offsets[k] = in.cols[host_prog.str_channel[k]].offsets;
             strs.bytes[k] = (const uint8_t*)in.cols[host_prog.str_channel[k]].data;
         }
+        cur_strs = strs;
         unsigned int* d_err = ctx->d_scratch->fp_flags;
         unsigned int* d_anynull = d_err + 1;
         TG_CUDA(ctx, cudaMemsetAsync(d_err, 0, 8, ctx->stream));
@@ -1075,7 +1416,7 @@ struct FilterProjectOp : tgpu_op {
             }
             else TG_TRY(add_computed(pr, m, (int)pi, &outp, &cc));
         }
-        if (cc.oc.count > 0) {
+        if (cc.oc.count > 0 || cc.oc.str_count > 0) {
             int pgrid = tg_grid(ctx, m, FP_THREADS, 8);
             TG_TRY(jit_prepare(in));
             if (jit_project) {
@@ -1096,6 +1437,8 @@ struct FilterProjectOp : tgpu_op {
         OutCols oc;
         std::vector<std::shared_ptr<DevBuf>> nullmaps;   // one byte per row, 1 = NULL
         std::vector<int> at;                             // output column of each computed column
+        std::vector<std::shared_ptr<DevBuf>> str_bufs;   // VARCHAR projection k: descriptors 2k, null map 2k + 1
+        std::vector<int> str_at;
         ComputedCols() { memset(&oc, 0, sizeof(oc)); }
     };
 
@@ -1103,6 +1446,21 @@ struct FilterProjectOp : tgpu_op {
     int add_computed(const tgpu_projection& pr, int64_t m, int pi, DevPage* outp, ComputedCols* cc)
     {
         DevColumn& c = outp->cols[pi];
+        if (pr.vtype == TGPU_V_VARCHAR) {
+            // the piece descriptors and null map; finish_computed assembles the UTF8 column
+            const int k = cc->oc.str_count++;
+            c.type = TGPU_UTF8;
+            c.length = m;
+            auto desc = std::make_shared<DevBuf>(), nm = std::make_shared<DevBuf>();
+            TG_TRY(desc->alloc(ctx, (size_t)m * host_prog.str_out[k].n * 8));
+            TG_TRY(nm->alloc(ctx, (size_t)m));
+            cc->oc.str_desc[k] = desc->p;
+            cc->oc.str_nullmap[k] = nm->as<uint8_t>();
+            cc->str_bufs.push_back(desc);
+            cc->str_bufs.push_back(nm);
+            cc->str_at.push_back(pi);
+            return TGPU_OK;
+        }
         const bool wide = pr.vtype == TGPU_V_DECIMAL && host_prog.temp_dec[pr.index] == 2;     // a long DECIMAL: 16-byte cells
         c.type = pr.vtype == TGPU_V_DOUBLE ? TGPU_FLOAT64 : pr.vtype == TGPU_V_BOOLEAN ? TGPU_INT8 : wide ? TGPU_INT128 : TGPU_INT64;
         c.length = m;
@@ -1130,6 +1488,52 @@ struct FilterProjectOp : tgpu_op {
         uint32_t any_null = (uint32_t)((uint64_t)word >> 32);
         for (int k = 0; k < cc.oc.count; k++)
             if ((any_null >> k) & 1) TG_TRY(attach_validity(cc.nullmaps[k]->as<uint8_t>(), &outp->cols[cc.at[k]]));
+        for (int k = 0; k < cc.oc.str_count; k++) TG_TRY(assemble_str(cc, k, d_err, &outp->cols[cc.str_at[k]]));
+        return TGPU_OK;
+    }
+
+    // VARCHAR projection k: row lengths from the piece descriptors, a 64-bit scan to offsets (a column past utf8_limit bytes fails
+    // before anything is written), then the bytes
+    int assemble_str(const ComputedCols& cc, int k, unsigned int* d_any, DevColumn* c)
+    {
+        const DStrOut& so = host_prog.str_out[k];
+        const int64_t m = c->length;
+        const int2* desc = (const int2*)cc.oc.str_desc[k];
+        const uint8_t* nullmap = cc.oc.str_nullmap[k];
+        DevBuf len, off64;
+        TG_TRY(len.alloc(ctx, (size_t)(m + 1) * 8));
+        TG_TRY(off64.alloc(ctx, (size_t)(m + 1) * 8));
+        TG_CUDA(ctx, cudaMemsetAsync(d_any, 0, 4, ctx->stream));
+        TG_LAUNCH(ctx, fp_str_lengths_kernel, tg_grid(ctx, m, 256, 8), 256, 0, desc, so.n, nullmap, m, len.as<long long>(), d_any);
+        TG_TRY(tg_exclusive_sum(ctx, len.as<long long>(), off64.as<long long>(), m + 1));
+        int64_t total = 0, any = 0;
+        TG_TRY(tg_read_i64(ctx, off64.as<long long>() + m, &total));
+        TG_TRY(tg_read_i64(ctx, d_any, &any));
+        if (total > utf8_limit)
+            return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "VARCHAR projection %d holds %lld bytes, past the %lld a UTF8 column holds", k, (long long)total,
+                           (long long)utf8_limit);
+        c->own_offsets = std::make_shared<DevBuf>();
+        TG_TRY(c->own_offsets->alloc(ctx, (size_t)(m + 1) * 4));
+        TG_LAUNCH(ctx, fp_str_narrow_kernel, tg_grid(ctx, m + 1, 256, 8), 256, 0, off64.as<long long>(), m + 1, c->own_offsets->as<int32_t>());
+        c->offsets = c->own_offsets->as<int32_t>();
+        c->own_data = std::make_shared<DevBuf>();
+        TG_TRY(c->own_data->alloc(ctx, (size_t)total));
+        c->data = c->own_data->p;
+        c->data_bytes = total;
+        StrSrcs srcs;
+        memset(&srcs, 0, sizeof(srcs));
+        for (int q = 0; q < so.n; q++) {
+            const int32_t src = so.src[q];
+            if (src == TGD_SRC_NONE) srcs.base[q] = nullptr;
+            else if (src >= 0) srcs.base[q] = cur_strs.bytes[host_prog.str_slot[src]];
+            else srcs.base[q] = d_prog.as<uint8_t>() + offsetof(DProgram, str_bytes) + host_prog.str_off[-(src + 1)];
+        }
+        if (total > 0) {
+            const int64_t tiles = tg_div_up(m, 32);
+            TG_LAUNCH(ctx, fp_str_assemble_kernel, tg_grid(ctx, tiles, FPS_WARPS, 8), FPS_WARPS * 32, 0, desc, so.n, srcs, c->offsets, m,
+                      c->own_data->as<uint8_t>());
+        }
+        if (any & 0xFFFFFFFFLL) TG_TRY(attach_validity(nullmap, c));
         return TGPU_OK;
     }
 
@@ -1287,6 +1691,8 @@ extern "C" int tgpu_filter_project_create(tgpu_ctx* ctx, const tgpu_expr_program
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
     std::unique_ptr<FilterProjectOp> op(new FilterProjectOp(ctx));
     TG_TRY(tg::expr_compile(ctx, program, &op->host_prog, &op->max_channel));
+    // a smaller byte limit for VARCHAR projection columns, so that the INT32_MAX guard can be exercised on small pages
+    if (const char* lim = getenv("TGPU_UTF8_COLUMN_LIMIT")) op->utf8_limit = std::min<int64_t>(INT32_MAX, std::max<int64_t>(0, atoll(lim)));
     if (program->num_projections > TGPU_MAX_CHANNELS) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "more than %d projections", TGPU_MAX_CHANNELS);
     for (int i = 0; i < program->num_projections; i++) {
         const tgpu_projection& p = program->projections[i];

@@ -32,6 +32,22 @@ struct DInsn {
     DOperand a, b, c;
 };
 
+// The source of a VARCHAR view: >= 0 a UTF8 channel, < 0 (but TGD_SRC_NONE) pool constant -(src + 1), TGD_SRC_NONE a NULL operand
+// One CONCAT instruction: its result's pieces (piece slots and their sources); a_slot / b_slot: the slot operand a / b is captured in
+// (-1: the operand is a CONCAT temp, whose pieces come first / last); inner: the result is read by a later CONCAT, so it carries its
+// operands' errors only and that CONCAT checks the length over all pieces (the variadic call's one check)
+struct DCat {
+    int8_t n, inner, a_slot, b_slot;
+    int8_t slot[TGD_MAX_PIECES];
+    int32_t src[TGD_MAX_PIECES];
+};
+// One VARCHAR projection: its temp and pieces (slot -1: the view in the temp itself)
+struct DStrOut {
+    int32_t temp, n;
+    int32_t slot[TGD_MAX_PIECES];
+    int32_t src[TGD_MAX_PIECES];
+};
+
 struct DProgram {
     int32_t num_insns;
     int32_t num_filter_insns;   // instructions [0, num_filter_insns) compute the filter
@@ -61,6 +77,15 @@ struct DProgram {
     int8_t temp_dec[TGPU_MAX_TEMPS];
     DDec dec[TGPU_MAX_INSNS];
     int64_t in_hi[128];
+    // string functions (FilterAndProject only; has_strfn = 0: none).  A VARCHAR TEMP operand's imm names the source of the view the
+    // temp holds (DStrSrc encoding).  A view temp holds (begin - source base) in its low and the length in its high 32 bits; a CONCAT
+    // temp holds the total length, its pieces live in piece slots.  cat[i]: CONCAT instruction i; str_out[k]: the k-th VARCHAR projection
+    int32_t has_strfn;
+    int32_t num_piece_slots;
+    int32_t num_str_outs;
+    int32_t strfn_pad;
+    DCat cat[TGPU_MAX_INSNS];
+    DStrOut str_out[TGD_MAX_STR_OUTS];
 };
 
 // the program has an instruction over VARCHAR operands (or a LIKE)
@@ -107,14 +132,31 @@ __device__ __forceinline__ uint32_t vm_carried(const DOperand& o, uint32_t errs)
     return o.kind == TGPU_OPND_TEMP ? (errs >> (4 * o.index)) & 0xFu : 0u;
 }
 
-__device__ __forceinline__ uint32_t vm_temp_error(uint32_t errs, int t) { return (errs >> (4 * t)) & 0xFu; }
+__device__ __forceinline__ uint32_t vm_temp_error(uint32_t errs, int t)
+{
+    const uint32_t e = (errs >> (4 * t)) & 0xFu;
+    return e == TG_ERR_CODE_CONCAT ? (uint32_t)TG_ERR_BIT_CONCAT_TOO_LARGE : e;
+}
 
-// Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
-// [temp][thread] array (stride tstride).  Returns the updated null bitmask; *errs holds the TG_ERR_BIT_* each temp
-// carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.  `split` / `split_row`: see vm_fetch.
-// A VARCHAR operand: a UTF8 channel (through `strs`), a pool constant or NULL
+// the first byte of a VARCHAR source (DCat::src encoding): a UTF8 channel's byte buffer or a pool constant
+__device__ __forceinline__ const uint8_t* vm_src_base(const DProgram* __restrict__ prog, const StrCols& strs, int32_t src)
+{
+    if (src == TGD_SRC_NONE) return nullptr;
+    if (src >= 0) return strs.bytes[prog->str_slot[src]];
+    return prog->str_bytes + prog->str_off[-(src + 1)];
+}
+
+__device__ __forceinline__ int32_t vm_opnd_src(const DOperand& o)
+{
+    if (o.kind == TGPU_OPND_COLUMN) return o.index;
+    if (o.kind == TGPU_OPND_CONST) return (int32_t)(-(o.imm + 1));
+    if (o.kind == TGPU_OPND_TEMP) return (int32_t)o.imm;
+    return TGD_SRC_NONE;
+}
+
+// A VARCHAR operand: a UTF8 channel (through `strs`), a pool constant, NULL, or a temp holding a view (begin - source base, length)
 __device__ __forceinline__ StrRef vm_fetch_str(const DProgram* __restrict__ prog, const DOperand& o, const DColumns& cols, const StrCols& strs, int64_t row,
-                                               bool* is_null)
+                                               bool* is_null, const int64_t* temps = nullptr, int tstride = 0, uint32_t nullbits = 0)
 {
     if (o.kind == TGPU_OPND_COLUMN) {
         *is_null = !tg_valid(cols.cols[o.index].validity, row);
@@ -125,17 +167,24 @@ __device__ __forceinline__ StrRef vm_fetch_str(const DProgram* __restrict__ prog
         *is_null = false;
         return StrRef{prog->str_bytes + prog->str_off[o.imm], prog->str_len[o.imm]};
     }
+    if (o.kind == TGPU_OPND_TEMP) {
+        *is_null = (nullbits >> o.index) & 1;
+        if (*is_null) return StrRef{nullptr, 0};
+        const int64_t v = temps[o.index * tstride];
+        return StrRef{vm_src_base(prog, strs, (int32_t)o.imm) + (uint32_t)v, (int32_t)(v >> 32)};
+    }
     *is_null = true;
     return StrRef{nullptr, 0};
 }
 
-// One string operation: BOOLEAN result, NULL as for the numeric operations, never an error (its operands are never temps)
-__device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog, const DInsn& in, const DColumns& cols, const StrCols& strs, int64_t row)
+// One string predicate: BOOLEAN result, NULL as for the numeric operations
+__device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog, const DInsn& in, const DColumns& cols, const StrCols& strs, int64_t row,
+                                              const int64_t* temps = nullptr, int tstride = 0, uint32_t nullbits = 0)
 {
     Value r;
     r.bits = 0;
     bool an, bn = true, cn = true;
-    const StrRef a = vm_fetch_str(prog, in.a, cols, strs, row, &an);
+    const StrRef a = vm_fetch_str(prog, in.a, cols, strs, row, &an, temps, tstride, nullbits);
     switch (in.op) {
         case TGPU_EX_IS_NULL: r.is_null = false; r.bits = an ? 1 : 0; return r;
         case TGPU_EX_IS_NOT_NULL: r.is_null = false; r.bits = an ? 0 : 1; return r;
@@ -156,8 +205,8 @@ __device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog,
             return r;
         }
         case TGPU_EX_BETWEEN: {
-            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn);
-            const StrRef c = vm_fetch_str(prog, in.c, cols, strs, row, &cn);
+            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn, temps, tstride, nullbits);
+            const StrRef c = vm_fetch_str(prog, in.c, cols, strs, row, &cn, temps, tstride, nullbits);
             const bool n1 = an || bn, n2 = an || cn;
             const bool f1 = !n1 && tg_str_cmp(a, b) < 0, f2 = !n2 && tg_str_cmp(a, c) > 0;
             r.is_null = !(f1 || f2) && (n1 || n2);
@@ -165,12 +214,99 @@ __device__ __forceinline__ Value vm_apply_str(const DProgram* __restrict__ prog,
             return r;
         }
         default: {
-            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn);
+            const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn, temps, tstride, nullbits);
             r.is_null = an || bn;
             if (!r.is_null) r.bits = tg_str_cmp_op(in.op, a, b) ? 1 : 0;
             return r;
         }
     }
+}
+
+// The error a string predicate's result carries: its VARCHAR temp operands' (a view carries the error of a substr's start or length),
+// by vm_error's rules
+__device__ __forceinline__ uint32_t vm_error_str_pred(const DProgram* __restrict__ prog, const DInsn& in, const DColumns& cols, const StrCols& strs, int64_t row,
+                                                      const int64_t* temps, int tstride, uint32_t nullbits, uint32_t te)
+{
+    const uint32_t ea = vm_carried(in.a, te);
+    if (in.op == TGPU_EX_IS_NULL || in.op == TGPU_EX_IS_NOT_NULL || in.op == TGPU_EX_LIKE || in.op == TGPU_EX_IN) return ea;
+    bool an, bn;
+    const StrRef a = vm_fetch_str(prog, in.a, cols, strs, row, &an, temps, tstride, nullbits);
+    if (ea || an) return ea;
+    const uint32_t eb = vm_carried(in.b, te);
+    if (in.op != TGPU_EX_BETWEEN || eb) return eb;
+    const StrRef b = vm_fetch_str(prog, in.b, cols, strs, row, &bn, temps, tstride, nullbits);
+    if (!bn && tg_str_cmp(b, a) > 0) return 0;
+    return vm_carried(in.c, te);
+}
+
+// One instruction over VARCHAR operands in the interpreter: predicates, LENGTH, the views SUBSTR and the trims write (begin - source base
+// in the low word, length in the high word), and CONCAT, which captures its new pieces in `pieces` and writes the total length
+__device__ __forceinline__ void vm_step_str(const DProgram* __restrict__ prog, int pc, const DInsn& in, const DColumns& cols, const StrCols& strs, int64_t row,
+                                            int64_t* temps, int tstride, uint32_t* nullbits, uint32_t* te, int64_t* pieces)
+{
+    int64_t r = 0;
+    bool rn;
+    uint32_t e;
+    const uint32_t nb = *nullbits;
+    switch (in.op) {
+        case TGPU_EX_LENGTH: case TGPU_EX_SUBSTR: case TGPU_EX_LTRIM: case TGPU_EX_RTRIM: case TGPU_EX_TRIM: {
+            bool an;
+            const StrRef a = vm_fetch_str(prog, in.a, cols, strs, row, &an, temps, tstride, nb);
+            const uint32_t ea = vm_carried(in.a, *te);
+            if (in.op == TGPU_EX_LENGTH) {
+                rn = an;
+                e = ea;
+                if (!an) r = tg_utf8_count(a);
+                break;
+            }
+            StrRef v = a;
+            if (in.op == TGPU_EX_SUBSTR) {
+                const bool has_len = in.c.kind != TGPU_OPND_NONE;
+                const Value b = vm_fetch(in.b, cols, row, temps, tstride, nb);
+                Value c;
+                c.bits = 0;
+                c.is_null = false;
+                if (has_len) c = vm_fetch(in.c, cols, row, temps, tstride, nb);
+                rn = an || b.is_null || c.is_null;
+                e = vm_error_call(an, ea, b.is_null, vm_carried(in.b, *te), has_len ? vm_carried(in.c, *te) : 0u, rn, 0u);
+                if (!rn) v = tg_substr(a, b.bits, has_len, c.bits);
+            }
+            else {
+                rn = an;
+                e = ea;
+                if (!rn) v = tg_trim(a, in.op != TGPU_EX_RTRIM, in.op != TGPU_EX_LTRIM);
+            }
+            if (!rn) r = (int64_t)(uint32_t)(v.p - vm_src_base(prog, strs, vm_opnd_src(in.a))) | ((int64_t)v.len << 32);
+            break;
+        }
+        case TGPU_EX_CONCAT: {
+            const DCat& k = prog->cat[pc];
+            bool an, bn;
+            StrRef a = StrRef{nullptr, 0}, b = StrRef{nullptr, 0};
+            if (k.a_slot >= 0) a = vm_fetch_str(prog, in.a, cols, strs, row, &an, temps, tstride, nb);
+            else an = (nb >> in.a.index) & 1;
+            if (k.b_slot >= 0) b = vm_fetch_str(prog, in.b, cols, strs, row, &bn, temps, tstride, nb);
+            else bn = (nb >> in.b.index) & 1;
+            rn = an || bn;
+            if (!rn) {
+                if (k.a_slot >= 0) pieces[k.a_slot] = (int64_t)(uint32_t)(a.p - vm_src_base(prog, strs, vm_opnd_src(in.a))) | ((int64_t)a.len << 32);
+                if (k.b_slot >= 0) pieces[k.b_slot] = (int64_t)(uint32_t)(b.p - vm_src_base(prog, strs, vm_opnd_src(in.b))) | ((int64_t)b.len << 32);
+                for (int q = 0; q < k.n; q++) r += pieces[k.slot[q]] >> 32;
+            }
+            e = vm_error_call(an, vm_carried(in.a, *te), bn, vm_carried(in.b, *te), 0u, rn, !k.inner && r > TGD_MAX_CONCAT_BYTES ? TG_ERR_CODE_CONCAT : 0u);
+            break;
+        }
+        default: {
+            const Value v = vm_apply_str(prog, in, cols, strs, row, temps, tstride, nb);
+            r = v.bits;
+            rn = v.is_null;
+            e = vm_error_str_pred(prog, in, cols, strs, row, temps, tstride, nb, *te);
+            break;
+        }
+    }
+    temps[in.dst * tstride] = r;
+    *nullbits = (nb & ~(1u << in.dst)) | ((rn ? 1u : 0u) << in.dst);
+    *te = (*te & ~(0xFu << (4 * in.dst))) | (e << (4 * in.dst));
 }
 
 // A DECIMAL operand (or the BIGINT operand of a cast to DECIMAL) as a 128-bit value: `lng` = a long decimal (a TGPU_INT128 channel's
@@ -235,12 +371,15 @@ __device__ __forceinline__ void vm_step_dec(const DProgram* __restrict__ prog, c
     *te = (*te & ~(0xFu << (4 * in.dst))) | (e << (4 * in.dst));
 }
 
-// STR: the program may hold string operations (FilterAndProject), read through `strs`.  DEC: the program may hold DECIMAL operations
+// Runs instructions [first, last) for one row.  `temps` points at this thread's column of the shared
+// [temp][thread] array (stride tstride).  Returns the updated null bitmask; *errs holds the TG_ERR_BIT_* each temp
+// carries (4 bits per temp, see vm_error): the caller raises those of the temps it reads.  `split` / `split_row`: see vm_fetch.
+// STR: the program may hold string operations (FilterAndProject), read through `strs`; `pieces`: the thread's concatenation piece slots.  DEC: the program may hold DECIMAL operations
 // (FilterAndProject), whose temps keep their high words in `thi` (same layout as `temps`)
 template <bool STR = false, bool DEC = false>
 __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, int first, int last, const DColumns& cols, int64_t row,
                                            int64_t* temps, int tstride, uint32_t nullbits, uint32_t* errs, int split = 0, int64_t split_row = 0,
-                                           const StrCols* strs = nullptr, int64_t* thi = nullptr)
+                                           const StrCols* strs = nullptr, int64_t* thi = nullptr, int64_t* pieces = nullptr)
 {
     uint32_t te = *errs;
     for (int pc = first; pc < last; pc++) {
@@ -250,10 +389,7 @@ __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, in
             continue;
         }
         if (STR && in.vtype == TGPU_V_VARCHAR) {
-            const Value v = vm_apply_str(prog, in, cols, *strs, row);
-            temps[in.dst * tstride] = v.bits;
-            nullbits = (nullbits & ~(1u << in.dst)) | ((v.is_null ? 1u : 0u) << in.dst);
-            te &= ~(0xFu << (4 * in.dst));
+            vm_step_str(prog, pc, in, cols, *strs, row, temps, tstride, &nullbits, &te, pieces);
             continue;
         }
         Value a = vm_fetch(in.a, cols, row, temps, tstride, nullbits, split, split_row);

@@ -349,6 +349,8 @@ class Call:
     """op: one of abi.EX_*; args: expressions.  vtype is the OPERAND type (result of comparisons is BOOLEAN).
     EX_IN takes in_list (str / bytes values for a VARCHAR operand, unscaled ints for a DECIMAL one); EX_LIKE takes the constant pattern
     and an optional one-character escape (str / bytes): `value LIKE pattern [ESCAPE escape]`.
+    String functions: EX_LENGTH(s) gives BIGINT; EX_SUBSTR(s, start[, length]) with BIGINT start and length, EX_LTRIM / EX_RTRIM /
+    EX_TRIM(s) and EX_CONCAT(a, b) give VARCHAR (see concat() for more than two pieces).
     DECIMAL: the result type of +, -, *, / follows the reference's default rules (legacy=True: the legacy ones) unless result_dtype gives
     it; EX_CAST_TO_DECIMAL needs result_dtype."""
 
@@ -365,7 +367,7 @@ class Call:
             self.result_vtype = abi.V_BOOLEAN
         elif op in (abi.EX_CAST_BIGINT_TO_DOUBLE, abi.EX_CAST_DECIMAL_TO_DOUBLE):
             self.result_vtype = abi.V_DOUBLE
-        elif op in (abi.EX_CAST_DOUBLE_TO_BIGINT, abi.EX_CAST_DECIMAL_TO_BIGINT):
+        elif op in (abi.EX_CAST_DOUBLE_TO_BIGINT, abi.EX_CAST_DECIMAL_TO_BIGINT, abi.EX_LENGTH):
             self.result_vtype = abi.V_BIGINT
         elif op == abi.EX_CAST_TO_DECIMAL:
             if result_dtype is None:
@@ -380,6 +382,17 @@ class Call:
     @property
     def vtype(self):
         return self.result_vtype
+
+
+def concat(*args):
+    """concat(x1, ..., xn) and x1 || ... || xn as the left-deep chain of binary EX_CONCATs the library evaluates (the same value and the
+    same error as the variadic call)"""
+    if len(args) < 2:
+        raise ValueError("There must be two or more concatenation arguments")
+    e = Call(abi.EX_CONCAT, args[0], args[1])
+    for a in args[2:]:
+        e = Call(abi.EX_CONCAT, e, a)
+    return e
 
 
 class PageProcessorProgram:
