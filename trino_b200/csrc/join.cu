@@ -1533,6 +1533,14 @@ bool join_filter_type_ok(const DevColumn& c) { return c.elem_size() != 0 && c.el
 
 int key_kind_of(int type) { return type == TGPU_FLOAT64 ? KEY_DOUBLE : KEY_INT; }
 
+// a probe channel can be looked up in a table keyed by one fixed-width channel: VARCHAR, long DECIMAL and REAL builds are generic
+// lookups, so a probe channel of those types (read as 1- or 4-byte integers otherwise) never belongs to such a table
+bool probe_key_fits_keyed_table(int probe_type, int build_type)
+{
+    if (probe_type == TGPU_UTF8 || probe_type == TGPU_INT128 || probe_type == TGPU_FLOAT32) return false;
+    return key_kind_of(probe_type) == key_kind_of(build_type);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1624,8 +1632,11 @@ int lookup_positions(tgpu_ctx* ctx, const tgpu_lookup* lk, const DevColumn& key,
 {
     int64_t n = key.length;
     if (n == 0) return TGPU_OK;
-    if (key.type == TGPU_UTF8) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "variable-width join keys are not supported on the GPU path");
-    if (key_kind_of(key.type) != key_kind_of(lk->key_type) || key.elem_size() == 0)
+    if (lk->positions == 0) {      // nothing to match, and a build that never saw a page has no key type to compare with: every row misses
+        TG_CUDA(ctx, cudaMemsetAsync(d_out, 0xFF, (size_t)n * 4, ctx->stream));
+        return TGPU_OK;
+    }
+    if (!probe_key_fits_keyed_table(key.type, lk->key_type) || key.elem_size() == 0)
         return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "probe key type %d does not match build key type %d", key.type, lk->key_type);
     const JoinSlot* table = lk->table.as<JoinSlot>();
     bool fast = key.type == TGPU_INT64 && !key.validity;
@@ -1660,10 +1671,15 @@ int lookup_positions(tgpu_ctx* ctx, const tgpu_lookup* lk, const DevColumn& key,
 int lookup_positions_generic(tgpu_ctx* ctx, const tgpu_lookup* lk, const std::vector<const DevColumn*>& keys, int64_t n, int* d_out)
 {
     if (keys.size() != lk->build_keys.size()) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "probe has %zu join channels, build has %zu", keys.size(), lk->build_keys.size());
-    for (size_t c = 0; c < keys.size(); c++) {
-        bool pu = keys[c]->type == TGPU_UTF8, bu = lk->build_keys[c].type == TGPU_UTF8, pd = keys[c]->type == TGPU_FLOAT64, bd = lk->build_keys[c].type == TGPU_FLOAT64;
-        bool pr = keys[c]->type == TGPU_FLOAT32, br = lk->build_keys[c].type == TGPU_FLOAT32;
-        if (pu != bu || pd != bd || pr != br) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "join channel %zu: probe type %d does not match build type %d", c, keys[c]->type, lk->build_keys[c].type);
+    // col_value_equal decides from the probe channel how both sides are read: VARCHAR, DOUBLE, REAL and long DECIMAL must agree per channel
+    // (a 16-byte probe channel would read past the end of an 8-byte build column).  Integer channels of different widths compare by value,
+    // each side read at its own width, as in a lookup keyed by one channel.  A build that never saw a page has no channel types and no row
+    // to compare with: every probe row misses
+    for (size_t c = 0; c < keys.size() && lk->positions > 0; c++) {
+        const DevColumn &p = *keys[c], &b = lk->build_keys[c];
+        bool same = (p.type == TGPU_UTF8) == (b.type == TGPU_UTF8) && (p.type == TGPU_FLOAT64) == (b.type == TGPU_FLOAT64) &&
+                    (p.type == TGPU_FLOAT32) == (b.type == TGPU_FLOAT32) && (p.type == TGPU_INT128) == (b.type == TGPU_INT128);
+        if (!same) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "join channel %zu: probe type %d does not match build type %d", c, p.type, b.type);
     }
     if (n == 0) return TGPU_OK;
     DevColumn fp;
@@ -2138,8 +2154,8 @@ struct JoinProbeOp : tgpu_op {
         *handled = false;
         
         if (lookup->has_dups && !single_match) return TGPU_OK;
-        if (lookup->num_output > 4 || key.type == TGPU_UTF8) return TGPU_OK;
-        if (key_kind_of(key.type) != key_kind_of(lookup->key_type)) return TGPU_OK;   // reported by the general path
+        if (lookup->num_output > 4) return TGPU_OK;
+        if (!probe_key_fits_keyed_table(key.type, lookup->key_type)) return TGPU_OK;   // reported by the general path
         for (int32_t b = 0; b < lookup->num_output; b++) {
             const DevColumn& c = lookup->store.cols[1 + b];
             if (c.elem_size() == 0 || c.elem_size() > 8 || c.validity) return TGPU_OK;      // (the fused gather moves 1 / 2 / 4 / 8-byte payloads)
