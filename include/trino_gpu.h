@@ -475,13 +475,17 @@ int tgpu_semi_join_create(tgpu_ctx* ctx, tgpu_lookup* lookup, int32_t probe_join
 /* DynamicFilterSourceOperator / JoinDomainBuilder (M/operator/DynamicFilterSourceOperator.java, M/operator/JoinDomainBuilder.java):
  * the domain of the build-side join key read off the finished table: min, max and number of distinct non-NULL keys, and the keys
  * themselves (ascending) when there are at most `max_values` of them (distinct_out > max_values: only min/max are meaningful, the
- * reference's fallback to a range).  Single BIGINT-family key only. */
+ * reference's fallback to a range).  distinct_out == 0 (no build rows, or only NULL keys): min_out = INT64_MAX > max_out = INT64_MIN,
+ * and the caller must use a NONE domain.  Single integer-family key only (BIGINT, INTEGER, DATE, SMALLINT, TINYINT, short DECIMAL);
+ * DOUBLE, REAL, VARCHAR, long DECIMAL and multi-channel keys answer TGPU_ERR_NOT_SUPPORTED. */
 int tgpu_lookup_key_domain(tgpu_ctx* ctx, tgpu_lookup* lookup, int64_t max_values, int64_t* min_out, int64_t* max_out, int64_t* distinct_out,
                            int64_t* values_out, int32_t* has_null_out);
 
 /* DynamicPageFilter (M/sql/gen/columnar/DynamicPageFilter.java:47-211): the probe-side half of dynamic filtering.  One Domain per
  * filtered channel = `null_allowed` + a value set (Domain.includesNullableValue): ALL, NONE, one inclusive range [min, max]
- * (integer family, and DOUBLE by value), or DISCRETE values (integer family; any order, sorted here).  Filters apply in the given order to
+ * (integer family (not long DECIMAL), and DOUBLE by value), or DISCRETE values (integer family (not long DECIMAL); any order, sorted
+ * here).  ALL and NONE take a channel of any type; RANGE / DISCRETE over REAL, VARCHAR or long DECIMAL channels and DISCRETE over DOUBLE
+ * answer TGPU_ERR_NOT_SUPPORTED at the first page.  Filters apply in the given order to
  * the surviving rows (DynamicFilterEvaluator.evaluate :160-178); a filter that, after >= 2047 input positions, passes more than
  * selectivity_threshold of them is switched off (EffectiveFilterProfiler :181-210).  A Range with an exclusive upper bound over integers is
  * passed as max = bound - 1.  Zero domains = TupleDomain.all() (every page passes through); TupleDomain.none() = one NONE domain.

@@ -5,6 +5,9 @@ after another to the surviving positions (DynamicFilterEvaluator.evaluate :160-1
 (:181-210: once a filter has seen >= 2047 input positions and passed more than selectivityThreshold of them it is skipped from the
 next page on).  A Domain contains a row's value iff the value is NULL and nulls are allowed, or it is non-NULL and in the value set
 (S/predicate/Domain.java includesNullableValue).  Pinned on the cases of T/sql/gen/TestDynamicPageFilter.java (tests/test_oracle_dynamic_filter.py).
+
+A DOUBLE range (`double=True`) compares by value, as DoubleType.compare does: bounds and column values are raw IEEE bits (the
+LongArrayBlock of a DOUBLE column), decoded to float64 first, so -0.0 == 0.0 and NaN lies in no range.
 """
 import numpy as np
 
@@ -12,9 +15,13 @@ ALL, NONE, RANGE, DISCRETE = 0, 1, 2, 3
 MIN_SAMPLE_POSITIONS = 2047
 
 
+def _as_double(bits):
+    return np.asarray(bits, dtype=np.int64).view(np.float64)
+
+
 class Domain:
-    def __init__(self, channel, kind, null_allowed=False, lo=0, hi=0, values=None):
-        self.channel, self.kind, self.null_allowed, self.lo, self.hi = channel, kind, null_allowed, lo, hi
+    def __init__(self, channel, kind, null_allowed=False, lo=0, hi=0, values=None, double=False):
+        self.channel, self.kind, self.null_allowed, self.lo, self.hi, self.double = channel, kind, null_allowed, lo, hi, double
         self.values = None if values is None else np.asarray(sorted(values), dtype=np.int64)
 
     def contains(self, values, nulls):
@@ -24,6 +31,9 @@ class Domain:
             ok = np.ones(n, dtype=bool)
         elif self.kind == NONE:
             ok = np.zeros(n, dtype=bool)
+        elif self.kind == RANGE and self.double:
+            x = _as_double(values)
+            ok = (x >= _as_double([self.lo])[0]) & (x <= _as_double([self.hi])[0])     # NaN compares false both ways
         elif self.kind == RANGE:
             ok = (values >= self.lo) & (values <= self.hi)          # inclusive bounds; an exclusive integer bound arrives as bound - 1
         else:

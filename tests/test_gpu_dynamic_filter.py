@@ -5,7 +5,6 @@ import pytest
 
 import oracle_lib as o
 from test_oracle_dynamic_filter import df, golden_cases
-from trino_b200 import abi
 from trino_b200 import operators as ops
 from trino_b200.page import Block, Page
 
@@ -72,7 +71,7 @@ def test_all_none_and_build_side_domain(ctx):
     op = ops.DynamicFilterOperatorFactory(ctx, [ops.ColumnDomain.none(0)]).create_operator()    # TupleDomain.none(): testNonePageFilter :95-103
     assert _selected_rows(op, page) == []
     op.close()
-    op = ops.DynamicFilterOperatorFactory(ctx, [ops.ColumnDomain(1, abi.DOMAIN_RANGE, False, *np.array([0.0, 1.0]).view(np.int64).tolist())]).create_operator()
+    op = ops.DynamicFilterOperatorFactory(ctx, [ops.ColumnDomain.double_range(1, 0.0, 1.0)]).create_operator()
     assert _selected_rows(op, page) == [(1, 0.5)]                              # DOUBLE range by value, NULL rejected
     op.close()
     # end to end: the build side's key domain (tgpu_lookup_key_domain) prunes the probe page before the join

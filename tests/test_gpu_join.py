@@ -381,6 +381,76 @@ def test_build_side_key_domain(ctx):
     assert (lo, hi, cnt, has_null) == (-2**63, 7, 3, False) and list(values) == [-2**63, 3, 7]
     lookup.close()
     b.close()
+    # every integer key type (the last: short DECIMAL), the type's extremes as keys
+    for make, lo_t, hi_t in ((Block.integer, -2**31, 2**31 - 1), (Block.date, -719_162, 2_932_896), (Block.smallint, -2**15, 2**15 - 1),
+                             (Block.tinyint, -128, 127), (Block.bigint, -10**18 + 1, 10**18 - 1)):
+        keys = np.concatenate([rng.integers(max(lo_t, -60), min(hi_t, 60), 3000, endpoint=True), [lo_t, hi_t, lo_t]])
+        nulls = rng.random(len(keys)) < 0.05
+        nulls[-3:] = False
+        _check_key_domain(ctx, [Page(make(keys[:1000], nulls[:1000])), Page(make(keys[1000:], nulls[1000:]))], keys, nulls)
+    # no key at all: the domain is empty (min INT64_MAX > max INT64_MIN) and the caller uses a NONE domain
+    _check_key_domain(ctx, [Page(Block.bigint([]), position_count=0)], np.zeros(0, dtype=np.int64), np.zeros(0, dtype=bool))
+    _check_key_domain(ctx, [Page(Block.integer(np.arange(50), np.ones(50, dtype=bool)))], np.arange(50), np.ones(50, dtype=bool))
+    # keys without one 64-bit integer form are not collected
+    for build, channels in ((Page(Block.varchar(["a", "b"])), [0]), (Page(Block.real([1.5, 2.5])), [0]), (Page(Block.int128([10**30, 1])), [0]),
+                            (Page(Block.double([1.5, -0.0])), [0]), (Page(Block.bigint([1, 2]), Block.bigint([3, 4])), [0, 1])):
+        bridge = ops.JoinBridge()
+        b = ops.HashBuilderOperatorFactory(ctx, bridge, channels, []).create_operator()
+        b.add_input(build)
+        b.finish()
+        with pytest.raises(abi.TrinoGpuError) as err:
+            bridge.lookup_source.key_domain(8)
+        assert err.value.code == abi.ERR_NOT_SUPPORTED
+        bridge.lookup_source.close()
+        b.close()
+
+
+def _check_key_domain(ctx, build_pages, keys, nulls, out=()):
+    """tgpu_lookup_key_domain of a build against np.unique of its non-NULL keys, at max_values 0, one less than the distinct count,
+    exactly the distinct count and far above it"""
+    b, lookup = _build_lookup(ctx, build_pages, out=out)
+    want = np.unique(np.asarray(keys, dtype=np.int64)[~nulls])
+    d = len(want)
+    lo_want, hi_want = (int(want[0]), int(want[-1])) if d else (2**63 - 1, -2**63)
+    for max_values in sorted({0, max(d - 1, 0), d, d + 100}):
+        lo, hi, cnt, values, has_null = lookup.key_domain(max_values)
+        assert (lo, hi, cnt, has_null) == (lo_want, hi_want, d, bool(nulls.any())), max_values
+        if d <= max_values:
+            assert values is not None and values.tolist() == want.tolist(), max_values
+        else:
+            assert values is None, max_values
+    lookup.close()
+    b.close()
+
+
+@pytest.mark.parametrize("mode", ["0", "1", "2", None, "roomy", "narrow"])
+def test_key_domain_under_every_table_layout(ctx, monkeypatch, mode):
+    """The key domain is read off the 16-byte table whatever its layout: mix(key) (mode 0), line-local (1), order-preserving lines (2,
+    the default), without the dense geometry attempt or without the packed / wide slots.  Key sets: dense keys with a small payload (4-byte
+    packed slots under mode 2), strided keys with a wide payload (8-byte packed slots), duplicate keys (position links), and INT64_MIN
+    alone and beside other keys."""
+    monkeypatch.delenv("TGPU_JOIN_HASH", raising=False)
+    if mode == "roomy":
+        monkeypatch.setenv("TGPU_JOIN_NO_DENSE", "1")
+    elif mode == "narrow":
+        monkeypatch.setenv("TGPU_JOIN_NO_WIDE", "1")
+    elif mode is not None:
+        monkeypatch.setenv("TGPU_JOIN_HASH", mode)
+    rng = np.random.default_rng(23)
+    no_nulls = lambda k: np.zeros(len(k), dtype=bool)
+    dense = rng.permutation(np.arange(-5000, 20_000))
+    _check_key_domain(ctx, [Page(Block.bigint(dense), Block.integer((dense % 100).astype(np.int32)))], dense, no_nulls(dense), out=[1])
+    strided = rng.permutation(np.arange(0, 8 * 30_000, 8)) + 10**15
+    _check_key_domain(ctx, [Page(Block.bigint(strided), Block.bigint(rng.integers(-2**62, 2**62, len(strided))))], strided, no_nulls(strided), out=[1])
+    dups = rng.integers(-3000, 3000, 40_000)
+    nulls = rng.random(len(dups)) < 0.02
+    _check_key_domain(ctx, [Page(Block.bigint(dups, nulls), Block.bigint(np.arange(len(dups))))], dups, nulls, out=[1])
+    for keys in ([-2**63], [-2**63, -2**63, 5, 2**63 - 1, -1], np.concatenate([[-2**63], np.arange(-100, 4000)])):
+        keys = np.asarray(keys, dtype=np.int64)
+        _check_key_domain(ctx, [Page(Block.bigint(keys), Block.bigint(np.arange(len(keys))))], keys, no_nulls(keys), out=[1])
+    for make in (Block.integer, Block.smallint, Block.tinyint):              # narrow keys next to their type's minimum
+        narrow = np.concatenate([[-128], rng.integers(-128, 128, 500)])
+        _check_key_domain(ctx, [Page(make(narrow))], narrow, no_nulls(narrow))
 
 
 @pytest.mark.parametrize("mode", ["0", "1", "2", None, "span", "roomy", "narrow", "wide"])

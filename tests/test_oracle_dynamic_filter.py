@@ -43,8 +43,33 @@ def golden_cases():
     return cases
 
 
+def double_bits(values):
+    """raw IEEE bits of DOUBLE values (None = NULL) as a column (values, nulls) of the oracle"""
+    vals = np.array([0.0 if v is None else v for v in values], dtype=np.float64).view(np.int64)
+    nulls = np.array([v is None for v in values])
+    return vals, nulls if nulls.any() else None
+
+
+def double_range(channel, lo, hi, null_allowed=False):
+    return df.Domain(channel, df.RANGE, null_allowed, *np.array([lo, hi], dtype=np.float64).view(np.int64).tolist(), double=True)
+
+
+def double_range_cases():
+    """DOUBLE ranges by value (DoubleType.compare): -0.0 == 0.0, NaN lies in no range, negative bounds order by value, not by bits"""
+    inf, nan = float("inf"), float("nan")
+    neg_nan = -np.float64(nan)
+    return [
+        ("double range: -0.0 == 0.0", [double_range(0, 0.0, 1.0)], 1.0,
+         [[double_bits([-0.0, 0.0, 1.0, -5e-324, 0.5, 1.0000000000000002, None])], [double_bits([0.0, -0.0, 5e-324, -5e-324])]],
+         [[0, 1, 2, 4], [0, 1, 2]]),
+        ("double range: [-0.0, -0.0]", [double_range(0, -0.0, -0.0, True)], 1.0, [[double_bits([0.0, -0.0, 5e-324, None])]], [[0, 1, 3]]),
+        ("double range: NaN lies in no range", [double_range(0, -inf, inf)], 1.0, [[double_bits([nan, inf, -inf, 0.0, neg_nan, 1e308])]], [[1, 2, 3, 5]]),
+        ("double range: negative bounds", [double_range(0, -2.5, -1.0)], 1.0, [[double_bits([-3.0, -2.5, -1.5, -1.0, -0.5, 1.0, -inf])]], [[1, 2, 3]]),
+    ]
+
+
 def test_oracle_reproduces_the_reference_cases():
-    for name, domains, threshold, pages, expected in golden_cases():
+    for name, domains, threshold, pages, expected in golden_cases() + double_range_cases():
         ev = df.DynamicFilterEvaluator(domains, threshold)
         for page, want in zip(pages, expected):
             got = ev.evaluate(page)

@@ -147,6 +147,9 @@ struct DynFilterOp : tgpu_op {
             const bool dbl = col.type == TGPU_FLOAT64;
             if (col.type == TGPU_FLOAT32 && d.kind != TGPU_DOMAIN_ALL && d.kind != TGPU_DOMAIN_NONE)
                 return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "dynamic filter domains over REAL columns stay on the Java filter");
+            // bounds and values are 64-bit: a long DECIMAL value cannot be compared with them
+            if (col.type == TGPU_INT128 && d.kind != TGPU_DOMAIN_ALL && d.kind != TGPU_DOMAIN_NONE)
+                return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "dynamic filter value sets over long DECIMAL columns stay on the Java filter");
             if (col.elem_size() == 0 && d.kind != TGPU_DOMAIN_ALL && d.kind != TGPU_DOMAIN_NONE)
                 return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "dynamic filter value sets over variable-width columns stay on the Java filter");
             if (dbl && d.kind == TGPU_DOMAIN_DISCRETE) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "discrete DOUBLE domains stay on the Java filter");

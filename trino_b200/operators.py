@@ -988,7 +988,14 @@ class ColumnDomain:
 
     @staticmethod
     def range(channel, lo, hi_exclusive, null_allowed=False):
+        """[lo, hi_exclusive) over an integer channel (the bound becomes hi_exclusive - 1); DOUBLE channels take double_range"""
         return ColumnDomain(channel, abi.DOMAIN_RANGE, null_allowed, lo=lo, hi=hi_exclusive - 1)
+
+    @staticmethod
+    def double_range(channel, lo, hi, null_allowed=False):
+        """[lo, hi] over a DOUBLE channel, both bounds inclusive floats (passed as their raw IEEE bits; compared by value)"""
+        lo_bits, hi_bits = np.array([lo, hi], dtype=np.float64).view(np.int64).tolist()
+        return ColumnDomain(channel, abi.DOMAIN_RANGE, null_allowed, lo=lo_bits, hi=hi_bits)
 
 
 class DynamicFilterOperator(Operator):
