@@ -10,14 +10,14 @@ from q6 import INPUT_TYPES, q6_aggregators, q6_program
 from trino_b200 import abi
 
 
-def _selftest(nullable_mask):
+def _selftest(nullable_mask, step=abi.STEP_SINGLE, aggs=None):
     lib = abi.load_library()
     prog = q6_program()
-    aggs = q6_aggregators()
+    aggs = aggs or q6_aggregators()
     fns = (abi.AggFn * len(aggs))()
     for i, a in enumerate(aggs):
         fns[i].function, fns[i].input_channel, fns[i].mask_channel = a.function, a.input_channel, a.mask_channel
-    spec = abi.AggSpec(0, None, abi.STEP_SINGLE, len(aggs), C.cast(fns, C.POINTER(abi.AggFn)), 1, 0, C.pointer(prog.struct))
+    spec = abi.AggSpec(0, None, step, len(aggs), C.cast(fns, C.POINTER(abi.AggFn)), 1, 0, C.pointer(prog.struct))
     types = (C.c_int32 * 7)(*INPUT_TYPES)
     n = C.c_int64()
     buf = C.create_string_buffer(1 << 17)
@@ -56,6 +56,15 @@ def test_global_kernel_has_no_table_and_no_atomics():
         assert word not in src, word
     # register accumulators: every update indexes the accumulator array with a constant at stride 1
     assert re.search(r"acc_update_private\(\d+, acc \+ \d+ \* T, T, ", src)
+
+
+def test_refuses_what_the_operator_refuses():
+    """The hook builds the operator as tgpu_aggregation_create does, so a spec the operator refuses is refused before any source is
+    generated: here Q6's sum(revenue) behind a fused pre-stage on a FINAL step, whose input is accumulator state rather than raw rows
+    (the kernel itself would plan and compile)"""
+    st, _, src = _selftest(0, step=abi.STEP_FINAL, aggs=q6_aggregators()[:1])
+    assert st == abi.ERR_INVALID_ARGUMENT
+    assert src == ""
 
 
 # ---- the keyed kernel (tg_agg_small_jit, HashAggregationOperator's path S) over every argument type ----------------------------------

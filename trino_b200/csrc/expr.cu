@@ -970,6 +970,28 @@ void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last)
     }
 }
 
+void fp_emit_temps(std::string& s, const DProgram& prog)
+{
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(s, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    // high words of the temps that hold a long DECIMAL
+    for (int t = 0; t < TGPU_MAX_TEMPS; t++)
+        if ((prog.long_temps >> t) & 1) fp_appendf(s, "    long long th%d = 0;\n", t);
+    // string functions: the views temps hold and the captured concatenation pieces
+    if (prog.has_strfn) {
+        for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(s, "    StrRef v%d = {nullptr, 0};\n", t);
+        for (int q = 0; q < prog.num_piece_slots; q++) fp_appendf(s, "    StrRef q%d = {nullptr, 0};\n", q);
+    }
+}
+
+void fp_mark_columns(const DProgram& prog, int first, int last, bool* used)
+{
+    for (int i = first; i < last; i++) {
+        const DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
+        for (auto* o : ops)
+            if (o->kind == TGPU_OPND_COLUMN) used[o->index] = true;
+    }
+}
+
 }  // namespace tg
 
 namespace {
@@ -1079,15 +1101,7 @@ static std::string gen_fp_source(const DProgram& prog, const int* elems, int num
         else fp_appendf(loads, " const bool c%dn = false;\n", c);
         if (str_used[c]) fp_appendf(loads, "    const StrRef s%d = tg_str(strs, %d, row);\n", c, prog.str_slot[c]);
     }
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
-    // high words of the temps that hold a long DECIMAL
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++)
-        if ((prog.long_temps >> t) & 1) fp_appendf(temps, "    long long th%d = 0;\n", t);
-    // string functions: the views temps hold and the captured concatenation pieces
-    if (prog.has_strfn) {
-        for (int t = 0; t < TGPU_MAX_TEMPS; t++) fp_appendf(temps, "    StrRef v%d = {nullptr, 0};\n", t);
-        for (int q = 0; q < prog.num_piece_slots; q++) fp_appendf(temps, "    StrRef q%d = {nullptr, 0};\n", q);
-    }
+    fp_emit_temps(temps, prog);
     const bool wide_out = prog.long_temps != 0;
     // value, NULL flag and carried error of the temp behind each computed output column (the only errors a projection raises)
     std::string output_switch = "    for (int c = 0; c < out.count; c++) {\n      long long v = 0; bool isn = true; unsigned int e = 0;\n";
@@ -1719,20 +1733,10 @@ extern "C" int tgpu_jit_selftest_filter_project(const tgpu_expr_program* program
     int32_t max_channel = -1;
     int st = tg::expr_compile(&fake, program, &prog, &max_channel);
     if (st != TGPU_OK) return st;
-    int elems[TGPU_MAX_CHANNELS] = {0};
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        DevColumn col;
-        col.type = channel_types[c];
-        elems[c] = col.elem_size();
-    }
     std::vector<int> pass;
     for (int32_t i = 0; i < program->num_projections; i++)
         if (program->projections[i].kind == 0) pass.push_back(program->projections[i].index);
-    std::string src = gen_fp_source(prog, elems, num_channels, nullable_mask, pass);
-    if (source_out && source_cap > 0) { strncpy(source_out, src.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
-    std::string cubin;
-    st = tg::jit_compile_cubin(&fake, src, &cubin);
-    if (st != TGPU_OK) { if (source_out && source_cap > 0) { strncpy(source_out, fake.err.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; } return st; }
-    *cubin_bytes = (int64_t)cubin.size();
-    return TGPU_OK;
+    return tg::jit_selftest(channel_types, num_channels, [&](const int* elems) {
+        return gen_fp_source(prog, elems, num_channels, nullable_mask, pass);
+    }, cubin_bytes, source_out, source_cap);
 }

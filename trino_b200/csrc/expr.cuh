@@ -441,6 +441,10 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* program, DProgram* out,
 // (temp i's value, NULL flag and carried error bits), which the caller declares
 void fp_appendf(std::string& s, const char* fmt, ...);
 void fp_emit_insns(std::string& s, const DProgram& prog, int first, int last);
+// the declarations of every temp's locals (with the high words of long DECIMAL temps and the views of string functions)
+void fp_emit_temps(std::string& s, const DProgram& prog);
+// used[k] = true for every channel k that instructions [first, last) read as an operand
+void fp_mark_columns(const DProgram& prog, int first, int last, bool* used);
 // fail with the error one set of TG_ERR_BIT_* bits stands for (TGPU_OK when none is set)
 int expr_raise(tgpu_ctx* ctx, int64_t errbits);
 

@@ -1400,28 +1400,6 @@ __global__ void __launch_bounds__(256) agg_skip_kernel(DColumns cols, int64_t n,
 // NVRTC specialisation of path S: straight-line typed code for the row program (filter + projections +
 // key packing + accumulator updates) plugged into agg_small_body<P> of device_lib.cuh.
 // =====================================================================================================
-static void appendf(std::string& s, const char* fmt, ...)
-{
-    char buf[1024];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof(buf), fmt, ap);
-    va_end(ap);
-    s += buf;
-}
-
-static std::string gen_operand(const DOperand& o)
-{
-    char buf[128];
-    switch (o.kind) {
-        case TGPU_OPND_COLUMN: snprintf(buf, sizeof(buf), "Value{c%d, c%dn}", o.index, o.index); break;
-        case TGPU_OPND_TEMP: snprintf(buf, sizeof(buf), "Value{t%d, tn%d}", o.index, o.index); break;
-        case TGPU_OPND_CONST: snprintf(buf, sizeof(buf), "Value{(long long)0x%llxULL, false}", (unsigned long long)o.imm); break;
-        default: snprintf(buf, sizeof(buf), "Value{0, true}"); break;
-    }
-    return buf;
-}
-
 // `elems[c]` = element size of input channel c (0 = not a fixed-width column); bit c of nullable_mask = channel c has a validity bitmap
 // rows in flight per thread of the fused general kernel (TGPU_AGG_G_ROWS: 1, 2, 4 or 8; experiments)
 static int general_rows_per_thread()
@@ -1451,11 +1429,9 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         }
     };
     if (prog) {
+        fp_mark_columns(*prog, 0, prog->num_insns, used);
         for (int i = 0; i < prog->num_insns; i++) {
             const DInsn& in = prog->insns[i];
-            const DOperand* ops[3] = {&in.a, &in.b, &in.c};
-            for (auto* o : ops)
-                if (o->kind == TGPU_OPND_COLUMN) used[o->index] = true;
             bool n;
             switch (in.op) {
                 case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: n = false; break;
@@ -1490,65 +1466,59 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
     if (global && compact == 0) kinds[compact++] = ACC_ROWS;      // (no aggregate at all: one unused counter keeps the kernel well-formed)
     map->compact_count = compact;
 
-    appendf(s, "struct Prog {\n  static constexpr int L = %d, A = %d, R = 4, GR = %d;\n  static constexpr bool VEC = %s, SPECIALS = %s;\n", L, compact, general_rows_per_thread(),
-            vec ? "true" : "false", plan.num_keys == 1 ? "true" : "false");
+    fp_appendf(s, "struct Prog {\n  static constexpr int L = %d, A = %d, R = 4, GR = %d;\n  static constexpr bool VEC = %s, SPECIALS = %s;\n", L, compact, general_rows_per_thread(),
+               vec ? "true" : "false", plan.num_keys == 1 ? "true" : "false");
     s += "  __device__ static __forceinline__ int acc_kind(int a) {\n    switch (a) {\n";
-    for (int a = 0; a < compact; a++) appendf(s, "      case %d: return %d;\n", a, kinds[a]);
+    for (int a = 0; a < compact; a++) fp_appendf(s, "      case %d: return %d;\n", a, kinds[a]);
     s += "      default: return 0;\n    }\n  }\n";
     s += "  struct Regs {\n";
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++)
-        if (used[c]) appendf(s, "    long long c%d; bool c%dn;\n", c, c);
+        if (used[c]) fp_appendf(s, "    long long c%d; bool c%dn;\n", c, c);
     s += "  };\n";
-    for (int i = 0; i < plan.num_srcs; i++) appendf(s, "  long long v%d; bool vn%d;\n", i, i);
+    for (int i = 0; i < plan.num_srcs; i++) fp_appendf(s, "  long long v%d; bool vn%d;\n", i, i);
     // global kernel: the columns the filter reads are loaded first, the others only for rows that passed it (agg_global_body)
     bool early[TGPU_MAX_CHANNELS] = {false};
     const bool has_filter = prog && prog->filter_temp >= 0;
-    if (has_filter)
-        for (int i = 0; i < prog->num_filter_insns; i++) {
-            const DInsn& in = prog->insns[i];
-            const DOperand* ops[3] = {&in.a, &in.b, &in.c};
-            for (auto* o : ops)
-                if (o->kind == TGPU_OPND_COLUMN) early[o->index] = true;
-        }
+    if (has_filter) fp_mark_columns(*prog, 0, prog->num_filter_insns, early);
     for (int c = 0; c < TGPU_MAX_CHANNELS; c++) early[c] = early[c] || !has_filter;
     auto loads = [&](const char* name, const char* name4, int which /* 0 all, 1 early, 2 late */) {
         auto wanted = [&](int c) { return used[c] && (which == 0 || (which == 1) == early[c]); };
         // all global loads of a row, nothing else: the body issues them for R rows back to back
-        appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row, Regs& r) {\n", name);
+        fp_appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row, Regs& r) {\n", name);
         for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
             if (!wanted(c)) continue;
-            appendf(s, "    r.c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
-            if ((nullable_mask >> c) & 1) appendf(s, " r.c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
-            else appendf(s, " r.c%dn = false;\n", c);
+            fp_appendf(s, "    r.c%d = tg_load_elem<%d>(cols.cols[%d].data, row);", c, elems[c], c);
+            if ((nullable_mask >> c) & 1) fp_appendf(s, " r.c%dn = !tg_valid(cols.cols[%d].validity, row);\n", c, c);
+            else fp_appendf(s, " r.c%dn = false;\n", c);
         }
         s += "  }\n";
         // the same for FOUR CONSECUTIVE rows starting at a multiple of 4 (VEC kernels: every column base is 16-byte aligned): one or two
         // 16-byte loads per wide column, one 4-byte load per INT8 column, the four validity bits from one byte
-        appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row0, Regs (&r)[4]) {\n", name4);
+        fp_appendf(s, "  __device__ __forceinline__ void %s(const DColumns& cols, long long row0, Regs (&r)[4]) {\n", name4);
         for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
             if (!wanted(c)) continue;
             switch (elems[c]) {
                 case 8:
-                    appendf(s, "    { const longlong2* p = (const longlong2*)((const char*)cols.cols[%d].data + row0 * 8); longlong2 a = p[0], b = p[1];"
-                               " r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = b.x; r[3].c%d = b.y; }\n", c, c, c, c, c);
+                    fp_appendf(s, "    { const longlong2* p = (const longlong2*)((const char*)cols.cols[%d].data + row0 * 8); longlong2 a = p[0], b = p[1];"
+                                  " r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = b.x; r[3].c%d = b.y; }\n", c, c, c, c, c);
                     break;
                 case 4:
-                    appendf(s, "    { int4 a = *(const int4*)((const char*)cols.cols[%d].data + row0 * 4); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                            c, c, c, c, c);
+                    fp_appendf(s, "    { int4 a = *(const int4*)((const char*)cols.cols[%d].data + row0 * 4); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                               c, c, c, c, c);
                     break;
                 case 2:
-                    appendf(s, "    { short4 a = *(const short4*)((const char*)cols.cols[%d].data + row0 * 2); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                            c, c, c, c, c);
+                    fp_appendf(s, "    { short4 a = *(const short4*)((const char*)cols.cols[%d].data + row0 * 2); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                               c, c, c, c, c);
                     break;
                 default:
-                    appendf(s, "    { char4 a = *(const char4*)((const char*)cols.cols[%d].data + row0); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
-                            c, c, c, c, c);
+                    fp_appendf(s, "    { char4 a = *(const char4*)((const char*)cols.cols[%d].data + row0); r[0].c%d = a.x; r[1].c%d = a.y; r[2].c%d = a.z; r[3].c%d = a.w; }\n",
+                               c, c, c, c, c);
                     break;
             }
             if ((nullable_mask >> c) & 1)
-                appendf(s, "    { const uint8_t* v = cols.cols[%d].validity; unsigned int b = v ? ((unsigned int)v[row0 >> 3] >> (row0 & 7)) : 0xfu;"
-                           " r[0].c%dn = !(b & 1); r[1].c%dn = !(b & 2); r[2].c%dn = !(b & 4); r[3].c%dn = !(b & 8); }\n", c, c, c, c, c);
-            else appendf(s, "    r[0].c%dn = r[1].c%dn = r[2].c%dn = r[3].c%dn = false;\n", c, c, c, c);
+                fp_appendf(s, "    { const uint8_t* v = cols.cols[%d].validity; unsigned int b = v ? ((unsigned int)v[row0 >> 3] >> (row0 & 7)) : 0xfu;"
+                              " r[0].c%dn = !(b & 1); r[1].c%dn = !(b & 2); r[2].c%dn = !(b & 4); r[3].c%dn = !(b & 8); }\n", c, c, c, c, c);
+            else fp_appendf(s, "    r[0].c%dn = r[1].c%dn = r[2].c%dn = r[3].c%dn = false;\n", c, c, c, c);
         }
         s += "  }\n";
     };
@@ -1557,39 +1527,19 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         loads("load_late", "load4_late", 2);
     }
     else loads("load", "load4", 0);
-    auto opnd_error = [](const DOperand& o) { return o.kind == TGPU_OPND_TEMP ? "te" + std::to_string(o.index) : std::string("0u"); };
-    auto emit_insn = [&](const DInsn& in) {
-        if (in.op == TGPU_EX_IN) {
-            int li = (int)in.b.imm;
-            appendf(s, "    { Value a = %s; bool hit = false;\n", gen_operand(in.a).c_str());
-            for (int k = 0; k < prog->in_count[li]; k++) {
-                unsigned long long c = (unsigned long long)prog->in_values[prog->in_offset[li] + k];
-                if (in.vtype == TGPU_V_DOUBLE) appendf(s, "      hit |= __longlong_as_double(a.bits) == __longlong_as_double((long long)0x%llxULL);\n", c);
-                else appendf(s, "      hit |= a.bits == (long long)0x%llxULL;\n", c);
-            }
-            appendf(s, "      t%d = hit ? 1 : 0; tn%d = a.is_null; te%d = %s; }\n", in.dst, in.dst, in.dst, opnd_error(in.a).c_str());
-        }
-        else {
-            // operands are read into locals first: dst may be one of them, and vm_error needs their values
-            appendf(s, "    { Value a = %s, b = %s, c = %s; unsigned int e = 0; Value x = vm_apply(%d, %d, a, b, c, &e);\n", gen_operand(in.a).c_str(),
-                    gen_operand(in.b).c_str(), gen_operand(in.c).c_str(), in.op, in.vtype);
-            appendf(s, "      e = vm_error(%d, %d, a, %s, b, %s, c, %s, e); t%d = x.bits; tn%d = x.is_null; te%d = e; }\n", in.op, in.vtype,
-                    opnd_error(in.a).c_str(), opnd_error(in.b).c_str(), opnd_error(in.c).c_str(), in.dst, in.dst, in.dst);
-        }
-    };
+    // (fp_emit_insns writes the program over these locals; it has no VARCHAR or DECIMAL instructions: build_agg_op refuses them)
     auto emit_columns_and_temps = [&](bool only_early) {
         for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++)
-            if (used[c] && (!only_early || early[c])) appendf(s, "    const long long c%d = r.c%d; const bool c%dn = r.c%dn;\n", c, c, c, c);
-        if (prog)
-            for (int t = 0; t < TGPU_MAX_TEMPS; t++) appendf(s, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+            if (used[c] && (!only_early || early[c])) fp_appendf(s, "    const long long c%d = r.c%d; const bool c%dn = r.c%dn;\n", c, c, c, c);
+        if (prog) fp_emit_temps(s, *prog);
     };
     if (global) {
         // the filter alone, over the early columns (its errors count on every row); row() evaluates it again for the rows that passed
         s += "  __device__ __forceinline__ bool filter(const Regs& r, unsigned int* err) {\n";
         if (has_filter) {
             emit_columns_and_temps(true);
-            for (int i = 0; i < prog->num_filter_insns; i++) emit_insn(prog->insns[i]);
-            appendf(s, "    *err |= te%d;\n    return !(tn%d || t%d == 0);\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
+            fp_emit_insns(s, *prog, 0, prog->num_filter_insns);
+            fp_appendf(s, "    *err |= te%d;\n    return !(tn%d || t%d == 0);\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
         }
         else s += "    return true;\n";
         s += "  }\n";
@@ -1598,24 +1548,20 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
     emit_columns_and_temps(false);
     if (prog) {
         // the filter's errors count on every row, a projection's only when the aggregation reads it (see vm_error)
-        auto filter_check = [&]() {
-            appendf(s, "    *err |= te%d;\n    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
-        };
-        for (int i = 0; i < prog->num_insns; i++) {
-            if (i == prog->num_filter_insns && prog->filter_temp >= 0) filter_check();
-            emit_insn(prog->insns[i]);
-        }
-        if (prog->num_filter_insns == prog->num_insns && prog->filter_temp >= 0) filter_check();
+        fp_emit_insns(s, *prog, 0, prog->num_filter_insns);
+        if (prog->filter_temp >= 0)
+            fp_appendf(s, "    *err |= te%d;\n    if (tn%d || t%d == 0) return false;\n", prog->filter_temp, prog->filter_temp, prog->filter_temp);
+        fp_emit_insns(s, *prog, prog->num_filter_insns, prog->num_insns);
         for (int i = 0; i < plan.num_srcs; i++)
-            if (plan.srcs[i].is_temp) appendf(s, "    *err |= te%d;\n", plan.srcs[i].index);
+            if (plan.srcs[i].is_temp) fp_appendf(s, "    *err |= te%d;\n", plan.srcs[i].index);
     }
     for (int i = 0; i < plan.num_srcs; i++) {
-        if (plan.srcs[i].is_temp) appendf(s, "    v%d = t%d; vn%d = tn%d;\n", i, plan.srcs[i].index, i, plan.srcs[i].index);
-        else appendf(s, "    v%d = c%d; vn%d = c%dn;\n", i, plan.srcs[i].index, i, plan.srcs[i].index);
+        if (plan.srcs[i].is_temp) fp_appendf(s, "    v%d = t%d; vn%d = tn%d;\n", i, plan.srcs[i].index, i, plan.srcs[i].index);
+        else fp_appendf(s, "    v%d = c%d; vn%d = c%dn;\n", i, plan.srcs[i].index, i, plan.srcs[i].index);
     }
     if (plan.num_keys == 1) {
         int k = plan.key_src[0];
-        appendf(s, "    if (vn%d) { *special = 0; return true; }\n    unsigned long long u = (unsigned long long)v%d;\n", k, k);
+        fp_appendf(s, "    if (vn%d) { *special = 0; return true; }\n    unsigned long long u = (unsigned long long)v%d;\n", k, k);
         if (plan.key_is_double[0])
             s += "    if ((u << 1) == 0) u = 0;\n    if ((u & 0x7FFFFFFFFFFFFFFFULL) > 0x7FF0000000000000ULL) u = 0x7FF8000000000000ULL;\n";
         s += "    if (u == TGD_EMPTY_KEY) { *special = 1; return true; }\n    *pk = u;\n";
@@ -1625,7 +1571,7 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         int shift = 0;
         for (int kk = 0; kk < plan.num_keys; kk++) {
             int src = plan.key_src[kk], bits = plan.key_bits[kk];
-            appendf(s, "    k |= (vn%d ? 1ULL : ((((unsigned long long)v%d) & 0x%llxULL) << 1)) << %d;\n", src, src, (1ULL << bits) - 1, shift);
+            fp_appendf(s, "    k |= (vn%d ? 1ULL : ((((unsigned long long)v%d) & 0x%llxULL) << 1)) << %d;\n", src, src, (1ULL << bits) - 1, shift);
             shift += bits + 1;
         }
         s += "    *pk = k;\n";
@@ -1639,15 +1585,15 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         std::string cond = "true";
         if (d.mask >= 0) { char b[64]; snprintf(b, sizeof(b), "(!vn%d && v%d != 0)", d.mask, d.mask); cond = b; }
         if (d.kind != ACC_ROWS && src_nullable(d.src)) { char b[64]; snprintf(b, sizeof(b), " && !vn%d", d.src); cond += b; }
-        if (d.kind == ACC_ROWS) appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, 0);\n", cond.c_str(), d.kind, map->of_plan[a]);
-        else appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, v%d);\n", cond.c_str(), d.kind, map->of_plan[a], d.src);
+        if (d.kind == ACC_ROWS) fp_appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, 0);\n", cond.c_str(), d.kind, map->of_plan[a]);
+        else fp_appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, v%d);\n", cond.c_str(), d.kind, map->of_plan[a], d.src);
     }
     s += "  }\n";
     if (global) {
         // AggregationOperator: the one-group kernel alone (agg_global_body), no key table and no record reductions
         s += "};\n";
-        appendf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) tg_agg_global_jit(DColumns cols, long long n, unsigned long long* part, unsigned int* err) {\n",
-                S_THREADS, min_blocks);
+        fp_appendf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) tg_agg_global_jit(DColumns cols, long long n, unsigned long long* part, unsigned int* err) {\n",
+                   S_THREADS, min_blocks);
         s += "  Prog p;\n  agg_global_body(p, cols, n, part, err);\n}\n";
         return s;
     }
@@ -1661,33 +1607,33 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
         if (d.mask >= 0) { char b[64]; snprintf(b, sizeof(b), "(!vn%d && v%d != 0)", d.mask, d.mask); cond = b; }
         const bool nullable = d.src >= 0 && src_nullable(d.src);
         if (d.kind == ACC_NONNULL) {
-            if (nullable) appendf(s, "    if (%s && vn%d) atomicAdd(acc + %d, 1ULL);\n", cond.c_str(), d.src, a);
+            if (nullable) fp_appendf(s, "    if (%s && vn%d) atomicAdd(acc + %d, 1ULL);\n", cond.c_str(), d.src, a);
             continue;
         }
         if (d.kind != ACC_ROWS && nullable) { char b[64]; snprintf(b, sizeof(b), " && !vn%d", d.src); cond += b; }
         switch (d.kind) {
-            case ACC_ROWS: appendf(s, "    if (%s) atomicAdd(acc + %d, 1ULL);\n", cond.c_str(), a); break;
-            case ACC_SUM_F64: appendf(s, "    if (%s) atomicAdd((double*)(acc + %d), __longlong_as_double(v%d));\n", cond.c_str(), a, d.src); break;
-            case ACC_SUM_F64_FROM_I64: appendf(s, "    if (%s) atomicAdd((double*)(acc + %d), (double)v%d);\n", cond.c_str(), a, d.src); break;
+            case ACC_ROWS: fp_appendf(s, "    if (%s) atomicAdd(acc + %d, 1ULL);\n", cond.c_str(), a); break;
+            case ACC_SUM_F64: fp_appendf(s, "    if (%s) atomicAdd((double*)(acc + %d), __longlong_as_double(v%d));\n", cond.c_str(), a, d.src); break;
+            case ACC_SUM_F64_FROM_I64: fp_appendf(s, "    if (%s) atomicAdd((double*)(acc + %d), (double)v%d);\n", cond.c_str(), a, d.src); break;
             case ACC_SUM_I64_LO:
                 // (values that fit 32 unsigned bits have nothing to add to the high word: one reduction less per row)
-                appendf(s, "    if (%s) { atomicAdd(acc + %d, (unsigned long long)v%d & 0xFFFFFFFFULL); if ((v%d >> 32) != 0) atomicAdd(acc + %d, (unsigned long long)(v%d >> 32)); }\n",
-                        cond.c_str(), a, d.src, d.src, a + 1, d.src);
+                fp_appendf(s, "    if (%s) { atomicAdd(acc + %d, (unsigned long long)v%d & 0xFFFFFFFFULL); if ((v%d >> 32) != 0) atomicAdd(acc + %d, (unsigned long long)(v%d >> 32)); }\n",
+                           cond.c_str(), a, d.src, d.src, a + 1, d.src);
                 break;
-            case ACC_MIN_F64: appendf(s, "    if (%s) atomicMin(acc + %d, f64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
-            case ACC_MAX_F64: appendf(s, "    if (%s) atomicMax(acc + %d, f64_order_key_max(v%d));\n", cond.c_str(), a, d.src); break;
-            case ACC_MIN_I64: appendf(s, "    if (%s) atomicMin(acc + %d, i64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
-            case ACC_MAX_I64: appendf(s, "    if (%s) atomicMax(acc + %d, i64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
+            case ACC_MIN_F64: fp_appendf(s, "    if (%s) atomicMin(acc + %d, f64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
+            case ACC_MAX_F64: fp_appendf(s, "    if (%s) atomicMax(acc + %d, f64_order_key_max(v%d));\n", cond.c_str(), a, d.src); break;
+            case ACC_MIN_I64: fp_appendf(s, "    if (%s) atomicMin(acc + %d, i64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
+            case ACC_MAX_I64: fp_appendf(s, "    if (%s) atomicMax(acc + %d, i64_order_key(v%d));\n", cond.c_str(), a, d.src); break;
             default: break;
         }
     }
     s += "  }\n};\n";
-    appendf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) tg_agg_small_jit(DColumns cols, long long n, SmallOut out) {\n", S_THREADS, min_blocks);
+    fp_appendf(s, "extern \"C\" __global__ void __launch_bounds__(%d, %d) tg_agg_small_jit(DColumns cols, long long n, SmallOut out) {\n", S_THREADS, min_blocks);
     s += "  extern __shared__ unsigned long long smem_u64[];\n  Prog p;\n  agg_small_body(p, cols, n, out, smem_u64);\n}\n";
     {
         const char* e = getenv("TGPU_AGG_G_MINB");
-        appendf(s, "extern \"C\" __global__ void __launch_bounds__(256, %d) tg_agg_general_jit(DColumns cols, long long n, const int* rows, long long first, const int* stamp_rows,\n",
-                e ? atoi(e) : 4);
+        fp_appendf(s, "extern \"C\" __global__ void __launch_bounds__(256, %d) tg_agg_general_jit(DColumns cols, long long n, const int* rows, long long first, const int* stamp_rows,\n",
+                   e ? atoi(e) : 4);
     }
     s += ""
          "    long long page_base, unsigned long long* recs, long long cap, int W, int* tickets, int budget_per_way, int* deferred, unsigned int* err_out) {\n"
@@ -2292,21 +2238,13 @@ struct AggOp : tgpu_op {
         // one small readback per page: overflow flag + error bits, then the group count
         int64_t word = 0;
         TG_TRY(tg_read_i64(ctx, d_overflow, &word));
-        if ((uint32_t)(word >> 32)) TG_TRY(raise((uint32_t)(word >> 32)));
+        if ((uint32_t)(word >> 32)) TG_TRY(expr_raise(ctx, (uint32_t)(word >> 32)));
         *overflowed = (word & 0xFFFFFFFFLL) != 0;
         if (!*overflowed) {
             int64_t cnt = 0;
             TG_TRY(tg_read_i64(ctx, st_count.p, &cnt));
             group_count = (int32_t)(cnt & 0xFFFFFFFFLL);
         }
-        return TGPU_OK;
-    }
-
-    int raise(uint32_t errbits)
-    {
-        if (errbits & TG_ERR_BIT_DIV_ZERO) return tg_fail(ctx, TGPU_ERR_DIVISION_BY_ZERO, "Division by zero");
-        if (errbits & TG_ERR_BIT_OVERFLOW) return tg_fail(ctx, TGPU_ERR_NUMERIC_VALUE_OUT_OF_RANGE, "bigint arithmetic overflow");
-        if (errbits & TG_ERR_BIT_INVALID_CAST) return tg_fail(ctx, TGPU_ERR_INVALID_CAST_ARGUMENT, "Unable to cast double to bigint");
         return TGPU_OK;
     }
 
@@ -2579,7 +2517,7 @@ struct AggOp : tgpu_op {
                 for (int w = 0; w < WAYS; w++) f_used += counters[w];
                 f_specials += counters[WAYS + 1];
                 left = counters[WAYS];
-                TG_TRY(raise((uint32_t)counters[WAYS + 2]));
+                TG_TRY(expr_raise(ctx, (uint32_t)counters[WAYS + 2]));
             }
             else {
                 f_used += counters[0];
@@ -2852,7 +2790,7 @@ struct AggOp : tgpu_op {
         TG_LAUNCH(ctx, agg_global_fold_kernel, 1, 256, 0, plan, part, grid, map.compact_count, map, state());
         int64_t word = 0;
         TG_TRY(tg_read_i64(ctx, d_flags, &word));
-        return raise((uint32_t)(word >> 32));
+        return expr_raise(ctx, (uint32_t)(word >> 32));
     }
 
     // ---- Operator protocol --------------------------------------------------------------------------
@@ -3292,7 +3230,7 @@ struct AggOp : tgpu_op {
         TG_CUDA(ctx, cudaMemcpyAsync(h_any.data(), anyflags.p, outp.cols.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
         int64_t errw = 0;
         TG_TRY(tg_read_i64(ctx, d_err, &errw));
-        TG_TRY(raise((uint32_t)(errw & 0xFFFFFFFFLL)));
+        TG_TRY(expr_raise(ctx, (uint32_t)(errw & 0xFFFFFFFFLL)));
         for (size_t c = 0; c < outp.cols.size(); c++) {
             if (!h_any[c]) continue;
             outp.cols[c].own_validity = bitmaps[c];
@@ -3443,7 +3381,8 @@ struct AggOp : tgpu_op {
     bool is_finished() override { return finished && next_out >= pending.size(); }
 };
 
-int build_agg_op(tgpu_ctx* ctx, const tgpu_agg_spec* spec, AggOp** out)
+// the operator of a spec, host side only (tgpu_jit_selftest_agg builds it without a device); the creators then call upload_pre
+int build_agg_op(tgpu_ctx* ctx, const tgpu_agg_spec* spec, std::unique_ptr<AggOp>* out)
 {
     if (spec->num_keys < 0 || spec->num_aggs < 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "negative counts in aggregation spec");
     if (spec->step < TGPU_STEP_SINGLE || spec->step > TGPU_STEP_INTERMEDIATE) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "bad aggregation step");
@@ -3482,11 +3421,19 @@ int build_agg_op(tgpu_ctx* ctx, const tgpu_agg_spec* spec, AggOp** out)
             op->pre_in_values.emplace_back(spec->pre->in_lists[i].values, spec->pre->in_lists[i].values + spec->pre->in_lists[i].count);
         op->pre_filter_temp = spec->pre->filter_temp;
         op->pre_num_filter_insns = spec->pre->num_filter_insns;
-        TG_TRY(op->d_prog.alloc(ctx, sizeof(DProgram)));
-        TG_CUDA(ctx, cudaMemcpyAsync(op->d_prog.p, &op->host_prog, sizeof(DProgram), cudaMemcpyHostToDevice, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
-    *out = op.release();
+    *out = std::move(op);
+    return TGPU_OK;
+}
+
+// the device copy of the fused pre-stage program, which the interpreter kernels read
+int upload_pre(AggOp* op)
+{
+    if (!op->has_pre) return TGPU_OK;
+    tgpu_ctx* ctx = op->ctx;
+    TG_TRY(op->d_prog.alloc(ctx, sizeof(DProgram)));
+    TG_CUDA(ctx, cudaMemcpyAsync(op->d_prog.p, &op->host_prog, sizeof(DProgram), cudaMemcpyHostToDevice, ctx->stream));
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return TGPU_OK;
 }
 
@@ -3496,9 +3443,10 @@ extern "C" int tgpu_agg_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec, tgpu_op
 {
     if (!ctx || !spec || !out) return TGPU_ERR_INVALID_ARGUMENT;
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    AggOp* op = nullptr;
+    std::unique_ptr<AggOp> op;
     TG_TRY(build_agg_op(ctx, spec, &op));
-    *out = op;
+    TG_TRY(upload_pre(op.get()));
+    *out = op.release();
     return TGPU_OK;
 }
 
@@ -3514,9 +3462,9 @@ extern "C" int tgpu_aggregation_create(tgpu_ctx* ctx, const tgpu_agg_spec* spec,
     if (spec->num_input_channels < 0 || (spec->num_input_channels > 0 && !spec->input_channel_types))
         return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "AggregationOperator needs input_channel_types: they shape the output row when no page arrives");
     TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    AggOp* raw = nullptr;
-    TG_TRY(build_agg_op(ctx, spec, &raw));
-    std::unique_ptr<AggOp> op(raw);
+    std::unique_ptr<AggOp> op;
+    TG_TRY(build_agg_op(ctx, spec, &op));
+    TG_TRY(upload_pre(op.get()));
     op->global = true;
     TG_TRY(op->start_global());
     *out = op.release();
@@ -3588,10 +3536,10 @@ extern "C" int tgpu_groupby_hash_create(tgpu_ctx* ctx, int32_t num_keys, const i
     spec.key_channels = key_channels;
     spec.step = TGPU_STEP_SINGLE;
     spec.expected_groups = expected_groups;
-    AggOp* op = nullptr;
+    std::unique_ptr<AggOp> op;
     TG_TRY(build_agg_op(ctx, &spec, &op));
     op->gids_only = true;
-    *out = op;
+    *out = op.release();
     return TGPU_OK;
 }
 
@@ -3629,29 +3577,13 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
 {
     if (!spec || !channel_types || !cubin_bytes) return TGPU_ERR_INVALID_ARGUMENT;
     tgpu_ctx fake;
-    AggOp* op = nullptr;
-    {
-        // build_agg_op touches the device only when a pre-program has to be uploaded: mimic it on the host
-        std::unique_ptr<AggOp> o(new AggOp(&fake));
-        o->key_channels.assign(spec->key_channels, spec->key_channels + spec->num_keys);
-        o->fns.assign(spec->aggs, spec->aggs + spec->num_aggs);
-        o->step = spec->step;
-        o->global = spec->num_keys == 0;        // tgpu_aggregation_create's operator: the one-group kernel
-        if (spec->pre) {
-            o->has_pre = true;
-            int st = tg::expr_compile(&fake, spec->pre, &o->host_prog, &o->prog_max_channel);
-            if (st != TGPU_OK) return st;
-            if (tg::expr_uses_strings(o->host_prog)) return TGPU_ERR_NOT_SUPPORTED;
-            if (tg::expr_uses_decimals(o->host_prog)) return TGPU_ERR_NOT_SUPPORTED;
-            o->projections.assign(spec->pre->projections, spec->pre->projections + spec->pre->num_projections);
-        }
-        op = o.release();
-    }
-    std::unique_ptr<AggOp> guard(op);
+    std::unique_ptr<AggOp> op;
+    int st = build_agg_op(&fake, spec, &op);
+    if (st != TGPU_OK) return st;
+    op->global = spec->num_keys == 0;        // tgpu_aggregation_create's operator: the one-group kernel
     DevPage in;
     in.rows = 0;
     in.cols.resize(num_channels);
-    int elems[TGPU_MAX_CHANNELS] = {0};
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) in.cols[c].type = channel_types[c];
     op->key_dicts.resize(op->key_channels.size());
     for (size_t k = 0; k < op->key_channels.size(); k++) {
@@ -3661,17 +3593,14 @@ extern "C" int tgpu_jit_selftest_agg(const tgpu_agg_spec* spec, const int32_t* c
             in.cols[ch].type = TGPU_INT32;
         }
     }
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) elems[c] = in.cols[c].elem_size();
-    int st = op->make_plan(in);
+    st = op->make_plan(in);
     if (st != TGPU_OK) return st;
+    std::vector<int32_t> types;
+    for (const DevColumn& col : in.cols) types.push_back(col.type);
     AccMap map;
     // (TGPU_JIT_SELFTEST_VEC: the variant with the four-consecutive-rows loader, as launched for 16-byte aligned columns)
-    std::string src = gen_agg_small_source(op->plan, op->has_pre ? &op->host_prog : nullptr, elems, num_channels, 4, op->global ? GLOBAL_MIN_BLOCKS : 2,
-                                           nullable_mask, &map, getenv("TGPU_JIT_SELFTEST_VEC") != nullptr, op->global);
-    if (source_out && source_cap > 0) { strncpy(source_out, src.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
-    std::string cubin;
-    st = tg::jit_compile_cubin(&fake, src, &cubin);
-    if (st != TGPU_OK) { if (source_out && source_cap > 0) { strncpy(source_out, fake.err.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; } return st; }
-    *cubin_bytes = (int64_t)cubin.size();
-    return TGPU_OK;
+    return tg::jit_selftest(types.data(), num_channels, [&](const int* elems) {
+        return gen_agg_small_source(op->plan, op->has_pre ? &op->host_prog : nullptr, elems, num_channels, 4, op->global ? GLOBAL_MIN_BLOCKS : 2, nullable_mask,
+                                    &map, getenv("TGPU_JIT_SELFTEST_VEC") != nullptr, op->global);
+    }, cubin_bytes, source_out, source_cap);
 }

@@ -123,6 +123,28 @@ int jit_compile_cubin(tgpu_ctx* ctx, const std::string& body, std::string* cubin
     return TGPU_OK;
 }
 
+int jit_selftest(const int32_t* channel_types, int32_t num_channels, const std::function<std::string(const int* elems)>& gen, int64_t* cubin_bytes,
+                 char* source_out, int64_t source_cap)
+{
+    int elems[TGPU_MAX_CHANNELS] = {0};
+    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
+        DevColumn col;
+        col.type = channel_types[c];
+        elems[c] = col.elem_size();
+    }
+    auto copy_out = [&](const std::string& text) {
+        if (source_out && source_cap > 0) { strncpy(source_out, text.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
+    };
+    const std::string src = gen(elems);
+    copy_out(src);
+    tgpu_ctx host;
+    std::string cubin;
+    const int st = jit_compile_cubin(&host, src, &cubin);
+    if (st != TGPU_OK) { copy_out(host.err); return st; }
+    *cubin_bytes = (int64_t)cubin.size();
+    return TGPU_OK;
+}
+
 int jit_get_function(tgpu_ctx* ctx, const std::string& body, const char* kernel_name, void** fn_out)
 {
     std::string key = std::to_string(ctx->device) + "|" + kernel_name + "|" + body;

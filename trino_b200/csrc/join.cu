@@ -1482,11 +1482,7 @@ std::string gen_join_filter_source(const DProgram& prog, int nb, const int* elem
 {
     std::string s, loads, temps;
     bool used[TGPU_MAX_CHANNELS] = {false};
-    for (int i = 0; i < prog.num_filter_insns; i++) {
-        const tg::DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
-        for (auto* o : ops)
-            if (o->kind == TGPU_OPND_COLUMN) used[o->index] = true;
-    }
+    tg::fp_mark_columns(prog, 0, prog.num_filter_insns, used);
     for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
         if (!used[c]) continue;
         const char* row = c < nb ? "b" : "p";
@@ -1494,7 +1490,7 @@ std::string gen_join_filter_source(const DProgram& prog, int nb, const int* elem
         if ((nullable_mask >> c) & 1) tg::fp_appendf(loads, " const bool c%dn = !tg_valid(cols.cols[%d].validity, %s);\n", c, c, row);
         else tg::fp_appendf(loads, " const bool c%dn = false;\n", c);
     }
-    for (int t = 0; t < TGPU_MAX_TEMPS; t++) tg::fp_appendf(temps, "    long long t%d = 0; bool tn%d = true; unsigned int te%d = 0;\n", t, t, t);
+    tg::fp_emit_temps(temps, prog);
     const int ft = prog.filter_temp;
     s += "struct JFProg {\n";
     s += "  static __device__ __forceinline__ bool eval(const DColumns& cols, long long p, long long b, unsigned int* errp) {\n";
@@ -2961,22 +2957,11 @@ extern "C" int tgpu_jit_selftest_join_filter(const tgpu_expr_program* program, i
     DProgram prog;
     int st = join_filter_compile(&fake, program, num_build_channels, &prog);
     if (st != TGPU_OK) return st;
-    for (int i = 0; i < prog.num_filter_insns; i++) {
-        const tg::DOperand* ops[3] = {&prog.insns[i].a, &prog.insns[i].b, &prog.insns[i].c};
-        for (auto* o : ops)
-            if (o->kind == TGPU_OPND_COLUMN && o->index >= num_channels) return TGPU_ERR_INVALID_ARGUMENT;     // outside the layout
-    }
-    int elems[TGPU_MAX_CHANNELS] = {0};
-    for (int c = 0; c < num_channels && c < TGPU_MAX_CHANNELS; c++) {
-        DevColumn col;
-        col.type = channel_types[c];
-        elems[c] = col.elem_size();
-    }
-    std::string src = gen_join_filter_source(prog, num_build_channels, elems, std::min<int32_t>(num_channels, TGPU_MAX_CHANNELS), nullable_mask);
-    if (source_out && source_cap > 0) { strncpy(source_out, src.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; }
-    std::string cubin;
-    st = tg::jit_compile_cubin(&fake, src, &cubin);
-    if (st != TGPU_OK) { if (source_out && source_cap > 0) { strncpy(source_out, fake.err.c_str(), (size_t)source_cap - 1); source_out[source_cap - 1] = 0; } return st; }
-    *cubin_bytes = (int64_t)cubin.size();
-    return TGPU_OK;
+    bool used[TGPU_MAX_CHANNELS] = {false};
+    tg::fp_mark_columns(prog, 0, prog.num_filter_insns, used);
+    for (int c = num_channels; c < TGPU_MAX_CHANNELS; c++)
+        if (used[c]) return TGPU_ERR_INVALID_ARGUMENT;     // outside the layout
+    return tg::jit_selftest(channel_types, num_channels, [&](const int* elems) {
+        return gen_join_filter_source(prog, num_build_channels, elems, std::min<int32_t>(num_channels, TGPU_MAX_CHANNELS), nullable_mask);
+    }, cubin_bytes, source_out, source_cap);
 }
