@@ -163,9 +163,30 @@ typedef enum tgpu_expr_op {
     TGPU_EX_SUBSTR = 51,           /* substr(a, b) / substr(a, b, c): b, c BIGINT, c TGPU_OPND_NONE for the two-argument form
                                       (:284-320, :331-378): VARCHAR                                                                */
     TGPU_EX_LTRIM = 52, TGPU_EX_RTRIM = 53, TGPU_EX_TRIM = 54, /* one-argument whitespace trims (:484-527): VARCHAR               */
-    TGPU_EX_CONCAT = 55            /* a || b (ConcatFunction.java:78-95): VARCHAR.  Lower concat(x1, ..., xn) to a left-deep chain of
+    TGPU_EX_CONCAT = 55,           /* a || b (ConcatFunction.java:78-95): VARCHAR.  Lower concat(x1, ..., xn) to a left-deep chain of
                                       binary CONCATs: the same value and the same error                                            */
+    /* conditionals (see the note below the enum).  vtype BIGINT, DOUBLE, BOOLEAN or DECIMAL; VARCHAR answers NOT_SUPPORTED at create */
+    TGPU_EX_IF = 60,               /* a ? b : c.  The one opcode whose vtype is NOT operand a's type: a is BOOLEAN; b, c and the result
+                                      have vtype.  c may be TGPU_OPND_NULL (CASE without ELSE).  Value: b when a is non-NULL and TRUE,
+                                      otherwise c (with c's NULL flag).  Error: a's; else b's when a is TRUE, otherwise c's
+                                      (IfCodeGenerator.java:47-62)                                                                 */
+    TGPU_EX_COALESCE = 61          /* a if a is non-NULL, otherwise b; a, b and the result have vtype.  Error: a's; else none when a is
+                                      non-NULL, otherwise b's (CoalesceCodeGenerator.java:45-75)                                    */
 } tgpu_expr_op;
+
+/* Conditionals.  Every operand of IF and COALESCE is evaluated on every row and one is selected; only the errors of the operand the
+ * reference would have evaluated are carried, so a branch it skips raises nothing.  For DECIMAL the signature's b, c (COALESCE: a, b) and
+ * result must be one type (the planner has already coerced the branches to the result type), else INVALID_ARGUMENT; a condition that is
+ * not BOOLEAN is INVALID_ARGUMENT too (a temp at create; a channel at add_input, which must be TGPU_INT8 whatever the vtype).  Only FilterAndProject and the fused aggregation pre-stage evaluate them; join filters answer
+ * NOT_SUPPORTED.  The special forms lower onto the two opcodes (SqlToRowExpressionTranslator.java:280-400):
+ *   searched CASE WHEN c1 THEN r1 ... ELSE e END, IF(c, r[, e]):  the right-deep chain IF(c1, r1, IF(c2, r2, ... e)), as visitCase builds
+ *   simple CASE v WHEN w1 THEN r1 ... ELSE e END:  t = v; IF(EQ(t, w1), r1, IF(EQ(t, w2), r2, ... e)) with t the FIRST operand of each
+ *       EQ.  The call rule (operands' errors in order, stopping at the first NULL operand) then gives SwitchCodeGenerator.java:77-169
+ *       exactly: v's error comes first, and a NULL v evaluates no w (every EQ is NULL without reading w's error) and falls to ELSE.
+ *   COALESCE(a1, ..., an):  COALESCE(a1, COALESCE(a2, ... an)): the arguments' errors left to right up to the first non-NULL one.
+ *   NULLIF(a, b):  t = a; IF(EQ(cast(t), cast(b)), NULL, t), the casts to the comparison's common type.  By the same call rule a NULL a
+ *       stops the EQ before b, so b's error is not raised, and the result is t, NULL (NullIfCodeGenerator.java:62-105); otherwise the
+ *       EQ carries a's, then b's error; equal gives NULL, and NULL or not equal the uncast a. */
 
 /* TGPU_V_VARCHAR: =, <>, <, <=, >, >=, BETWEEN, IN, IS [NOT] NULL and LIKE read it and give BOOLEAN; LENGTH gives BIGINT; SUBSTR, the
  * trims and CONCAT give VARCHAR.  A VARCHAR operand is a TGPU_OPND_COLUMN naming a TGPU_UTF8 channel (the bytes between offsets[i]

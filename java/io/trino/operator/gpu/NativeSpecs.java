@@ -86,6 +86,17 @@ public final class NativeSpecs
     public static final int EX_TRIM = 54;
     public static final int EX_CONCAT = 55;
     public static final int MAX_CONCAT_PIECES = 8;
+    // Conditional special forms (SpecialForm IF, SWITCH / WHEN, COALESCE, NULL_IF of SqlToRowExpressionTranslator) lower onto two opcodes
+    // whose vtype is the result type (BIGINT, DOUBLE, BOOLEAN or DECIMAL; a VARCHAR result keeps the Java operator): EX_IF(a, b, c) is
+    // a ? b : c with a BOOLEAN condition (c TGPU_OPND_NULL for a CASE without ELSE), EX_COALESCE(a, b) the first non-NULL operand.
+    //   IF(c, r, e) and a searched CASE: the right-deep chain IF(c1, r1, IF(c2, r2, ... e)).
+    //   SWITCH(v, WHEN(w1, r1), ..., e): v into a temp t, then IF(EQ(t, w1), r1, IF(EQ(t, w2), r2, ... e)), t the FIRST operand of each
+    //   EQ, so that v's error comes first and a NULL v reaches e without any w's error.
+    //   COALESCE(a1, ..., an): COALESCE(a1, COALESCE(a2, ... an)).
+    //   NULL_IF(a, b): a into a temp t, then IF(EQ(cast(t), cast(b)), NULL, t) with the casts of the resolved EQUAL's argument type.
+    // For DECIMAL the signature's selected operands and result are the one (coerced) result type.  Join filters keep the Java operator.
+    public static final int EX_IF = 60;
+    public static final int EX_COALESCE = 61;
 
     /** the opcode of a one-call string function (by its resolved name and argument count), or -1 when it keeps the Java operator */
     public static int stringFunctionOpcode(String name, int arity)

@@ -30,6 +30,8 @@ EX_CAST_TO_DECIMAL, EX_CAST_DECIMAL_TO_BIGINT, EX_CAST_DECIMAL_TO_DOUBLE = 32, 3
 # string functions over a VARCHAR operand a: LENGTH gives BIGINT, the others VARCHAR; SUBSTR reads BIGINT b (and c, or OPND_NONE)
 EX_LENGTH, EX_SUBSTR, EX_LTRIM, EX_RTRIM, EX_TRIM, EX_CONCAT = 50, 51, 52, 53, 54, 55
 MAX_CONCAT_PIECES, MAX_VARCHAR_PROJECTIONS = 8, 8
+# conditionals: EX_IF(a, b, c) is a ? b : c with BOOLEAN a and vtype the type of b, c and the result; EX_COALESCE(a, b)
+EX_IF, EX_COALESCE = 60, 61
 V_BIGINT, V_DOUBLE, V_BOOLEAN, V_VARCHAR, V_DECIMAL = 0, 1, 2, 3, 4
 MAX_STRINGS, MAX_STRING_BYTES, MAX_LIKE_PATTERNS = 128, 4096, 8
 OPND_NONE, OPND_COLUMN, OPND_TEMP, OPND_CONST, OPND_NULL = 0, 1, 2, 3, 4

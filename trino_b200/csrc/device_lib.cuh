@@ -41,7 +41,8 @@ enum {
     TGD_EX_AND = 20, TGD_EX_OR = 21, TGD_EX_NOT = 22, TGD_EX_IS_NULL = 23, TGD_EX_IS_NOT_NULL = 24, TGD_EX_BETWEEN = 25,
     TGD_EX_CAST_BIGINT_TO_DOUBLE = 30, TGD_EX_CAST_DOUBLE_TO_BIGINT = 31, TGD_EX_CAST_TO_DECIMAL = 32, TGD_EX_CAST_DECIMAL_TO_BIGINT = 33,
     TGD_EX_CAST_DECIMAL_TO_DOUBLE = 34, TGD_EX_IN = 40, TGD_EX_LIKE = 41,
-    TGD_EX_LENGTH = 50, TGD_EX_SUBSTR = 51, TGD_EX_LTRIM = 52, TGD_EX_RTRIM = 53, TGD_EX_TRIM = 54, TGD_EX_CONCAT = 55
+    TGD_EX_LENGTH = 50, TGD_EX_SUBSTR = 51, TGD_EX_LTRIM = 52, TGD_EX_RTRIM = 53, TGD_EX_TRIM = 54, TGD_EX_CONCAT = 55,
+    TGD_EX_IF = 60, TGD_EX_COALESCE = 61
 };
 // TGD_V_DECIMAL_LONG is internal: the output-column type of a long DECIMAL projection (16-byte cells: high word, low word)
 enum { TGD_V_BIGINT = 0, TGD_V_DOUBLE = 1, TGD_V_BOOLEAN = 2, TGD_V_VARCHAR = 3, TGD_V_DECIMAL = 4, TGD_V_DECIMAL_LONG = 5 };
@@ -596,6 +597,14 @@ __device__ __forceinline__ Value vm_apply(int op, int vtype, Value a, Value b, V
             else r = llround(x);
             break;
         }
+        // both operands were evaluated; the select keeps one (its value and NULL flag)
+        case TGD_EX_IF: {
+            const bool t = !a.is_null && a.bits != 0;
+            r = t ? b.bits : c.bits;
+            rn = t ? b.is_null : c.is_null;
+            break;
+        }
+        case TGD_EX_COALESCE: r = a.is_null ? b.bits : a.bits; rn = a.is_null && b.is_null; break;
         default: break;
     }
     res.bits = r;
@@ -613,12 +622,17 @@ __device__ __forceinline__ Value vm_apply(int op, int vtype, Value a, Value b, V
 //             (BetweenCodeGenerator.java:62-80)
 //   calls:    the operands' errors in order, stopping at the first NULL operand (BytecodeUtils.java:303-306), then their own
 //   IS [NOT] NULL, MOV: the operand's
+//   IF:       the condition's; then the THEN operand's when the condition is TRUE, otherwise the ELSE operand's
+//             (IfCodeGenerator.java:47-62: a NULL condition counts as FALSE)
+//   COALESCE: the first operand's; none when it is non-NULL, otherwise the second's (CoalesceCodeGenerator.java:45-75)
 __device__ __forceinline__ uint32_t vm_error(int op, int vtype, Value a, uint32_t ea, Value b, uint32_t eb, Value c, uint32_t ec, uint32_t own)
 {
     if (ea) return ea;
     switch (op) {
         case TGD_EX_AND: return (!a.is_null && a.bits == 0) ? 0 : eb;
         case TGD_EX_OR: return (!a.is_null && a.bits != 0) ? 0 : eb;
+        case TGD_EX_IF: return (!a.is_null && a.bits != 0) ? eb : ec;
+        case TGD_EX_COALESCE: return a.is_null ? eb : 0;
         case TGD_EX_BETWEEN:
             if (a.is_null) return 0;
             if (eb) return eb;
@@ -1054,6 +1068,9 @@ __device__ __forceinline__ DVal vm_apply_dec(int op, int vtype, const DDec& d, D
             r.v.lo = (unsigned long long)__double_as_longlong(d.la ? tgd_u128_div_pow10_to_double(a.v, d.k1)
                                                                    : __ddiv_rn((double)(long long)a.v.lo, (double)d.m0));
             break;
+        // a is the BOOLEAN condition (la = 0); b, c and the result are one DECIMAL type, so both words are selected as they are
+        case TGD_EX_IF: r = (!a.is_null && a.v.lo != 0ULL) ? b : c; break;
+        case TGD_EX_COALESCE: r = a.is_null ? b : a; break;
         default: break;
     }
     if (!d.lr && op != TGD_EX_MOV) r.v.hi = (unsigned long long)((long long)r.v.lo >> 63);
@@ -1070,6 +1087,8 @@ __device__ __forceinline__ uint32_t vm_error_dec(int op, DVal a, uint32_t ea, DV
             if (eb) return eb;
             if (!b.is_null && u128_cmp(b.v, a.v) > 0) return 0;
             return ec;
+        case TGD_EX_IF: return (!a.is_null && a.v.lo != 0ULL) ? eb : ec;
+        case TGD_EX_COALESCE: return a.is_null ? eb : 0;
         case TGD_EX_ADD: case TGD_EX_SUB: case TGD_EX_MUL: case TGD_EX_DIV:
         case TGD_EX_EQ: case TGD_EX_NE: case TGD_EX_LT: case TGD_EX_LE: case TGD_EX_GT: case TGD_EX_GE:
             if (a.is_null) return 0;

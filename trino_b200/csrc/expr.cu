@@ -376,7 +376,7 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
         const bool unary = s.op == TGPU_EX_MOV || s.op == TGPU_EX_NEG || s.op == TGPU_EX_IS_NULL || s.op == TGPU_EX_IS_NOT_NULL || s.op == TGPU_EX_IN ||
                            s.op == TGPU_EX_CAST_TO_DECIMAL || s.op == TGPU_EX_CAST_DECIMAL_TO_BIGINT || s.op == TGPU_EX_CAST_DECIMAL_TO_DOUBLE ||
                            s.op == TGPU_EX_NOT;
-        const int used = unary ? 1 : s.op == TGPU_EX_BETWEEN ? 3 : 2;
+        const int used = unary ? 1 : (s.op == TGPU_EX_BETWEEN || s.op == TGPU_EX_IF) ? 3 : 2;
         if (!dec_insn(s)) {
             // a numeric instruction never reads a DECIMAL temp or a channel read as DECIMAL
             for (int k = 0; k < used && k < 3; k++) {
@@ -412,13 +412,16 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
                 if (s.vtype != TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: this cast reads a DECIMAL operand", i);
                 break;
             case TGPU_EX_MOD: return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: DECIMAL %% is not evaluated on the GPU", i);
+            case TGPU_EX_IF: case TGPU_EX_COALESCE: res_dec = true; break;
             default: return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: op %d does not take DECIMAL operands", i, s.op);
         }
+        // operand k is DECIMAL (IF's condition is a BOOLEAN: it keeps ot[0] = not a DECIMAL, so la = 0 and it is read as a plain word)
+        auto dec_opnd = [&](int k) { return opnd_dec && !(s.op == TGPU_EX_IF && k == 0); };
         DecType ot[3], rt;
         const tgpu_decimal_type* st[3] = {&sig.a, &sig.b, &sig.c};
         const int nopnd = s.op == TGPU_EX_IN ? 1 : used;
         for (int k = 0; k < nopnd; k++) {
-            if (!opnd_dec) continue;
+            if (!dec_opnd(k)) continue;
             if (!valid(*st[k])) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad DECIMAL type of operand %d", i, k);
             ot[k] = DecType{st[k]->precision, st[k]->scale};
         }
@@ -434,7 +437,7 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
                     return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: temp %d does not hold the operand's type", i, o.index);
             }
             else if (o.kind == TGPU_OPND_COLUMN) {
-                if (!opnd_dec) {
+                if (!dec_opnd(k)) {
                     if (col_seen[o.index] == 1) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads DECIMAL channel %d as another type", i, o.index);
                     col_seen[o.index] = 2;
                 }
@@ -445,7 +448,7 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
                     col_t[o.index] = ot[k];
                 }
             }
-            else if (o.kind == TGPU_OPND_CONST && opnd_dec) {
+            else if (o.kind == TGPU_OPND_CONST && dec_opnd(k)) {
                 long long hi = o.imm.i64 >> 63, lo = o.imm.i64;
                 if (ot[k].lng()) {
                     if (o.imm.i64 < 0 || o.imm.i64 >= p->num_decimal_constants)
@@ -480,6 +483,8 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
             return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: compared DECIMAL operands have different types", i);
         if ((s.op == TGPU_EX_MOV || s.op == TGPU_EX_NEG) && !(rt == ot[0]))
             return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: the result has another type than the operand", i);
+        if ((s.op == TGPU_EX_IF && !(ot[1] == rt && ot[2] == rt)) || (s.op == TGPU_EX_COALESCE && !(ot[0] == rt && ot[1] == rt)))
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: the operands of IF / COALESCE and its result are not one DECIMAL type", i);
         x.la = ot[0].lng();
         x.lb = ot[1].lng();
         x.lc = ot[2].lng();
@@ -532,6 +537,23 @@ static int compile_decimals(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram*
         if (res_dec && rt.lng()) out->long_temps |= 1u << s.dst;
     }
     for (int t = 0; t < TGPU_MAX_TEMPS; t++) out->temp_dec[t] = temp_t[t].p == 0 ? 0 : temp_t[t].lng() ? 2 : 1;
+    return TGPU_OK;
+}
+
+// IF / COALESCE (vtype not VARCHAR): IF's condition is BOOLEAN; the selected operands are present and, when temps, hold vtype (a channel's
+// type is known only at add_input, a constant has no type of its own).  Runs before the instruction's own result is recorded in `ts`.
+static int check_conditional(tgpu_ctx* ctx, const tgpu_expr_insn& s, int i, const TempState& ts)
+{
+    const bool is_if = s.op == TGPU_EX_IF;
+    auto temp_vt = [&](const tgpu_operand& o) { return o.index >= 0 && o.index < TGPU_MAX_TEMPS ? ts.vt[o.index] : -1; };
+    if (is_if && (s.a.kind == TGPU_OPND_NONE || (s.a.kind == TGPU_OPND_TEMP && temp_vt(s.a) != TGPU_V_BOOLEAN)))
+        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: the condition of IF is BOOLEAN", i);
+    const tgpu_operand* sel[2] = {is_if ? &s.b : &s.a, is_if ? &s.c : &s.b};
+    for (const tgpu_operand* o : sel) {
+        if (o->kind == TGPU_OPND_NONE) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: IF / COALESCE is missing an operand", i);
+        if (o->kind == TGPU_OPND_TEMP && temp_vt(*o) != s.vtype)
+            return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: temp %d does not hold the vtype of IF / COALESCE", i, o->index);
+    }
     return TGPU_OK;
 }
 
@@ -601,6 +623,10 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
         DInsn& d = out->insns[i];
         if (s.dst < 0 || s.dst >= TGPU_MAX_TEMPS) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: dst temp out of range", i);
         if (s.vtype < 0 || s.vtype > TGPU_V_DECIMAL) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: bad vtype", i);
+        const bool cond = s.op == TGPU_EX_IF || s.op == TGPU_EX_COALESCE;
+        // a VARCHAR temp is a view of one static source: a per-row choice between two sources does not fit it
+        if (cond && s.vtype == TGPU_V_VARCHAR) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "insn %d: IF / COALESCE with a VARCHAR result is not evaluated on the GPU", i);
+        if (cond) TG_TRY(check_conditional(ctx, s, i, ts));
         if (s.vtype == TGPU_V_VARCHAR || s.op == TGPU_EX_LIKE) {
             TG_TRY(compile_varchar_insn(ctx, p, i, out, max_channel, &ts));
             continue;
@@ -617,6 +643,7 @@ int expr_compile(tgpu_ctx* ctx, const tgpu_expr_program* p, DProgram* out, int32
             case TGPU_EX_AND: case TGPU_EX_OR: case TGPU_EX_NOT: case TGPU_EX_IS_NULL: case TGPU_EX_IS_NOT_NULL: case TGPU_EX_BETWEEN:
             case TGPU_EX_CAST_BIGINT_TO_DOUBLE: case TGPU_EX_CAST_DOUBLE_TO_BIGINT:
             case TGPU_EX_CAST_TO_DECIMAL: case TGPU_EX_CAST_DECIMAL_TO_BIGINT: case TGPU_EX_CAST_DECIMAL_TO_DOUBLE:
+            case TGPU_EX_IF: case TGPU_EX_COALESCE:
                 break;
             case TGPU_EX_IN:
                 if (s.b.imm.i64 < 0 || s.b.imm.i64 >= p->num_in_lists) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d: IN list index out of range", i);
@@ -1343,10 +1370,14 @@ struct FilterProjectOp : tgpu_op {
             const DOperand* ops[3] = {&host_prog.insns[i].a, &host_prog.insns[i].b, &host_prog.insns[i].c};
             const bool str = host_prog.insns[i].vtype == TGPU_V_VARCHAR;
             const DDec& dd = host_prog.dec[i];
+            // IF's condition is BOOLEAN whatever the vtype: a BOOLEAN channel is TGPU_INT8 (a DOUBLE read as raw bits would make -0.0 TRUE)
+            const bool if_cond_col = host_prog.insns[i].op == TGPU_EX_IF && ops[0]->kind == TGPU_OPND_COLUMN;
+            if (if_cond_col && in.cols[ops[0]->index].type != TGPU_INT8)
+                return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "insn %d reads channel %d as the BOOLEAN condition of IF, the page's channel is not INT8", i, ops[0]->index);
             if (dd.is_dec && host_prog.insns[i].vtype == TGPU_V_DECIMAL) {
-                // a short DECIMAL channel is TGPU_INT64, a long one TGPU_INT128
+                // a short DECIMAL channel is TGPU_INT64, a long one TGPU_INT128 (IF's condition, checked above, is not a DECIMAL operand)
                 const bool lng[3] = {dd.la != 0, dd.lb != 0, dd.lc != 0};
-                for (int k = 0; k < 3; k++) {
+                for (int k = if_cond_col ? 1 : 0; k < 3; k++) {
                     if (ops[k]->kind != TGPU_OPND_COLUMN) continue;
                     const int want = lng[k] ? TGPU_INT128 : TGPU_INT64;
                     if (in.cols[ops[k]->index].type != want)

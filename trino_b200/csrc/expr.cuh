@@ -414,7 +414,7 @@ __device__ __forceinline__ uint32_t vm_run(const DProgram* __restrict__ prog, in
             }
         }
         else {
-            if (in.op == TGPU_EX_BETWEEN) {
+            if (in.op == TGPU_EX_BETWEEN || in.op == TGPU_EX_IF) {
                 c = vm_fetch(in.c, cols, row, temps, tstride, nullbits, split, split_row);
                 ec = vm_carried(in.c, te);
             }

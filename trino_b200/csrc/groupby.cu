@@ -1438,6 +1438,8 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
                 case TGPU_EX_MOV: case TGPU_EX_NEG: case TGPU_EX_NOT: case TGPU_EX_CAST_BIGINT_TO_DOUBLE: case TGPU_EX_CAST_DOUBLE_TO_BIGINT: case TGPU_EX_IN:
                     n = opnd_nullable(in.a); break;
                 case TGPU_EX_BETWEEN: n = opnd_nullable(in.a) || opnd_nullable(in.b) || opnd_nullable(in.c); break;
+                case TGPU_EX_IF: n = opnd_nullable(in.b) || opnd_nullable(in.c); break;          // either branch may be selected
+                case TGPU_EX_COALESCE: n = opnd_nullable(in.a) && opnd_nullable(in.b); break;   // NULL only when both are
                 default: n = opnd_nullable(in.a) || opnd_nullable(in.b); break;
             }
             temp_nullable[in.dst] = n;

@@ -1521,6 +1521,9 @@ int join_filter_compile(tgpu_ctx* ctx, const tgpu_expr_program* program, int32_t
     TG_TRY(tg::expr_compile(ctx, program, out, &max_channel));
     if (tg::expr_uses_strings(*out)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters do not evaluate VARCHAR operations");
     if (tg::expr_uses_decimals(*out)) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters do not evaluate DECIMAL operations");
+    for (int i = 0; i < out->num_insns; i++)
+        if (out->insns[i].op == TGPU_EX_IF || out->insns[i].op == TGPU_EX_COALESCE)
+            return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "join filters do not evaluate IF or COALESCE");
     return TGPU_OK;
 }
 

@@ -395,6 +395,129 @@ def concat(*args):
     return e
 
 
+# ---- conditional special forms (SqlToRowExpressionTranslator.java:280-400) --------------------------------------------------------
+# The branches of one form have one type: the planner has already coerced them to the result type.  IF and the binary COALESCE are
+# instructions (abi.EX_IF, abi.EX_COALESCE); CASE, the simple CASE, NULLIF and a longer COALESCE keep the tree as written (the reference
+# evaluator reads it) and carry in `lowered` the tree of IF / COALESCE / EQ nodes PageProcessorProgram compiles.  A node that appears
+# twice in `lowered` (the simple CASE's value, NULLIF's first argument) is evaluated once.  VARCHAR results are not evaluated on the GPU.
+def _branch_type(*exprs):
+    """(vtype, dtype) of a form's result: its first branch that is not a bare NULL, else its first"""
+    for e in exprs:
+        if not isinstance(e, Null):
+            return e.vtype, getattr(e, "dtype", None)
+    return exprs[0].vtype, getattr(exprs[0], "dtype", None)
+
+
+class If:
+    """IF(cond, then[, else_]): then when cond is TRUE, otherwise else_ (NULL when missing); cond is BOOLEAN"""
+    lowered = None
+
+    def __init__(self, cond, then, else_=None):
+        self.vtype, self.dtype = _branch_type(then, else_) if else_ is not None else _branch_type(then)
+        self.cond, self.then = cond, then
+        self.else_ = else_ if else_ is not None else Null(self.vtype, self.dtype)
+
+
+class Case:
+    """searched CASE WHEN cond1 THEN r1 ... [ELSE else_] END: whens = [(cond, result), ...]; lowered to the right-deep IF chain"""
+
+    def __init__(self, whens, else_=None):
+        if not whens:
+            raise ValueError("CASE needs at least one WHEN")
+        self.whens, self.else_ = [tuple(w) for w in whens], else_
+        self.vtype, self.dtype = _branch_type(*[r for _, r in self.whens], *([else_] if else_ is not None else []))
+        e = else_
+        for c, r in reversed(self.whens):
+            e = If(c, r, e)
+        self.lowered = e
+
+
+class Switch:
+    """simple CASE value WHEN w1 THEN r1 ... [ELSE else_] END: whens = [(w, result), ...], each w of value's type.  Lowered to
+    IF(value = w1, r1, IF(value = w2, r2, ... else_)) with value the first operand of every EQ: value's error comes first, and a NULL
+    value makes every EQ NULL without reading any w's error, as SwitchCodeGenerator does"""
+
+    def __init__(self, value, whens, else_=None):
+        if not whens:
+            raise ValueError("CASE needs at least one WHEN")
+        self.value, self.whens, self.else_ = value, [tuple(w) for w in whens], else_
+        self.vtype, self.dtype = _branch_type(*[r for _, r in self.whens], *([else_] if else_ is not None else []))
+        e = else_
+        for w, r in reversed(self.whens):
+            e = If(Call(abi.EX_EQ, value, w), r, e)
+        self.lowered = e
+
+
+class Coalesce:
+    """COALESCE(a1, ..., an): the first non-NULL argument.  More than two arguments lower to COALESCE(a1, COALESCE(a2, ...))"""
+
+    def __init__(self, *args):
+        if len(args) < 2:
+            raise ValueError("COALESCE needs at least two arguments")
+        self.args = list(args)
+        self.vtype, self.dtype = _branch_type(*args)
+        self.lowered = Coalesce(args[0], Coalesce(*args[1:])) if len(args) > 2 else None
+
+
+def _cast(e, vtype, dtype=None):
+    """e as (vtype, dtype): the cast the planner puts around a comparison operand of another type"""
+    ev, ed = e.vtype, getattr(e, "dtype", None)
+    if ev == vtype and (vtype != abi.V_DECIMAL or tuple(ed) == tuple(dtype)):
+        return e
+    if ev == abi.V_BIGINT and vtype == abi.V_DOUBLE:
+        return Call(abi.EX_CAST_BIGINT_TO_DOUBLE, e)
+    if ev == abi.V_DECIMAL and vtype == abi.V_DOUBLE:
+        return Call(abi.EX_CAST_DECIMAL_TO_DOUBLE, e)
+    if ev in (abi.V_BIGINT, abi.V_DECIMAL) and vtype == abi.V_DECIMAL:
+        return Call(abi.EX_CAST_TO_DECIMAL, e, result_dtype=dtype)
+    raise ValueError("no cast from vtype %d to vtype %d" % (ev, vtype))
+
+
+class NullIf:
+    """NULLIF(a, b): NULL when a = b, otherwise a.  compare_as: the common type of the comparison when it is not a's, as a vtype or
+    (vtype, dtype).  Lowered to IF(cast(a) = cast(b), NULL, a) with a evaluated once: a NULL a stops the EQ before b, so b raises
+    nothing, as NullIfCodeGenerator does"""
+
+    def __init__(self, a, b, compare_as=None):
+        self.a, self.b = a, b
+        self.vtype, self.dtype = a.vtype, getattr(a, "dtype", None)
+        if compare_as is None:
+            cv, cd = self.vtype, self.dtype
+        elif isinstance(compare_as, int):
+            cv, cd = compare_as, None
+        else:
+            cv, cd = compare_as
+        self.compare_as = (cv, cd)
+        self.lowered = If(Call(abi.EX_EQ, _cast(a, cv, cd), _cast(b, cv, cd)), Null(self.vtype, self.dtype), a)
+
+
+def _lower(e):
+    while getattr(e, "lowered", None) is not None:
+        e = e.lowered
+    return e
+
+
+def _children(e):
+    """the operands of an instruction node (after _lower)"""
+    if isinstance(e, Call):
+        return e.args
+    if isinstance(e, If):
+        return [e.cond, e.then, e.else_]
+    if isinstance(e, Coalesce):
+        return e.args
+    return []
+
+
+def _count_reads(e, reads):
+    """reads[id(node)]: how many instruction operands read each node of the tree below e (once per edge); each node is visited once"""
+    for c in _children(e):
+        c = _lower(c)
+        first = id(c) not in reads
+        reads[id(c)] = reads.get(id(c), 0) + 1
+        if first:
+            _count_reads(c, reads)
+
+
 class PageProcessorProgram:
     """Compiles expression trees (the RowExpressions of LocalExecutionPlanner.java:2111-2114) to the three-address
     tgpu_expr_program.  `projections`: ints pass a channel through, expressions are computed."""
@@ -458,6 +581,16 @@ class PageProcessorProgram:
         return self.strings.index(b)
 
     def _emit(self, e):
+        """one tree (the filter or a projection): a node read by several operands within it is emitted once, at its first use, and its
+        temp is freed after its last reader"""
+        self._reads, self._done = {}, {}
+        _count_reads(_lower(e), self._reads)
+        return self._emit_node(e)
+
+    def _emit_node(self, e):
+        e = _lower(e)
+        if id(e) in self._done:
+            return self._done[id(e)]
         if isinstance(e, Col):
             return (abi.OPND_COLUMN, e.channel, 0)
         if isinstance(e, Const) and e.vtype == abi.V_VARCHAR:
@@ -473,7 +606,20 @@ class PageProcessorProgram:
             return (abi.OPND_CONST, 0, imm.i64)
         if isinstance(e, Null):
             return (abi.OPND_NULL, 0, 0)
-        ops = [self._emit(a) for a in e.args]
+        if isinstance(e, (If, Coalesce)):
+            kids = [_lower(k) for k in _children(e)]
+            ops = [self._emit_node(k) for k in kids]
+            self._release(kids, ops)
+            dst = self._alloc()
+            sig = None
+            if e.vtype == abi.V_DECIMAL:
+                dts = [getattr(k, "dtype", None) or e.dtype for k in kids]
+                sig = (None, dts[1], dts[2], e.dtype) if isinstance(e, If) else (dts[0], dts[1], None, e.dtype)
+            self._push(abi.EX_IF if isinstance(e, If) else abi.EX_COALESCE, e.vtype, dst, *ops, sig=sig)
+            self._done[id(e)] = (abi.OPND_TEMP, dst, 0)
+            return self._done[id(e)]
+        kids = [_lower(a) for a in e.args]
+        ops = [self._emit_node(a) for a in kids]
         b = None
         if e.op == abi.EX_LIKE:
             self.like_patterns.append((_utf8(e.pattern), b"" if e.escape is None else _utf8(e.escape)))
@@ -495,9 +641,7 @@ class PageProcessorProgram:
                 vals.append(imm.i64)
             self.in_lists.append(vals)
             b = (abi.OPND_CONST, 0, len(self.in_lists) - 1)
-        for o in ops:   # operand temps die here (projection temps are never passed as operands twice)
-            if o[0] == abi.OPND_TEMP and o[1] != self.filter_temp:
-                self.live.discard(o[1])
+        self._release(kids, ops)
         dst = self._alloc()
         sig = None
         if e.operand_vtype == abi.V_DECIMAL or e.dtype is not None:
@@ -506,10 +650,21 @@ class PageProcessorProgram:
                 dts = [dts[0], None, None]
             sig = (dts[0], dts[1], dts[2], e.dtype)
         self._push(e.op, e.operand_vtype, dst, ops[0], b if b else (ops[1] if len(ops) > 1 else None), ops[2] if len(ops) > 2 else None, sig=sig)
-        return (abi.OPND_TEMP, dst, 0)
+        self._done[id(e)] = (abi.OPND_TEMP, dst, 0)
+        return self._done[id(e)]
+
+    def _release(self, kids, ops):
+        """operand temps die after their last reader (the filter's temp lives on: projections are emitted after it)"""
+        for k, o in zip(kids, ops):
+            if o[0] == abi.OPND_TEMP and o[1] != self.filter_temp:
+                self._reads[id(k)] -= 1
+                if self._reads[id(k)] == 0:
+                    self.live.discard(o[1])
 
     def _build(self):
         n = len(self.insns)
+        if n > 64:
+            raise ValueError("expression needs more than 64 instructions")
         self._insns = (abi.ExprInsn * max(1, n))()
         for i, (op, vt, dst, a, b, c) in enumerate(self.insns):
             ins = self._insns[i]
