@@ -306,9 +306,16 @@ typedef enum tgpu_agg_function {
     TGPU_AGG_MAX = 5,
     TGPU_AGG_SUM_DECIMAL = 6, /* DecimalSumAggregation.java:44-146: input TGPU_INT64 (short decimal) or TGPU_INT128 (long decimal) -> DECIMAL(38, s)
                                  as TGPU_INT128; "Decimal overflow" (NUMERIC_VALUE_OUT_OF_RANGE) when the sum leaves +-10^38                   */
-    TGPU_AGG_AVG_DECIMAL = 7  /* DecimalAverageAggregation.java:54-176: same inputs -> DECIMAL(p, s) of the input: sum / count rounded HALF_UP, as
+    TGPU_AGG_AVG_DECIMAL = 7, /* DecimalAverageAggregation.java:54-176: same inputs -> DECIMAL(p, s) of the input: sum / count rounded HALF_UP, as
                                  TGPU_INT64 for a short decimal and TGPU_INT128 for a long one (tgpu_agg_fn.reserved names the result type in a
                                  FINAL step, where the state no longer tells)                                                                   */
+    /* Variance family (VarianceAggregation.java:34-116), in both tgpu_agg_create and tgpu_aggregation_create.  Input: a DOUBLE, or a BIGINT / INTEGER / SMALLINT / TINYINT value as (double) value; REAL, DECIMAL and VARCHAR are
+       not accepted.  State: VarianceState {count, mean, m2} (M/operator/aggregation/state/VarianceState.java), updated by Welford's step
+       (:35-41) and merged by Chan's combination (:43-59).  Result: DOUBLE.                                                             */
+    TGPU_AGG_VAR_SAMP = 8,    /* variance / var_samp, VarianceAggregation.java:52-67: m2 / (count - 1), NULL when count < 2             */
+    TGPU_AGG_VAR_POP = 9,     /* var_pop, :69-84: m2 / count, NULL when count == 0                                                       */
+    TGPU_AGG_STDDEV_SAMP = 10,/* stddev / stddev_samp, :86-101: sqrt(var_samp), correctly rounded                                        */
+    TGPU_AGG_STDDEV_POP = 11  /* stddev_pop, :103-116: sqrt(var_pop)                                                                     */
 } tgpu_agg_function;
 
 typedef enum tgpu_agg_step {   /* M/sql/planner/plan/AggregationNode.java:361-402 */
@@ -334,6 +341,8 @@ typedef struct tgpu_agg_fn {
  *   sum (decimal)  : TGPU_INT128 sum, INT64 overflow (LongDecimalWithOverflowState: total = sum + overflow * 2^128); the sum is NULL
  *                    when no input rows
  *   avg (decimal)  : TGPU_INT128 sum, INT64 overflow, INT64 count (LongDecimalWithOverflowAndLongState)
+ *   var_samp / var_pop / stddev_samp / stddev_pop : INT64 count, FLOAT64 m2, FLOAT64 mean - VarianceState's ROW(count, m2, mean), its
+ *                    fields sorted by name (StateCompiler.java:1059-1070); never NULL, (0, 0.0, 0.0) when no input rows
  * Variable-width (TGPU_UTF8) group-by keys are supported: each such key column owns a device string dictionary
  * (csrc/strdict.cuh, the AppendOnlyVariableWidthData analogue of M/operator/FlatHash.java:309-348); identity is exact
  * (full-byte comparison, colliding strings rehash), output key columns are UTF8 again.                                 */

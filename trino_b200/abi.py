@@ -37,6 +37,7 @@ MAX_STRINGS, MAX_STRING_BYTES, MAX_LIKE_PATTERNS = 128, 4096, 8
 OPND_NONE, OPND_COLUMN, OPND_TEMP, OPND_CONST, OPND_NULL = 0, 1, 2, 3, 4
 
 AGG_COUNT_STAR, AGG_COUNT, AGG_SUM, AGG_AVG, AGG_MIN, AGG_MAX, AGG_SUM_DECIMAL, AGG_AVG_DECIMAL = 0, 1, 2, 3, 4, 5, 6, 7
+AGG_VAR_SAMP, AGG_VAR_POP, AGG_STDDEV_SAMP, AGG_STDDEV_POP = 8, 9, 10, 11
 STEP_SINGLE, STEP_PARTIAL, STEP_FINAL, STEP_INTERMEDIATE = 0, 1, 2, 3
 JOIN_INNER, JOIN_PROBE_OUTER, JOIN_LOOKUP_OUTER, JOIN_FULL_OUTER = 0, 1, 2, 3
 COMM_ID_BYTES = 128

@@ -64,7 +64,10 @@ struct DDec {
 
 enum AccKind {
     ACC_ROWS = 0, ACC_NONNULL = 1, ACC_SUM_F64 = 2, ACC_SUM_I64_LO = 3, ACC_SUM_I64_HI = 4,
-    ACC_MIN_F64 = 5, ACC_MAX_F64 = 6, ACC_MIN_I64 = 7, ACC_MAX_I64 = 8, ACC_SUM_F64_FROM_I64 = 9
+    ACC_MIN_F64 = 5, ACC_MAX_F64 = 6, ACC_MIN_I64 = 7, ACC_MAX_I64 = 8, ACC_SUM_F64_FROM_I64 = 9,
+    // VarianceState {count, mean, m2} as three consecutive words (count, mean bits, m2 bits): the first word's kind names the input
+    // (a DOUBLE value, a BIGINT-family value, or an intermediate state row), the other two are ACC_VAR_MEAN / ACC_VAR_M2
+    ACC_VAR_F64 = 10, ACC_VAR_I64 = 11, ACC_VAR_STATE = 12, ACC_VAR_MEAN = 13, ACC_VAR_M2 = 14
 };
 
 #define TGD_EMPTY_KEY 0x8000000000000000ULL
@@ -1137,6 +1140,19 @@ __device__ __forceinline__ unsigned long long acc_combine(int kind, unsigned lon
     }
 }
 
+// VarianceState.update (M/operator/aggregation/state/VarianceState.java:35-41), Welford's step on (count, mean bits, m2 bits)
+__device__ __forceinline__ void acc_var_step(unsigned long long& n, unsigned long long& mean_bits, unsigned long long& m2_bits, double x)
+{
+    const long long c = (long long)n + 1;
+    double mean = __longlong_as_double((long long)mean_bits), m2 = __longlong_as_double((long long)m2_bits);
+    const double delta = __dsub_rn(x, mean);
+    mean = __dadd_rn(mean, __ddiv_rn(delta, __ll2double_rn(c)));
+    m2 = __dadd_rn(m2, __dmul_rn(delta, __dsub_rn(x, mean)));
+    n = (unsigned long long)c;
+    mean_bits = (unsigned long long)__double_as_longlong(mean);
+    m2_bits = (unsigned long long)__double_as_longlong(m2);
+}
+
 // one accumulator update by one row on a thread-private accumulator word; `hi_off` = distance to the HI half
 __device__ __forceinline__ void acc_update_private(int kind, unsigned long long* p, long long hi_off, long long bits)
 {
@@ -1154,9 +1170,48 @@ __device__ __forceinline__ void acc_update_private(int kind, unsigned long long*
         case ACC_MAX_F64: { unsigned long long k = f64_order_key_max(bits); if (k > *p) *p = k; break; }
         case ACC_MIN_I64: { unsigned long long k = i64_order_key(bits); if (k < *p) *p = k; break; }
         case ACC_MAX_I64: { unsigned long long k = i64_order_key(bits); if (k > *p) *p = k; break; }
+        case ACC_VAR_F64: case ACC_VAR_I64: {
+            unsigned long long n = *p, mean = p[hi_off], m2 = p[2 * hi_off];
+            acc_var_step(n, mean, m2, kind == ACC_VAR_F64 ? __longlong_as_double(bits) : __ll2double_rn(bits));
+            *p = n;
+            p[hi_off] = mean;
+            p[2 * hi_off] = m2;
+            break;
+        }
         default: break;
     }
 }
+
+// VarianceState.merge (VarianceState.java:43-59), Chan's combination of (n, mean, m2) with (nb, mb, qb), in place.  An empty side leaves
+// the other unchanged.  The new mean is written mean + delta * nb / n (not the reference's (n * mean + nb * mb) / n): it stays exact when
+// the two means agree, so a group of identical values keeps m2 == +0.0 however its rows were split.
+__device__ __forceinline__ void tgd_var_merge(unsigned long long& n, unsigned long long& mean, unsigned long long& m2,
+                                              unsigned long long nb, unsigned long long mb, unsigned long long qb)
+{
+    if ((long long)nb == 0) return;
+    if ((long long)n == 0) { n = nb; mean = mb; m2 = qb; return; }
+    const long long na = (long long)n, nt = na + (long long)nb;
+    const double ma = __longlong_as_double((long long)mean), dn = __ll2double_rn(nt), dnb = __ll2double_rn((long long)nb);
+    const double delta = __dsub_rn(__longlong_as_double((long long)mb), ma);
+    const double m = __dadd_rn(ma, __ddiv_rn(__dmul_rn(delta, dnb), dn));
+    const double cross = __ddiv_rn(__dmul_rn(__dmul_rn(__dmul_rn(delta, delta), dnb), __ll2double_rn(na)), dn);
+    const double q = __dadd_rn(__dadd_rn(__longlong_as_double((long long)m2), __longlong_as_double((long long)qb)), cross);
+    n = (unsigned long long)nt;
+    mean = (unsigned long long)__double_as_longlong(m);
+    m2 = (unsigned long long)__double_as_longlong(q);
+}
+
+// one intermediate state row (count, mean bits, m2 bits) merged into a thread-private variance accumulator; `hi_off` = word distance
+__device__ __forceinline__ void acc_var_merge_private(unsigned long long* p, long long hi_off, long long count, long long mean_bits, long long m2_bits)
+{
+    unsigned long long n = *p, mean = p[hi_off], m2 = p[2 * hi_off];
+    tgd_var_merge(n, mean, m2, (unsigned long long)count, (unsigned long long)mean_bits, (unsigned long long)m2_bits);
+    *p = n;
+    p[hi_off] = mean;
+    p[2 * hi_off] = m2;
+}
+
+__host__ __device__ __forceinline__ bool acc_is_var(int kind) { return kind == ACC_VAR_F64 || kind == ACC_VAR_I64 || kind == ACC_VAR_STATE; }
 
 // ---- small-group fused aggregation: kernel body as a template over a row program ------------------------
 // A row program P provides
@@ -1252,10 +1307,24 @@ __device__ __forceinline__ void agg_small_body(P& prog, const DColumns& cols, in
     for (int pair = warp; pair < (L + 2) * A; pair += nwarps) {
         int s = pair / A, a = pair % A;
         int kind = P::acc_kind(a);
-        if (kind == ACC_SUM_I64_HI) continue;   // reduced together with its LO half
+        if (kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;   // reduced together with their first word
         if (lfirst[s] == TGD_NO_ROW) continue;
         const unsigned long long* p = &acc[((size_t)s * A + a) * T];
-        if (kind == ACC_SUM_I64_LO) {
+        if (acc_is_var(kind)) {
+            unsigned long long n = 0, m = 0, q = 0;
+            for (int t = lane; t < T; t += 32) tgd_var_merge(n, m, q, p[t], p[t + T], p[t + 2 * T]);
+            for (int off = 16; off > 0; off >>= 1) {
+                const unsigned long long on = __shfl_xor_sync(0xffffffffu, n, off), om = __shfl_xor_sync(0xffffffffu, m, off),
+                                         oq = __shfl_xor_sync(0xffffffffu, q, off);
+                tgd_var_merge(n, m, q, on, om, oq);
+            }
+            if (lane == 0) {
+                out.blk_acc[(b * (L + 2) + s) * A + a] = n;
+                out.blk_acc[(b * (L + 2) + s) * A + a + 1] = m;
+                out.blk_acc[(b * (L + 2) + s) * A + a + 2] = q;
+            }
+        }
+        else if (kind == ACC_SUM_I64_LO) {
             const unsigned long long* ph = p + T;
             unsigned long long lo = 0, hi = 0;
             for (int t = lane; t < T; t += 32) { unsigned long long o = lo; lo += p[t]; hi += ph[t] + (lo < o ? 1 : 0); }
@@ -1292,8 +1361,17 @@ __device__ __forceinline__ void tgd_cta_reduce(const unsigned long long* acc, in
 #pragma unroll
     for (int a = 0; a < A; a++) {
         const int kind = kind_of(a);
-        if (kind == ACC_SUM_I64_HI) continue;
-        if (kind == ACC_SUM_I64_LO) {
+        if (kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;
+        if (acc_is_var(kind)) {
+            unsigned long long n = acc[a], m = acc[a + 1], q = acc[a + 2];
+            for (int off = 16; off > 0; off >>= 1) {
+                const unsigned long long on = __shfl_xor_sync(0xffffffffu, n, off), om = __shfl_xor_sync(0xffffffffu, m, off),
+                                         oq = __shfl_xor_sync(0xffffffffu, q, off);
+                tgd_var_merge(n, m, q, on, om, oq);
+            }
+            if (lane == 0) { wpart[warp * A + a] = n; wpart[warp * A + a + 1] = m; wpart[warp * A + a + 2] = q; }
+        }
+        else if (kind == ACC_SUM_I64_LO) {
             unsigned long long lo = acc[a], hi = acc[a + 1];
             for (int off = 16; off > 0; off >>= 1) {
                 unsigned long long ol = __shfl_xor_sync(0xffffffffu, lo, off), oh = __shfl_xor_sync(0xffffffffu, hi, off);
@@ -1310,8 +1388,15 @@ __device__ __forceinline__ void tgd_cta_reduce(const unsigned long long* acc, in
     __syncthreads();
     for (int a = threadIdx.x; a < A; a += blockDim.x) {
         const int kind = kind_of(a);
-        if (kind == ACC_SUM_I64_HI) continue;
-        if (kind == ACC_SUM_I64_LO) {
+        if (kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;
+        if (acc_is_var(kind)) {
+            unsigned long long n = 0, m = 0, q = 0;
+            for (int w = 0; w < nwarps; w++) tgd_var_merge(n, m, q, wpart[w * A + a], wpart[w * A + a + 1], wpart[w * A + a + 2]);
+            out[a] = n;
+            out[a + 1] = m;
+            out[a + 2] = q;
+        }
+        else if (kind == ACC_SUM_I64_LO) {
             unsigned long long lo = 0, hi = 0;
             for (int w = 0; w < nwarps; w++) { unsigned long long o = lo; lo += wpart[w * A + a]; hi += wpart[w * A + a + 1] + (lo < o ? 1 : 0); }
             out[a] = lo;

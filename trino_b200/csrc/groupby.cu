@@ -66,6 +66,8 @@ constexpr int S_GMAX = 64;             // regular groups the S path can hold (+2
 constexpr int S_SPECIAL_NULL = 0;      // special slot for the NULL key (single-key case)
 constexpr int S_SPECIAL_SENTINEL = 1;  // special slot for a key whose bits equal EMPTY_KEY
 
+__host__ __device__ static inline bool is_variance(int function) { return function >= TGPU_AGG_VAR_SAMP && function <= TGPU_AGG_STDDEV_POP; }
+
 struct SrcRef {
     int32_t is_temp;   // 0: channel of the input page, 1: VM temporary of the pre program
     int32_t index;
@@ -259,8 +261,15 @@ __global__ void __launch_bounds__(S_THREADS) agg_small_kernel(AggPlan plan, DCol
         v.bits = 0; v.is_null = false;
         for (int a = 0; a < A; a++) {
             const AccDesc& d = plan.accs[a];
-            if (d.kind == ACC_SUM_I64_HI) continue;
+            if (d.kind == ACC_SUM_I64_HI || d.kind == ACC_VAR_MEAN || d.kind == ACC_VAR_M2) continue;
             if (!mask_selected(plan, d.mask, cols, row, temps, T, nb)) continue;
+            if (d.kind == ACC_VAR_STATE) {
+                Fetched c = fetch_src(plan.srcs[d.src], cols, row, temps, T, nb);
+                Fetched mean = fetch_src(plan.srcs[plan.accs[a + 1].src], cols, row, temps, T, nb);
+                Fetched m2 = fetch_src(plan.srcs[plan.accs[a + 2].src], cols, row, temps, T, nb);
+                if (!c.is_null) acc_var_merge_private(&acc[((size_t)slot * A + a) * T + tid], hi_off, c.bits, mean.bits, m2.bits);
+                continue;
+            }
             if (d.src >= 0 && d.src != last_src) { v = fetch_src(plan.srcs[d.src], cols, row, temps, T, nb); last_src = d.src; }
             if (d.kind != ACC_ROWS && v.is_null) continue;
             acc_update_private(d.kind, &acc[((size_t)slot * A + a) * T + tid], hi_off, v.bits);
@@ -279,10 +288,24 @@ __global__ void __launch_bounds__(S_THREADS) agg_small_kernel(AggPlan plan, DCol
     for (int pair = warp; pair < (L + 2) * A; pair += nwarps) {
         int s = pair / A, a = pair % A;
         int kind = plan.accs[a].kind;
-        if (kind == ACC_SUM_I64_HI) continue;   // reduced together with its LO half
+        if (kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;   // reduced together with their first word
         if (lfirst[s] == NO_ROW) continue;
         const unsigned long long* p = &acc[((size_t)s * A + a) * T];
-        if (kind == ACC_SUM_I64_LO) {
+        if (acc_is_var(kind)) {
+            unsigned long long n = 0, m = 0, q = 0;
+            for (int t = lane; t < T; t += 32) tgd_var_merge(n, m, q, p[t], p[t + T], p[t + 2 * T]);
+            for (int off = 16; off > 0; off >>= 1) {
+                const unsigned long long on = __shfl_xor_sync(0xffffffffu, n, off), om = __shfl_xor_sync(0xffffffffu, m, off),
+                                         oq = __shfl_xor_sync(0xffffffffu, q, off);
+                tgd_var_merge(n, m, q, on, om, oq);
+            }
+            if (lane == 0) {
+                out.blk_acc[(b * (L + 2) + s) * A + a] = n;
+                out.blk_acc[(b * (L + 2) + s) * A + a + 1] = m;
+                out.blk_acc[(b * (L + 2) + s) * A + a + 2] = q;
+            }
+        }
+        else if (kind == ACC_SUM_I64_LO) {
             const unsigned long long* ph = p + T;
             unsigned long long lo = 0, hi = 0;
             for (int t = lane; t < T; t += 32) { unsigned long long o = lo; lo += p[t]; hi += ph[t] + (lo < o ? 1 : 0); }
@@ -406,8 +429,22 @@ __global__ void __launch_bounds__(256) agg_small_merge_kernel(AggPlan plan, DCol
     for (int pair = tid; pair < (S_GMAX + 2) * A; pair += T) {
         int ps = pair / A, a = pair % A;
         int kind = plan.accs[a].kind;
-        if (pfirst[ps] == NO_ROW || kind == ACC_SUM_I64_HI) continue;
+        if (pfirst[ps] == NO_ROW || kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;
         int gid = pgid[ps];
+        if (acc_is_var(kind)) {
+            unsigned long long* w = &st.acc[(size_t)a * st.cap + gid];
+            unsigned long long n = w[0], m = w[st.cap], q = w[2 * st.cap];
+            for (int b = 0; b < B; b++)
+                for (int s = 0; s < L + 2; s++) {
+                    if (blk_ps[b * (L + 2) + s] != ps) continue;
+                    size_t at = ((size_t)b * (L + 2) + s) * map.compact_count + map.of_plan[a];
+                    tgd_var_merge(n, m, q, part.blk_acc[at], part.blk_acc[at + 1], part.blk_acc[at + 2]);
+                }
+            w[0] = n;
+            w[st.cap] = m;
+            w[2 * st.cap] = q;
+            continue;
+        }
         unsigned long long r = st.acc[(size_t)a * st.cap + gid];
         unsigned long long rh = kind == ACC_SUM_I64_LO ? st.acc[(size_t)(a + 1) * st.cap + gid] : 0;
         for (int b = 0; b < B; b++) {
@@ -470,8 +507,16 @@ __global__ void __launch_bounds__(S_THREADS) agg_global_kernel(AggPlan plan, DCo
         v.bits = 0; v.is_null = false;
         for (int a = 0; a < A; a++) {
             const AccDesc& d = plan.accs[a];
-            if (d.kind == ACC_SUM_I64_HI) continue;
+            if (d.kind == ACC_SUM_I64_HI || d.kind == ACC_VAR_MEAN || d.kind == ACC_VAR_M2) continue;
             if (!mask_selected(plan, d.mask, cols, row, temps, T, nb)) continue;
+            if (d.kind == ACC_VAR_STATE) {
+                // a state row (count, m2, mean): the sources of the three words
+                Fetched c = fetch_src(plan.srcs[d.src], cols, row, temps, T, nb);
+                Fetched mean = fetch_src(plan.srcs[plan.accs[a + 1].src], cols, row, temps, T, nb);
+                Fetched m2 = fetch_src(plan.srcs[plan.accs[a + 2].src], cols, row, temps, T, nb);
+                if (!c.is_null) acc_var_merge_private(&acc[a], 1, c.bits, mean.bits, m2.bits);
+                continue;
+            }
             if (d.src >= 0 && d.src != last_src) { v = fetch_src(plan.srcs[d.src], cols, row, temps, T, nb); last_src = d.src; }
             if (d.kind != ACC_ROWS && v.is_null) continue;
             acc_update_private(d.kind, &acc[a], 1, v.bits);
@@ -489,10 +534,26 @@ __global__ void __launch_bounds__(256) agg_global_fold_kernel(AggPlan plan, cons
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     for (int a = warp; a < plan.num_accs; a += nwarps) {
         const int kind = plan.accs[a].kind;
-        if (kind == ACC_SUM_I64_HI) continue;
+        if (kind == ACC_SUM_I64_HI || kind == ACC_VAR_MEAN || kind == ACC_VAR_M2) continue;
         const int c = map.of_plan[a];
         unsigned long long* s = &st.acc[(size_t)a * st.cap];
-        if (kind == ACC_SUM_I64_LO) {
+        if (acc_is_var(kind)) {
+            unsigned long long n = 0, m = 0, q = 0;
+            for (int b = lane; b < B; b += 32) tgd_var_merge(n, m, q, part[(size_t)b * C + c], part[(size_t)b * C + c + 1], part[(size_t)b * C + c + 2]);
+            for (int off = 16; off > 0; off >>= 1) {
+                const unsigned long long on = __shfl_xor_sync(0xffffffffu, n, off), om = __shfl_xor_sync(0xffffffffu, m, off),
+                                         oq = __shfl_xor_sync(0xffffffffu, q, off);
+                tgd_var_merge(n, m, q, on, om, oq);
+            }
+            if (lane == 0) {
+                unsigned long long sn = s[0], sm = s[st.cap], sq = s[2 * st.cap];
+                tgd_var_merge(sn, sm, sq, n, m, q);
+                s[0] = sn;
+                s[st.cap] = sm;
+                s[2 * st.cap] = sq;
+            }
+        }
+        else if (kind == ACC_SUM_I64_LO) {
             unsigned long long lo = 0, hi = 0;
             for (int b = lane; b < B; b += 32) { unsigned long long o = lo; lo += part[(size_t)b * C + c]; hi += part[(size_t)b * C + c + 1] + (lo < o ? 1 : 0); }
             for (int off = 16; off > 0; off >>= 1) {
@@ -673,7 +734,7 @@ __global__ void __launch_bounds__(256) g_accumulate_kernel(AggPlan plan, DColumn
         v.bits = 0; v.is_null = false;
         for (int a = 0; a < plan.num_accs; a++) {
             const AccDesc& d = plan.accs[a];
-            if (d.kind == ACC_SUM_I64_HI) continue;
+            if (d.kind == ACC_SUM_I64_HI || d.kind >= ACC_VAR_F64) continue;   // (variance words: var_pass_kernel)
             if (!mask_selected(plan, d.mask, cols, row, nullptr, 0, 0)) continue;
             if (d.src >= 0 && d.src != last_src) { v = fetch_src(plan.srcs[d.src], cols, row, nullptr, 0, 0); last_src = d.src; }
             if (d.kind != ACC_ROWS && v.is_null) continue;
@@ -696,6 +757,92 @@ __global__ void __launch_bounds__(256) g_accumulate_kernel(AggPlan plan, DColumn
                 default: break;
             }
         }
+    }
+}
+
+// Path G variance (multipass form: every row has its group id).  Per page and per variance accumulator `a`, with page scratch
+// sc = [pivot | n | sum | q] x cap words:
+//   pass 0  pivot[g] = the value (state input: the mean) of some row of g - any row's, so a group of identical values is exact below
+//   pass 1  n[g] += 1 and sum[g] += x - pivot (state input: n += count, sum += count * (mean - pivot))
+//   var_page_mean_kernel   sum[g] <- page mean = pivot + sum / n
+//   pass 2  q[g] += (x - mean)^2 (state input: q += m2 + count * (mean_i - mean)^2)
+//   var_page_merge_kernel  state[g] = merge(state[g], (n, mean, q)) (VarianceState.merge), and the scratch is cleared for the next page
+// Summing deviations from the group's own page mean keeps the page's m2 free of the cancellation of the sum-of-squares formula.
+__device__ __forceinline__ bool var_fetch(const AggPlan& plan, int a, const DColumns& cols, int64_t row, long long* cnt, double* x, double* m2)
+{
+    const AccDesc& d = plan.accs[a];
+    if (!mask_selected(plan, d.mask, cols, row, nullptr, 0, 0)) return false;
+    Fetched v = fetch_src(plan.srcs[d.src], cols, row, nullptr, 0, 0);
+    if (v.is_null) return false;
+    if (d.kind == ACC_VAR_STATE) {
+        *cnt = v.bits;
+        if (*cnt == 0) return false;
+        *x = __longlong_as_double(fetch_src(plan.srcs[plan.accs[a + 1].src], cols, row, nullptr, 0, 0).bits);
+        *m2 = __longlong_as_double(fetch_src(plan.srcs[plan.accs[a + 2].src], cols, row, nullptr, 0, 0).bits);
+    }
+    else {
+        *cnt = 1;
+        *x = d.kind == ACC_VAR_F64 ? __longlong_as_double(v.bits) : __ll2double_rn(v.bits);
+        *m2 = 0.0;
+    }
+    return true;
+}
+
+__global__ void __launch_bounds__(256) var_pass_kernel(AggPlan plan, int a, int pass, DColumns cols, int64_t n, const int* __restrict__ gids,
+                                                       unsigned long long* __restrict__ sc, int64_t cap)
+{
+    int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    unsigned long long* pivot = sc;
+    unsigned long long* pn = sc + cap;
+    double* psum = (double*)(sc + 2 * cap);
+    double* pq = (double*)(sc + 3 * cap);
+    for (; row < n; row += stride) {
+        long long cnt;
+        double x, m2;
+        if (!var_fetch(plan, a, cols, row, &cnt, &x, &m2)) continue;
+        const int g = gids[row];
+        if (pass == 0) pivot[g] = (unsigned long long)__double_as_longlong(x);
+        else if (pass == 1) {
+            atomicAdd(&pn[g], (unsigned long long)cnt);
+            const double dev = __dsub_rn(x, __longlong_as_double((long long)pivot[g]));
+            atomicAdd(&psum[g], plan.accs[a].kind == ACC_VAR_STATE ? __dmul_rn(__ll2double_rn(cnt), dev) : dev);
+        }
+        else {
+            const double dev = __dsub_rn(x, psum[g]);
+            const double sq = __dmul_rn(dev, dev);
+            atomicAdd(&pq[g], plan.accs[a].kind == ACC_VAR_STATE ? __dadd_rn(m2, __dmul_rn(__ll2double_rn(cnt), sq)) : sq);
+        }
+    }
+}
+
+__global__ void var_page_mean_kernel(unsigned long long* __restrict__ sc, int64_t cap, int64_t groups)
+{
+    int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    double* psum = (double*)(sc + 2 * cap);
+    for (; g < groups; g += stride) {
+        const long long c = (long long)sc[cap + g];
+        if (c > 0) psum[g] = __dadd_rn(__longlong_as_double((long long)sc[g]), __ddiv_rn(psum[g], __ll2double_rn(c)));
+    }
+}
+
+__global__ void var_page_merge_kernel(unsigned long long* __restrict__ sc, int64_t cap, int64_t groups, int a, AggState st)
+{
+    int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; g < groups; g += stride) {
+        const unsigned long long c = sc[cap + g];
+        if (c == 0) continue;
+        unsigned long long* w = &st.acc[(size_t)a * st.cap + g];
+        unsigned long long n0 = w[0], m0 = w[st.cap], q0 = w[2 * st.cap];
+        tgd_var_merge(n0, m0, q0, c, sc[2 * cap + g], sc[3 * cap + g]);
+        w[0] = n0;
+        w[st.cap] = m0;
+        w[2 * st.cap] = q0;
+        sc[cap + g] = 0;
+        sc[2 * cap + g] = 0;
+        sc[3 * cap + g] = 0;
     }
 }
 
@@ -1112,6 +1259,7 @@ struct OutSpec {
                                      //   9 = 7 for a FINAL / SINGLE step: raises "Decimal overflow" instead of carrying the count on
                                      // 10 / 11 decimal average -> INT128 / INT64: the same total divided by the row count a5 (a plain counter when
                                      //   a5 < 0: a1), rounded HALF_UP (DecimalAverageAggregation.average); NULL when the count is 0
+                                     // 12 var_samp, 13 var_pop, 14 stddev_samp, 15 stddev_pop over the variance state at a0 (count, mean, m2)
     int32_t a0[48], a1[48], a2[48], a3[48], a4[48], a5[48];
     void* data[48];
     unsigned char* nullmap[48];      // 1 = NULL
@@ -1222,6 +1370,19 @@ __global__ void agg_output_kernel(AggState st, int64_t count, OutSpec spec, unsi
                 }
                 case 4: isn = cnt == 0; outv = f64_from_order_key(x); break;
                 case 5: isn = cnt == 0; outv = (long long)(x ^ 0x8000000000000000ULL); break;
+                case 12: case 13: case 14: case 15: {
+                    // VarianceAggregation.java:52-116 over the state at a0 (count, mean, m2): m2 / (count - 1) (NULL below 2 rows) or
+                    // m2 / count (NULL at 0 rows), and Math.sqrt of either
+                    const long long n = (long long)x;
+                    const bool samp = spec.kind[c] == 12 || spec.kind[c] == 14;
+                    isn = samp ? n < 2 : n == 0;
+                    if (isn) break;
+                    const double m2 = __longlong_as_double((long long)st.acc[(size_t)(spec.a0[c] + 2) * st.cap + g]);
+                    double r = __ddiv_rn(m2, __ll2double_rn(samp ? n - 1 : n));
+                    if (spec.kind[c] >= 14) r = __dsqrt_rn(r);
+                    outv = __double_as_longlong(r);
+                    break;
+                }
                 case 7: case 8: case 9: case 10: case 11: {
                     // DecimalSumAggregation: state = (sum mod 2^128 as a signed 128-bit value, overflow) with
                     // total = signed128(sum) + overflow * 2^128 (addWithOverflow, S/type/Int128Math.java)
@@ -1382,6 +1543,19 @@ __global__ void __launch_bounds__(256) agg_skip_kernel(DColumns cols, int64_t n,
                     ((long long*)f.out0)[i] = on ? 1 : 0;
                     double v = f.in_is_double ? __longlong_as_double(bits) : (double)bits;
                     ((double*)f.out1)[i] = on ? v : 0.0;
+                    break;
+                }
+                case TGPU_AGG_VAR_SAMP: case TGPU_AGG_VAR_POP: case TGPU_AGG_STDDEV_SAMP: case TGPU_AGG_STDDEV_POP: {
+                    // one Welford step from the empty state (VarianceState.java:35-41): (1, 0 + x * (x - mean), 0 + x / 1) - m2 is +0.0
+                    // (NaN for a non-finite x) and the mean of -0.0 is +0.0; a NULL or masked row is the empty state (0, 0.0, 0.0)
+                    unsigned long long cnt = 0, mean = 0, m2 = 0;
+                    if (on) {
+                        cnt = 0;
+                        acc_var_step(cnt, mean, m2, f.in_is_double ? __longlong_as_double(bits) : __ll2double_rn(bits));
+                    }
+                    ((long long*)f.out0)[i] = (long long)cnt;
+                    ((unsigned long long*)f.out1)[i] = m2;
+                    ((unsigned long long*)f.out2)[i] = mean;
                     break;
                 }
                 default:                                                       // sum / min / max: the value itself (raw bits for DOUBLE)
@@ -1582,10 +1756,17 @@ static std::string gen_agg_small_source(const AggPlan& plan, const DProgram* pro
     s += "  __device__ __forceinline__ void accumulate(unsigned long long* acc, int T) {\n";
     for (int a = 0; a < plan.num_accs; a++) {
         const AccDesc& d = plan.accs[a];
-        if (d.kind == ACC_SUM_I64_HI) continue;
+        if (d.kind == ACC_SUM_I64_HI || d.kind == ACC_VAR_MEAN || d.kind == ACC_VAR_M2) continue;
         if (d.kind == ACC_NONNULL && !src_nullable(d.src)) continue;
         std::string cond = "true";
         if (d.mask >= 0) { char b[64]; snprintf(b, sizeof(b), "(!vn%d && v%d != 0)", d.mask, d.mask); cond = b; }
+        if (d.kind == ACC_VAR_STATE) {
+            // a state row (count, m2, mean) merged into the variance words; a NULL count is no state
+            if (src_nullable(d.src)) { char b[64]; snprintf(b, sizeof(b), " && !vn%d", d.src); cond += b; }
+            fp_appendf(s, "    if (%s) acc_var_merge_private(acc + %d * T, T, v%d, v%d, v%d);\n", cond.c_str(), map->of_plan[a], d.src, plan.accs[a + 1].src,
+                       plan.accs[a + 2].src);
+            continue;
+        }
         if (d.kind != ACC_ROWS && src_nullable(d.src)) { char b[64]; snprintf(b, sizeof(b), " && !vn%d", d.src); cond += b; }
         if (d.kind == ACC_ROWS) fp_appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, 0);\n", cond.c_str(), d.kind, map->of_plan[a]);
         else fp_appendf(s, "    if (%s) acc_update_private(%d, acc + %d * T, T, v%d);\n", cond.c_str(), d.kind, map->of_plan[a], d.src);
@@ -1711,6 +1892,8 @@ struct AggOp : tgpu_op {
     // path G
     DevBuf g_table, g_special;
     int64_t g_slots = 0;
+    DevBuf var_sc;                           // variance page scratch of the multipass form: [pivot | n | sum | q] x var_sc_cap
+    int64_t var_sc_cap = 0;
     // path G, fused form
     bool fused_general = false;
     DevBuf f_recs;
@@ -1795,6 +1978,23 @@ struct AggOp : tgpu_op {
         plan.accs[at] = AccDesc{kind, src, mask, 0};
         if (need == 2) plan.accs[at + 1] = AccDesc{ACC_SUM_I64_HI, src, mask, 0};
         plan.num_accs += need;
+        return at;
+    }
+
+    // the three words of a variance accumulator (count, mean, m2): over a raw value at `src`, or over the state columns count `src`,
+    // mean `mean_src` and m2 `m2_src`.  var_samp, var_pop, stddev_samp and stddev_pop of one input and mask share one.
+    int add_var_acc(int kind, int src, int mean_src, int m2_src, int mask)
+    {
+        for (int i = 0; i + 2 < plan.num_accs; i++)
+            if (plan.accs[i].kind == kind && plan.accs[i].src == src && plan.accs[i].mask == mask && plan.accs[i + 1].src == mean_src &&
+                plan.accs[i + 2].src == m2_src)
+                return i;
+        if (plan.num_accs + 3 > MAX_ACCS) return -1;
+        int at = plan.num_accs;
+        plan.accs[at] = AccDesc{kind, src, mask, 0};
+        plan.accs[at + 1] = AccDesc{ACC_VAR_MEAN, mean_src, mask, 0};
+        plan.accs[at + 2] = AccDesc{ACC_VAR_M2, m2_src, mask, 0};
+        plan.num_accs += 3;
         return at;
     }
 
@@ -2023,6 +2223,28 @@ struct AggOp : tgpu_op {
                 fp.in_elem_is_double = 0;
                 fn_input_types.push_back(type);
                 if (fp.acc_main < 0 || fp.acc_count < 0) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "too many accumulators");
+                fnplans.push_back(fp);
+                continue;
+            }
+            if (is_variance(f.function)) {
+                // VarianceAggregation.java:34-44: DOUBLE, or a BIGINT-family value as (double) value.  State input: the ROW(count BIGINT,
+                // m2 DOUBLE, mean DOUBLE) at input_channel, +1, +2.
+                src = src_of_channel(f.input_channel, &type, in);
+                if (src < 0) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "aggregate input channel %d out of range", f.input_channel);
+                if (type == TGPU_UTF8) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "aggregates over variable-width inputs are not supported");
+                if (type == TGPU_FLOAT32) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "aggregate function %d over a REAL channel: keep the Java accumulator", f.function);
+                if (type == TGPU_INT128) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "aggregate function %d over a 128-bit channel (only count and the decimal sum are built)", f.function);
+                if (!from_state) fp.acc_main = add_var_acc(type == TGPU_FLOAT64 ? ACC_VAR_F64 : ACC_VAR_I64, src, src, src, mask);
+                else {
+                    int t_m2 = 0, t_mean = 0;
+                    const int s_m2 = src_of_channel(f.input_channel + 1, &t_m2, in), s_mean = src_of_channel(f.input_channel + 2, &t_mean, in);
+                    if (type != TGPU_INT64 || s_m2 < 0 || s_mean < 0 || t_m2 != TGPU_FLOAT64 || t_mean != TGPU_FLOAT64)
+                        return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "the variance state is a BIGINT count, a DOUBLE m2 and a DOUBLE mean channel");
+                    fp.acc_main = add_var_acc(ACC_VAR_STATE, src, s_mean, s_m2, mask);
+                }
+                if (fp.acc_main < 0) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "too many accumulators");
+                fp.in_elem_is_double = type == TGPU_FLOAT64;
+                fn_input_types.push_back(type);
                 fnplans.push_back(fp);
                 continue;
             }
@@ -2389,6 +2611,27 @@ struct AggOp : tgpu_op {
         TG_TRY(run_general_ids(in, cols, gids.as<int>()));
         if (plan.num_accs > 0)
             TG_LAUNCH(ctx, g_accumulate_kernel, tg_grid(ctx, in.rows, 256, 8), 256, 0, plan, cols, in.rows, gids.as<int>(), state());
+        return var_passes(in, cols, gids.as<int>());
+    }
+
+    // the variance accumulators of a multipass page (var_pass_kernel); the page scratch is zero between pages
+    int var_passes(const DevPage& in, const DColumns& cols, const int* gids)
+    {
+        for (int a = 0; a < plan.num_accs; a++) {
+            if (!acc_is_var(plan.accs[a].kind)) continue;
+            if (var_sc_cap < st_cap) {
+                TG_TRY(var_sc.alloc(ctx, (size_t)st_cap * 4 * 8));
+                TG_CUDA(ctx, cudaMemsetAsync(var_sc.p, 0, (size_t)st_cap * 4 * 8, ctx->stream));
+                var_sc_cap = st_cap;
+            }
+            unsigned long long* sc = var_sc.as<unsigned long long>();
+            const int grid = tg_grid(ctx, in.rows, 256, 8), ggrid = tg_grid(ctx, std::max<int64_t>(group_count, 1), 256, 8);
+            for (int pass = 0; pass < 3; pass++) {
+                if (in.rows > 0) TG_LAUNCH(ctx, var_pass_kernel, grid, 256, 0, plan, a, pass, cols, in.rows, gids, sc, var_sc_cap);
+                if (pass == 1 && group_count > 0) TG_LAUNCH(ctx, var_page_mean_kernel, ggrid, 256, 0, sc, var_sc_cap, group_count);
+            }
+            if (group_count > 0) TG_LAUNCH(ctx, var_page_merge_kernel, ggrid, 256, 0, sc, var_sc_cap, group_count, a, state());
+        }
         return TGPU_OK;
     }
 
@@ -2397,6 +2640,9 @@ struct AggOp : tgpu_op {
     bool fused_ok() const
     {
         if (gids_only || plan.key_hashed) return false;
+        // a variance state is not a fire-and-forget reduction: the multipass form gives every row its group id (var_passes)
+        for (int a = 0; a < plan.num_accs; a++)
+            if (acc_is_var(plan.accs[a].kind)) return false;
         for (int k = 0; k < plan.num_keys; k++)
             if (plan.key_is_double[k]) return false;   // first-seen raw value (-0.0 vs +0.0) needs the representative row
         return true;
@@ -2951,11 +3197,11 @@ struct AggOp : tgpu_op {
                     const DevColumn* c = nullptr;
                     TG_TRY(channel(f.input_channel, &c));
                     outp.cols.push_back(*c);
-                    if (f.function == TGPU_AGG_AVG || f.function == TGPU_AGG_SUM_DECIMAL || f.function == TGPU_AGG_AVG_DECIMAL) {
+                    if (f.function == TGPU_AGG_AVG || f.function == TGPU_AGG_SUM_DECIMAL || f.function == TGPU_AGG_AVG_DECIMAL || is_variance(f.function)) {
                         TG_TRY(channel(f.input_channel + 1, &c));
                         outp.cols.push_back(*c);
                     }
-                    if (f.function == TGPU_AGG_AVG_DECIMAL) {
+                    if (f.function == TGPU_AGG_AVG_DECIMAL || is_variance(f.function)) {
                         TG_TRY(channel(f.input_channel + 2, &c));
                         outp.cols.push_back(*c);
                     }
@@ -3007,6 +3253,12 @@ struct AggOp : tgpu_op {
                         if (f.function == TGPU_AGG_AVG_DECIMAL) TG_TRY(new_col(TGPU_INT64, &k.out2));
                         break;
                     }
+                    case TGPU_AGG_VAR_SAMP: case TGPU_AGG_VAR_POP: case TGPU_AGG_STDDEV_SAMP: case TGPU_AGG_STDDEV_POP:
+                        // VarianceState of one row: ROW(count, m2, mean)
+                        TG_TRY(new_col(TGPU_INT64, &k.out0));
+                        TG_TRY(new_col(TGPU_FLOAT64, &k.out1));
+                        TG_TRY(new_col(TGPU_FLOAT64, &k.out2));
+                        break;
                     case TGPU_AGG_SUM: case TGPU_AGG_MIN: case TGPU_AGG_MAX: {
                         TG_TRY(new_col(k.in_is_double ? TGPU_FLOAT64 : TGPU_INT64, &k.out0));
                         auto nm = std::make_shared<DevBuf>();
@@ -3200,6 +3452,15 @@ struct AggOp : tgpu_op {
                     }
                     else TG_TRY(add_col(TGPU_INT128, 9, fp.acc_main, fp.acc_count, fp.acc2, fp.acc3, fp.acc4));
                     break;
+                case TGPU_AGG_VAR_SAMP: case TGPU_AGG_VAR_POP: case TGPU_AGG_STDDEV_SAMP: case TGPU_AGG_STDDEV_POP:
+                    if (partial_out) {
+                        // ROW(count BIGINT, m2 DOUBLE, mean DOUBLE), the state's fields sorted by name
+                        TG_TRY(add_col(TGPU_INT64, 0, fp.acc_main, -1));
+                        TG_TRY(add_col(TGPU_FLOAT64, 6, fp.acc_main + 2, -1));
+                        TG_TRY(add_col(TGPU_FLOAT64, 6, fp.acc_main + 1, -1));
+                    }
+                    else TG_TRY(add_col(TGPU_FLOAT64, 12 + (fp.function - TGPU_AGG_VAR_SAMP), fp.acc_main, -1));
+                    break;
                 case TGPU_AGG_AVG_DECIMAL:
                     if (partial_out) {
                         TG_TRY(add_col(TGPU_INT128, 7, fp.acc_main, fp.acc_count, fp.acc2, fp.acc3, fp.acc4));
@@ -3329,7 +3590,7 @@ struct AggOp : tgpu_op {
                 c.own_validity.reset();
                 c.validity = nullptr;                   // count over nothing is 0, not NULL
             }
-            else if (f.function == TGPU_AGG_AVG) TG_TRY(null_column(TGPU_FLOAT64, &c));
+            else if (f.function == TGPU_AGG_AVG || is_variance(f.function)) TG_TRY(null_column(TGPU_FLOAT64, &c));
             else if (f.function == TGPU_AGG_SUM_DECIMAL) TG_TRY(null_column(TGPU_INT128, &c));
             else if (f.function == TGPU_AGG_AVG_DECIMAL) TG_TRY(null_column(f.reserved == TGPU_INT64 ? TGPU_INT64 : TGPU_INT128, &c));
             else {

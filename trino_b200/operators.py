@@ -800,12 +800,14 @@ class PartialAggregationController:
             self.h = None
 
 
-_FLAT_STATE = {abi.AGG_AVG: 2, abi.AGG_SUM_DECIMAL: 2, abi.AGG_AVG_DECIMAL: 3}           # flat state columns per function (default 1)
+_FLAT_STATE = {abi.AGG_AVG: 2, abi.AGG_SUM_DECIMAL: 2, abi.AGG_AVG_DECIMAL: 3,           # flat state columns per function (default 1)
+               abi.AGG_VAR_SAMP: 3, abi.AGG_VAR_POP: 3, abi.AGG_STDDEV_SAMP: 3, abi.AGG_STDDEV_POP: 3}   # ROW(count, m2, mean)
 _DECIMAL_STATE = {abi.AGG_SUM_DECIMAL: "decimal_sum", abi.AGG_AVG_DECIMAL: "decimal_avg"}
 
 
 def _state_widths(aggregators):
-    """the reference's state type per aggregate: ROW(BIGINT, DOUBLE) for avg (2 flat columns), VARBINARY for the decimal states"""
+    """the reference's state type per aggregate: ROW(BIGINT, DOUBLE) for avg (2 flat columns), ROW(BIGINT, DOUBLE, DOUBLE) for the
+    variance family (3), VARBINARY for the decimal states"""
     return [_DECIMAL_STATE.get(a.function, _FLAT_STATE.get(a.function, 1)) for a in aggregators]
 
 
