@@ -12,11 +12,15 @@
 //   - output buffers are flushed per input page here (the reference flushes at 1 MB / 32768 rows,
 //     PositionsAppenderPageBuilder.java:34,132-142); values per partition and their order are identical.
 //
-// Device path: one kernel computes row hash -> partition id, a stable radix sort of (partition, row) pairs
-// yields the per-partition position lists, and one gather per column writes partition-contiguous buffers —
-// which are exactly the send buffers of the all-to-all.
+// Device paths.  The common one is the multi-split (multisplit.cuh, DESIGN.md §3.6): a histogram pass, an offsets pass and one
+// stable scatter move every fixed-width column of up to 8 bytes straight to its partition-contiguous place, which in the exchanges
+// is the send buffer or the destination's arena.  Replicated rows (nullChannel, replicatesAnyRow), variable-width and 16-byte
+// columns, more than 64 partitions or too many columns take the sort + compose path: one kernel computes row hash -> partition id,
+// a stable radix sort of (partition, row) pairs yields the per-partition position lists, and one gather per column writes the
+// partition's page.
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <chrono>
 
 #include "multisplit.cuh"
@@ -115,6 +119,91 @@ int host_type_hash(tgpu_ctx* ctx, const tgpu_column& c, uint64_t* out)
         default: return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "partition constant of type %d", c.type);
     }
 }
+
+// One lane of a multi-split: the values of column `col`, or (`nulls`) its NULL bytes, 1 = NULL.  `elem` is the scatter's
+// XchgCols.elem: the value width, 0 for a NULL-byte lane.  A NULL-byte lane without `src` (the page has no validity buffer) writes
+// all zeros: an exchange carries it when another rank's page of the same column has NULLs.
+struct XchgLane {
+    int col;
+    int32_t type;
+    int elem;
+    bool nulls;
+    const void* src;
+};
+
+size_t lane_bytes(const XchgLane& lane) { return lane.elem ? (size_t)lane.elem : 1; }
+
+// a value lane per column, followed by a NULL-byte lane where null_lane[c]
+std::vector<XchgLane> xchg_lanes(const DevPage& in, const std::vector<bool>& null_lane)
+{
+    std::vector<XchgLane> lanes;
+    for (int c = 0; c < (int)in.cols.size(); c++) {
+        lanes.push_back(XchgLane{c, in.cols[c].type, in.cols[c].elem_size(), false, in.cols[c].data});
+        if (null_lane[c]) lanes.push_back(XchgLane{c, in.cols[c].type, 0, true, in.cols[c].validity});
+    }
+    return lanes;
+}
+
+// the scatter's lane table; h_dst[lane * P + partition] is where the lane's rows of that partition start (uploaded to *d_dst)
+int xchg_cols(tgpu_ctx* ctx, const std::vector<XchgLane>& lanes, const std::vector<char*>& h_dst, DevBuf* d_dst, XchgCols* xc)
+{
+    TG_TRY(d_dst->alloc(ctx, h_dst.size() * sizeof(char*)));
+    TG_CUDA(ctx, cudaMemcpyAsync(d_dst->p, h_dst.data(), h_dst.size() * sizeof(char*), cudaMemcpyHostToDevice, ctx->stream));
+    memset(xc, 0, sizeof(*xc));
+    xc->count = (int32_t)lanes.size();
+    for (size_t l = 0; l < lanes.size(); l++) { xc->elem[l] = lanes[l].elem; xc->src[l] = lanes[l].src; }
+    xc->dst = d_dst->as<char*>();
+    return TGPU_OK;
+}
+
+// The page of `rows` rows whose lane l starts at base[l]: value lanes become its columns, owning owner[l] when `owner` is given and
+// aliasing memory they do not own otherwise; NULL-byte lanes are packed into validity bitmaps.  A page of 0 rows has no validity.
+int xchg_page(tgpu_ctx* ctx, const std::vector<XchgLane>& lanes, const std::vector<char*>& base, int64_t rows,
+              const std::vector<std::shared_ptr<DevBuf>>* owner, DevPage* out)
+{
+    out->rows = rows;
+    out->cols.resize((size_t)std::count_if(lanes.begin(), lanes.end(), [](const XchgLane& l) { return !l.nulls; }));
+    for (size_t l = 0; l < lanes.size(); l++) {
+        DevColumn& dst = out->cols[lanes[l].col];
+        if (!lanes[l].nulls) {
+            dst.type = lanes[l].type;
+            dst.length = rows;
+            dst.data = base[l];
+            if (owner) dst.own_data = (*owner)[l];
+        }
+        else if (rows > 0) {
+            tgpu_column bytemap_col;
+            memset(&bytemap_col, 0, sizeof(bytemap_col));
+            bytemap_col.type = TGPU_INT8;
+            bytemap_col.flags = TGPU_COL_NULLS_BYTEMAP;
+            bytemap_col.length = rows;
+            bytemap_col.data = base[l];
+            bytemap_col.validity = (const uint8_t*)base[l];
+            DevColumn packed;
+            TG_TRY(tg_ingest_column(ctx, &bytemap_col, true, &packed));
+            dst.own_validity = packed.own_validity;
+            dst.validity = packed.validity;
+        }
+    }
+    return TGPU_OK;
+}
+
+// TGPU_TRACE=1: mark() synchronises and prints the wall time since the previous mark (diagnostics only)
+struct PhaseTrace {
+    tgpu_ctx* ctx;
+    std::string who;
+    bool on = getenv("TGPU_TRACE") != nullptr;
+    std::chrono::steady_clock::time_point last = std::chrono::steady_clock::now();
+
+    void mark(const char* what)
+    {
+        if (!on) return;
+        cudaStreamSynchronize(ctx->stream);
+        auto now = std::chrono::steady_clock::now();
+        fprintf(stderr, "[tgpu %s] %-22s %8.3f ms\n", who.c_str(), what, std::chrono::duration<double, std::milli>(now - last).count());
+        last = now;
+    }
+};
 
 struct PartitionOp : tgpu_op {
     std::vector<int32_t> key_channels;
@@ -284,15 +373,7 @@ struct PartitionOp : tgpu_op {
     {
         const int P = partition_count, C = (int)in.cols.size();
         const int64_t n = in.rows;
-        const bool trace = getenv("TGPU_TRACE") != nullptr;
-        auto t_last = std::chrono::steady_clock::now();
-        auto mark = [&](const char* what) {
-            if (!trace) return;
-            cudaStreamSynchronize(ctx->stream);
-            auto now = std::chrono::steady_clock::now();
-            fprintf(stderr, "[tgpu partition] %-22s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(now - t_last).count());
-            t_last = now;
-        };
+        PhaseTrace trace{ctx, "partition"};
         const XchgGeom geom = xchg_geom(ctx, n, P, false);
         const int grid = geom.nchunks;
         DevBuf pids, hist, block_off, d_totals;
@@ -310,59 +391,28 @@ struct PartitionOp : tgpu_op {
         TG_CUDA(ctx, cudaMemcpyAsync(counts.data(), d_totals.p, (size_t)P * 8, cudaMemcpyDeviceToHost, ctx->stream));
         TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         for (int q = 0; q < P; q++) off[q + 1] = off[q] + counts[q];
-        mark("hist+offsets");
-        struct Lane { int elem; const void* src; std::shared_ptr<DevBuf> out; int col; bool nulls; };
-        std::vector<Lane> lanes;
-        for (int c = 0; c < C; c++) {
-            lanes.push_back(Lane{in.cols[c].elem_size(), in.cols[c].data, nullptr, c, false});
-            if (in.cols[c].validity) lanes.push_back(Lane{0, in.cols[c].validity, nullptr, c, true});
-        }
+        trace.mark("hist+offsets");
+        std::vector<bool> has_nulls(C);
+        for (int c = 0; c < C; c++) has_nulls[c] = in.cols[c].validity != nullptr;
+        const std::vector<XchgLane> lanes = xchg_lanes(in, has_nulls);
+        std::vector<std::shared_ptr<DevBuf>> out(lanes.size());
         std::vector<char*> h_dst(lanes.size() * P);
         for (size_t l = 0; l < lanes.size(); l++) {
-            int es = lanes[l].elem ? lanes[l].elem : 1;
-            lanes[l].out = std::make_shared<DevBuf>();
-            TG_TRY(lanes[l].out->alloc(ctx, (size_t)n * es));
-            for (int q = 0; q < P; q++) h_dst[l * P + q] = (char*)lanes[l].out->p + off[q] * es;
+            out[l] = std::make_shared<DevBuf>();
+            TG_TRY(out[l]->alloc(ctx, (size_t)n * lane_bytes(lanes[l])));
+            for (int q = 0; q < P; q++) h_dst[l * P + q] = (char*)out[l]->p + off[q] * lane_bytes(lanes[l]);
         }
         DevBuf d_dst;
-        TG_TRY(d_dst.alloc(ctx, h_dst.size() * sizeof(char*)));
-        TG_CUDA(ctx, cudaMemcpyAsync(d_dst.p, h_dst.data(), h_dst.size() * sizeof(char*), cudaMemcpyHostToDevice, ctx->stream));
         XchgCols xc;
-        memset(&xc, 0, sizeof(xc));
-        xc.count = (int32_t)lanes.size();
-        for (size_t l = 0; l < lanes.size(); l++) { xc.elem[l] = lanes[l].elem; xc.src[l] = lanes[l].src; }
-        xc.dst = d_dst.as<char*>();
+        TG_TRY(xchg_cols(ctx, lanes, h_dst, &d_dst, &xc));
         TG_TRY(xchg_launch_scatter(ctx, geom, ids_from_key ? nullptr : pids.as<uint8_t>(), n, P, block_off.as<long long>(), xc, &k, bucket_count, b2p));
-        mark("scatter");
+        trace.mark("scatter");
+        std::vector<char*> base(lanes.size());
         for (int q = 0; q < P; q++) {
             if (counts[q] == 0) continue;
+            for (size_t l = 0; l < lanes.size(); l++) base[l] = h_dst[l * P + q];
             DevPage outp;
-            outp.rows = counts[q];
-            outp.cols.resize(C);
-            for (auto& lane : lanes) {
-                DevColumn& dst = outp.cols[lane.col];
-                int es = lane.elem ? lane.elem : 1;
-                char* base = (char*)lane.out->p + off[q] * es;
-                if (!lane.nulls) {
-                    dst.type = in.cols[lane.col].type;
-                    dst.length = counts[q];
-                    dst.own_data = lane.out;     // all partitions alias slices of one buffer per column
-                    dst.data = base;
-                }
-                else {
-                    tgpu_column bytemap_col;
-                    memset(&bytemap_col, 0, sizeof(bytemap_col));
-                    bytemap_col.type = TGPU_INT8;
-                    bytemap_col.flags = TGPU_COL_NULLS_BYTEMAP;
-                    bytemap_col.length = counts[q];
-                    bytemap_col.data = base;
-                    bytemap_col.validity = (const uint8_t*)base;
-                    DevColumn packed;
-                    TG_TRY(tg_ingest_column(ctx, &bytemap_col, true, &packed));
-                    dst.own_validity = packed.own_validity;
-                    dst.validity = packed.validity;
-                }
-            }
+            TG_TRY(xchg_page(ctx, lanes, base, counts[q], &out, &outp));     // all partitions alias slices of one buffer per lane
             OwnedPage* o = tg_make_owned_page(std::move(outp));
             o->partition = q;
             pending.push_back(o);
@@ -628,17 +678,87 @@ extern "C" int tgpu_comm_arena_open(tgpu_ctx* ctx, const uint8_t* all_handles)
 // is the completeness path, the multi-split paths above are the fast ones.
 // ------------------------------------------------------------------------------------------------
 namespace {
+// the type of a column's values: a DICT32 or RLE column's is its dictionary's
+int32_t value_type(const tgpu_column& col)
+{
+    return (col.type == TGPU_DICT32 || col.type == TGPU_RLE) && col.dictionary ? col.dictionary->type : col.type;
+}
+
 bool exchange_needs_general_path(const PartitionOp* p, const tgpu_page* page)
 {
     if (p->null_channel >= 0 || p->replicates_any_row) return true;
     if (2 * page->num_columns > XMAXC) return true;
     for (int c = 0; c < page->num_columns; c++) {
-        const tgpu_column& col = page->columns[c];
-        int type = (col.type == TGPU_DICT32 || col.type == TGPU_RLE) && col.dictionary ? col.dictionary->type : col.type;
+        int type = value_type(page->columns[c]);
         if (type == TGPU_UTF8 || type == TGPU_INT128) return true;
     }
     return false;
 }
+
+// The checks the blocking and the split-phase exchange share.  *general: the page takes the general exchange, because the
+// multi-split does not carry its shape or has fewer partitions than there are ranks.
+int exchange_prologue(tgpu_ctx* ctx, const PartitionOp* p, const tgpu_page* page, bool* general)
+{
+    TG_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->comm) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "tgpu_comm_init has not been called");
+    const int W = ctx->world;
+    if (p->partition_count != W) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "partition count %d != world size %d", p->partition_count, W);
+    if (page->num_rows > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "page has more than 2^31-1 positions");
+    *general = exchange_needs_general_path(p, page) || W > XMAXP;
+    return TGPU_OK;
+}
+
+// The count matrix: the `per_rank` int64 entries every rank holds in d_mine, all-gathered into a host matrix with one row per
+// rank, in rank order.  One device-to-host copy and one wait.
+int count_matrix(tgpu_ctx* ctx, const DevBuf& d_mine, size_t per_rank, std::vector<long long>* matrix)
+{
+    const int W = ctx->world;
+    DevBuf d_all;
+    TG_TRY(d_all.alloc(ctx, (size_t)W * per_rank * 8));
+    if (W > 1) TG_NCCL(ctx, g_nccl.all_gather(d_mine.p, d_all.p, per_rank, NCCL_INT64, ctx->comm, ctx->stream));
+    else TG_CUDA(ctx, cudaMemcpyAsync(d_all.p, d_mine.p, per_rank * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    matrix->resize((size_t)W * per_rank);
+    TG_CUDA(ctx, cudaMemcpyAsync(matrix->data(), d_all.p, (size_t)W * per_rank * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return TGPU_OK;
+}
+
+// per column: does any rank's page carry NULLs (entry first + c of each rank's row of V entries), so that it needs a NULL-byte lane
+std::vector<bool> null_lanes(const std::vector<long long>& matrix, int W, int V, int first, int C)
+{
+    std::vector<bool> any(C, false);
+    for (int c = 0; c < C; c++)
+        for (int r = 0; r < W; r++) any[c] = any[c] || matrix[(size_t)r * V + first + c] != 0;
+    return any;
+}
+
+// Where the rows of a peer-store or split-phase exchange land in a destination's arena: one 256-byte aligned region per lane,
+// as many rows long as the destination receives, in lane order; inside a region the rows of lower-ranked senders come first.
+// Every sender and the receiver derive it from the same count matrix (entry d of each rank's row: its rows for destination d), so
+// they agree byte for byte.
+struct ArenaLayout {
+    std::vector<long long> total_recv_of, first_row;    // per destination: rows it receives, and where this rank's start
+    std::vector<size_t> es;                             // per lane: bytes per row
+
+    ArenaLayout(const std::vector<long long>& matrix, int W, int V, int me, const std::vector<XchgLane>& lanes) : total_recv_of(W, 0), first_row(W, 0)
+    {
+        for (int d = 0; d < W; d++)
+            for (int r = 0; r < W; r++) {
+                total_recv_of[d] += matrix[(size_t)r * V + d];
+                if (r < me) first_row[d] += matrix[(size_t)r * V + d];
+            }
+        for (auto& lane : lanes) es.push_back(lane_bytes(lane));
+    }
+    size_t region_off(int d, size_t lane) const
+    {
+        size_t off = 0;
+        for (size_t l = 0; l < lane; l++) off += (((size_t)total_recv_of[d] * es[l]) + 255) & ~(size_t)255;
+        return off;
+    }
+    size_t bytes(int d) const { return region_off(d, es.size()); }
+    // where this rank's rows of lane l go in the arena of destination d
+    char* dst(void* arena, int d, size_t l) const { return (char*)arena + region_off(d, l) + (size_t)first_row[d] * es[l]; }
+};
 
 // part[d]: the rows this rank has for rank d (nullptr = none); the parts must stay alive until this returns
 int exchange_pages(tgpu_ctx* ctx, const std::vector<const DevPage*>& part, const std::vector<int32_t>& types, tgpu_page** out)
@@ -664,16 +784,12 @@ int exchange_pages(tgpu_ctx* ctx, const std::vector<const DevPage*>& part, const
             }
         }
     }
-    std::vector<long long> all((size_t)W * W * V);
+    std::vector<long long> all;
     {
-        DevBuf d_mine, d_all;
+        DevBuf d_mine;
         TG_TRY(d_mine.alloc(ctx, mine.size() * 8));
-        TG_TRY(d_all.alloc(ctx, all.size() * 8));
         TG_CUDA(ctx, cudaMemcpyAsync(d_mine.p, mine.data(), mine.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-        if (W > 1) TG_NCCL(ctx, g_nccl.all_gather(d_mine.p, d_all.p, mine.size(), NCCL_INT64, ctx->comm, ctx->stream));
-        else TG_CUDA(ctx, cudaMemcpyAsync(d_all.p, d_mine.p, mine.size() * 8, cudaMemcpyDeviceToDevice, ctx->stream));
-        TG_CUDA(ctx, cudaMemcpyAsync(all.data(), d_all.p, all.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        TG_TRY(count_matrix(ctx, d_mine, mine.size(), &all));
     }
     auto info = [&](int sender, int dest, int k) { return all[((size_t)sender * W + dest) * V + k]; };
     long long total_recv = 0;
@@ -779,10 +895,7 @@ int exchange_pages(tgpu_ctx* ctx, const std::vector<const DevPage*>& part, const
 std::vector<int32_t> value_types_of(const tgpu_page* page)
 {
     std::vector<int32_t> types(page->num_columns);
-    for (int c = 0; c < page->num_columns; c++) {
-        const tgpu_column& col = page->columns[c];
-        types[c] = (col.type == TGPU_DICT32 || col.type == TGPU_RLE) && col.dictionary ? col.dictionary->type : col.type;
-    }
+    for (int c = 0; c < page->num_columns; c++) types[c] = value_type(page->columns[c]);
     return types;
 }
 
@@ -816,25 +929,14 @@ extern "C" int tgpu_exchange_partitioned_fenced(tgpu_ctx* ctx, tgpu_op* partitio
     PartitionOp* p = dynamic_cast<PartitionOp*>(partitioner);
     if (!ctx || !p || !page || !out) return TGPU_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->comm) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "tgpu_comm_init has not been called");
-    const int W = ctx->world;
-    if (p->partition_count != W) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "partition count %d != world size %d", p->partition_count, W);
-    int64_t n = page->num_rows;
-    if (n > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "page has more than 2^31-1 positions");
-    if (exchange_needs_general_path(p, page) || W > XMAXP) return exchange_general(ctx, p, page, out);
+    bool general = false;
+    TG_TRY(exchange_prologue(ctx, p, page, &general));
+    if (general) return exchange_general(ctx, p, page, out);
+    const int W = ctx->world, me = ctx->rank;
+    const int64_t n = page->num_rows;
     DevPage in;
     TG_TRY(tg_ingest_page(ctx, page, &in));
-    // TGPU_TRACE=1: synchronise and print the wall time of every phase (diagnostics only)
-    const bool trace = getenv("TGPU_TRACE") != nullptr;
-    auto t_last = std::chrono::steady_clock::now();
-    auto mark = [&](const char* what) {
-        if (!trace) return;
-        cudaStreamSynchronize(ctx->stream);
-        auto now = std::chrono::steady_clock::now();
-        fprintf(stderr, "[tgpu exchange rank %d] %-22s %8.3f ms\n", ctx->rank, what, std::chrono::duration<double, std::milli>(now - t_last).count());
-        t_last = now;
-    };
+    PhaseTrace trace{ctx, "exchange rank " + std::to_string(me)};
     const int C = (int)in.cols.size();
     // 1. partition ids + per-CTA histograms + offsets (stable multi-split, no sort)
     const XchgGeom geom = xchg_geom(ctx, n, W, W > 1);
@@ -854,82 +956,56 @@ extern "C" int tgpu_exchange_partitioned_fenced(tgpu_ctx* ctx, tgpu_op* partitio
         TG_CUDA(ctx, cudaMemcpyAsync(send_vec.data(), d_totals.p, (size_t)W * 8, cudaMemcpyDeviceToHost, ctx->stream));
         TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
-    mark("hist+offsets");
+    trace.mark("hist+offsets");
     for (int c = 0; c < C; c++) send_vec[W + c] = in.cols[c].validity ? 1 : 0;
     // 2. count matrix: every rank learns what every rank sends to whom (and which columns carry NULLs anywhere)
     const int V = W + C;
-    std::vector<long long> matrix((size_t)W * V);
-    DevBuf d_send, d_matrix;
+    std::vector<long long> matrix;
+    DevBuf d_send;
     TG_TRY(d_send.alloc(ctx, (size_t)V * 8));
-    TG_TRY(d_matrix.alloc(ctx, (size_t)W * V * 8));
     TG_CUDA(ctx, cudaMemcpyAsync(d_send.p, send_vec.data(), (size_t)V * 8, cudaMemcpyHostToDevice, ctx->stream));
-    TG_NCCL(ctx, g_nccl.all_gather(d_send.p, d_matrix.p, (size_t)V, NCCL_INT64, ctx->comm, ctx->stream));
-    TG_CUDA(ctx, cudaMemcpyAsync(matrix.data(), d_matrix.p, (size_t)W * V * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    mark("count all-gather");
-    std::vector<long long> send_counts(send_vec.begin(), send_vec.begin() + W), send_off(W + 1, 0), recv_counts(W), recv_off(W + 1, 0);
+    TG_TRY(count_matrix(ctx, d_send, V, &matrix));
+    trace.mark("count all-gather");
+    std::vector<long long> send_off(W + 1, 0), recv_counts(W), recv_off(W + 1, 0);
     for (int r = 0; r < W; r++) {
-        send_off[r + 1] = send_off[r] + send_counts[r];
-        recv_counts[r] = matrix[(size_t)r * V + ctx->rank];
+        send_off[r + 1] = send_off[r] + send_vec[r];
+        recv_counts[r] = matrix[(size_t)r * V + me];
         recv_off[r + 1] = recv_off[r] + recv_counts[r];
     }
-    long long total_recv = recv_off[W];
-    if (total_recv > (long long)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "exchange output exceeds 2^31-1 rows on rank %d", ctx->rank);
-    std::vector<bool> any_nulls(C, false);
-    for (int c = 0; c < C; c++)
-        for (int r = 0; r < W; r++) any_nulls[c] = any_nulls[c] || matrix[(size_t)r * V + W + c] != 0;
+    const long long total_recv = recv_off[W];
+    if (total_recv > (long long)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "exchange output exceeds 2^31-1 rows on rank %d", me);
     // 3. one scatter pass writes every column (and the NULL bytes of nullable columns) partition-contiguously
-    struct Lane { int elem; const void* src; DevBuf send; std::shared_ptr<DevBuf> recv; int col; bool nulls; };
-    std::vector<Lane> lanes;
-    for (int c = 0; c < C; c++) {
-        lanes.push_back(Lane{in.cols[c].elem_size(), in.cols[c].data, DevBuf(), nullptr, c, false});
-        if (any_nulls[c]) lanes.push_back(Lane{0, in.cols[c].validity, DevBuf(), nullptr, c, true});
-    }
-    // Peer-memory path: every rank can compute every destination's arena layout from the all-gathered count matrix
-    // (lane regions of total_recv(dst) x elem bytes, 256-byte aligned, in lane order), so the scatter kernel can store each
-    // row directly at its final address in the destination GPU's arena.
-    std::vector<long long> total_recv_of(W, 0);
-    for (int d = 0; d < W; d++)
-        for (int r = 0; r < W; r++) total_recv_of[d] += matrix[(size_t)r * V + d];
-    auto region_off = [&](int d, size_t lane) {
-        size_t off = 0;
-        for (size_t l = 0; l < lane; l++) off += (((size_t)total_recv_of[d] * (lanes[l].elem ? lanes[l].elem : 1)) + 255) & ~(size_t)255;
-        return off;
-    };
+    const std::vector<XchgLane> lanes = xchg_lanes(in, null_lanes(matrix, W, V, W, C));
+    // Peer-memory path: every rank knows every destination's arena layout, so the scatter kernel stores each row directly at its
+    // final address in the destination GPU's arena.
+    const ArenaLayout layout(matrix, W, V, me, lanes);
     bool p2p = !ctx->arena_peer[0].empty() && !getenv("TGPU_EXCHANGE_NCCL");
-    for (int d = 0; d < W && p2p; d++) p2p = region_off(d, lanes.size()) <= ctx->arena_bytes;
+    for (int d = 0; d < W && p2p; d++) p2p = layout.bytes(d) <= ctx->arena_bytes;
     const int arena = (int)(ctx->arena_epoch % TGPU_NUM_ARENAS);
+    std::vector<DevBuf> send(lanes.size());
+    std::vector<std::shared_ptr<DevBuf>> recv(lanes.size());
     std::vector<char*> h_dst(lanes.size() * W);
     for (size_t l = 0; l < lanes.size(); l++) {
-        int es = lanes[l].elem ? lanes[l].elem : 1;
+        const size_t es = lane_bytes(lanes[l]);
         if (p2p) {
-            for (int d = 0; d < W; d++) {
-                long long before = 0;   // rows of lower-ranked senders come first in the destination
-                for (int r = 0; r < ctx->rank; r++) before += matrix[(size_t)r * V + d];
-                h_dst[l * W + d] = (char*)ctx->arena_peer[arena][d] + region_off(d, l) + (size_t)before * es;
-            }
+            for (int d = 0; d < W; d++) h_dst[l * W + d] = layout.dst(ctx->arena_peer[arena][d], d, l);
             continue;
         }
-        TG_TRY(lanes[l].send.alloc(ctx, (size_t)std::max<int64_t>(n, 1) * es));
-        lanes[l].recv = std::make_shared<DevBuf>();
-        TG_TRY(lanes[l].recv->alloc(ctx, (size_t)std::max<long long>(total_recv, 1) * es));
-        for (int r = 0; r < W; r++) h_dst[l * W + r] = (char*)lanes[l].send.p + send_off[r] * es;
+        TG_TRY(send[l].alloc(ctx, (size_t)std::max<int64_t>(n, 1) * es));
+        recv[l] = std::make_shared<DevBuf>();
+        TG_TRY(recv[l]->alloc(ctx, (size_t)std::max<long long>(total_recv, 1) * es));
+        for (int r = 0; r < W; r++) h_dst[l * W + r] = (char*)send[l].p + send_off[r] * es;
         // rows that stay on this GPU are scattered straight into their final place in the receive buffer
-        h_dst[l * W + ctx->rank] = (char*)lanes[l].recv->p + recv_off[ctx->rank] * es;
+        h_dst[l * W + me] = (char*)recv[l]->p + recv_off[me] * es;
     }
-    mark("buffer allocation");
+    trace.mark("buffer allocation");
     DevBuf d_dst;
-    TG_TRY(d_dst.alloc(ctx, h_dst.size() * sizeof(char*)));
-    TG_CUDA(ctx, cudaMemcpyAsync(d_dst.p, h_dst.data(), h_dst.size() * sizeof(char*), cudaMemcpyHostToDevice, ctx->stream));
-    if (n > 0) {
-        XchgCols xc;
-        memset(&xc, 0, sizeof(xc));
-        xc.count = (int32_t)lanes.size();
-        for (size_t l = 0; l < lanes.size(); l++) { xc.elem[l] = lanes[l].elem; xc.src[l] = lanes[l].src; }
-        xc.dst = d_dst.as<char*>();
-        TG_TRY(xchg_launch_scatter(ctx, geom, pids.as<uint8_t>(), n, W, block_off.as<long long>(), xc));
-    }
-    mark("scatter");
+    XchgCols xc;
+    TG_TRY(xchg_cols(ctx, lanes, h_dst, &d_dst, &xc));
+    if (n > 0) TG_TRY(xchg_launch_scatter(ctx, geom, pids.as<uint8_t>(), n, W, block_off.as<long long>(), xc));
+    trace.mark("scatter");
+    std::vector<char*> base(lanes.size());
+    DevPage outp;
     if (p2p) {
         // the rows are already in the destination arenas; a 1-element all-reduce on the stream is the barrier that tells
         // every rank that all its senders' scatter kernels have completed
@@ -945,77 +1021,28 @@ extern "C" int tgpu_exchange_partitioned_fenced(tgpu_ctx* ctx, tgpu_op* partitio
         TG_TRY(token.alloc(ctx, 16));
         TG_CUDA(ctx, cudaMemsetAsync(token.p, 0, 16, ctx->stream));
         TG_NCCL(ctx, g_nccl.all_reduce(token.p, (char*)token.p + 8, 1, NCCL_INT64, 0 /* ncclSum */, ctx->comm, ctx->stream));
-        mark("p2p scatter + barrier");
+        trace.mark("p2p scatter + barrier");
         ctx->arena_epoch++;
-        DevPage outp;
-        outp.rows = total_recv;
-        outp.cols.resize(C);
+        for (size_t l = 0; l < lanes.size(); l++) base[l] = (char*)ctx->arena_local[arena] + layout.region_off(me, l);
+        TG_TRY(xchg_page(ctx, lanes, base, total_recv, nullptr, &outp));     // aliases the arena: valid until the second-next exchange on this context
+    }
+    else {
+        // 4. all-to-all with explicit counts: one NCCL group for every column
+        TG_NCCL(ctx, g_nccl.group_start());
         for (size_t l = 0; l < lanes.size(); l++) {
-            DevColumn& dst = outp.cols[lanes[l].col];
-            char* region = (char*)ctx->arena_local[arena] + region_off(ctx->rank, l);
-            if (!lanes[l].nulls) {
-                dst.type = in.cols[lanes[l].col].type;
-                dst.length = total_recv;
-                dst.data = region;     // aliases the arena: valid until the second-next exchange on this context
-            }
-            else if (total_recv > 0) {
-                tgpu_column bytemap_col;
-                memset(&bytemap_col, 0, sizeof(bytemap_col));
-                bytemap_col.type = TGPU_INT8;
-                bytemap_col.flags = TGPU_COL_NULLS_BYTEMAP;
-                bytemap_col.length = total_recv;
-                bytemap_col.data = region;
-                bytemap_col.validity = (const uint8_t*)region;
-                DevColumn packed;
-                TG_TRY(tg_ingest_column(ctx, &bytemap_col, true, &packed));
-                dst.own_validity = packed.own_validity;
-                dst.validity = packed.validity;
+            const size_t es = lane_bytes(lanes[l]);
+            for (int r = 0; r < W; r++) {
+                if (r == me) continue;
+                if (send_vec[r] > 0)
+                    TG_NCCL(ctx, g_nccl.send((const char*)send[l].p + send_off[r] * es, (size_t)send_vec[r] * es, NCCL_INT8, r, ctx->comm, ctx->stream));
+                if (recv_counts[r] > 0)
+                    TG_NCCL(ctx, g_nccl.recv((char*)recv[l]->p + recv_off[r] * es, (size_t)recv_counts[r] * es, NCCL_INT8, r, ctx->comm, ctx->stream));
             }
         }
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        OwnedPage* po = tg_make_owned_page(std::move(outp));
-        *out = &po->hdr;
-        return TGPU_OK;
-    }
-    // 4. all-to-all with explicit counts: one NCCL group for every column
-    TG_NCCL(ctx, g_nccl.group_start());
-    for (size_t l = 0; l < lanes.size(); l++) {
-        int es = lanes[l].elem ? lanes[l].elem : 1;
-        for (int r = 0; r < W; r++) {
-            if (r == ctx->rank) continue;
-            if (send_counts[r] > 0)
-                TG_NCCL(ctx, g_nccl.send((const char*)lanes[l].send.p + send_off[r] * es, (size_t)send_counts[r] * es, NCCL_INT8, r, ctx->comm, ctx->stream));
-            if (recv_counts[r] > 0)
-                TG_NCCL(ctx, g_nccl.recv((char*)lanes[l].recv->p + recv_off[r] * es, (size_t)recv_counts[r] * es, NCCL_INT8, r, ctx->comm, ctx->stream));
-        }
-    }
-    TG_NCCL(ctx, g_nccl.group_end());
-    mark("nccl send/recv");
-    DevPage outp;
-    outp.rows = total_recv;
-    outp.cols.resize(C);
-    for (auto& lane : lanes) {
-        DevColumn& dst = outp.cols[lane.col];
-        if (!lane.nulls) {
-            dst.type = in.cols[lane.col].type;
-            dst.length = total_recv;
-            dst.own_data = lane.recv;
-            dst.data = lane.recv->p;
-        }
-        else if (total_recv > 0) {
-            // pack the received byte map into an Arrow bitmap
-            tgpu_column bytemap_col;
-            memset(&bytemap_col, 0, sizeof(bytemap_col));
-            bytemap_col.type = TGPU_INT8;
-            bytemap_col.flags = TGPU_COL_NULLS_BYTEMAP;
-            bytemap_col.length = total_recv;
-            bytemap_col.data = lane.recv->p;
-            bytemap_col.validity = lane.recv->as<uint8_t>();
-            DevColumn packed;
-            TG_TRY(tg_ingest_column(ctx, &bytemap_col, true, &packed));
-            dst.own_validity = packed.own_validity;
-            dst.validity = packed.validity;
-        }
+        TG_NCCL(ctx, g_nccl.group_end());
+        trace.mark("nccl send/recv");
+        for (size_t l = 0; l < lanes.size(); l++) base[l] = (char*)recv[l]->p;
+        TG_TRY(xchg_page(ctx, lanes, base, total_recv, &recv, &outp));
     }
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // send buffers are released after the transfers have left them
     OwnedPage* o = tg_make_owned_page(std::move(outp));
@@ -1061,17 +1088,14 @@ extern "C" int tgpu_exchange_broadcast(tgpu_ctx* ctx, const tgpu_page* page, tgp
     const int64_t n = in.rows;
     // count matrix: rows and one "has NULLs" flag per column from every rank
     const int V = 1 + C;
-    std::vector<long long> mine(V, 0), matrix((size_t)W * V);
+    std::vector<long long> mine(V, 0), matrix;
     mine[0] = n;
     for (int c = 0; c < C; c++) mine[1 + c] = in.cols[c].validity ? 1 : 0;
-    DevBuf d_mine, d_matrix;
-    TG_TRY(d_mine.alloc(ctx, (size_t)V * 8));
-    TG_TRY(d_matrix.alloc(ctx, (size_t)W * V * 8));
     if (W > 1) {
+        DevBuf d_mine;
+        TG_TRY(d_mine.alloc(ctx, (size_t)V * 8));
         TG_CUDA(ctx, cudaMemcpyAsync(d_mine.p, mine.data(), (size_t)V * 8, cudaMemcpyHostToDevice, ctx->stream));
-        TG_NCCL(ctx, g_nccl.all_gather(d_mine.p, d_matrix.p, (size_t)V, NCCL_INT64, ctx->comm, ctx->stream));
-        TG_CUDA(ctx, cudaMemcpyAsync(matrix.data(), d_matrix.p, (size_t)W * V * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        TG_TRY(count_matrix(ctx, d_mine, V, &matrix));
     }
     else matrix = mine;
     const int my_rank = W > 1 ? ctx->rank : 0;
@@ -1079,62 +1103,38 @@ extern "C" int tgpu_exchange_broadcast(tgpu_ctx* ctx, const tgpu_page* page, tgp
     for (int r = 0; r < W; r++) off[r + 1] = off[r] + matrix[(size_t)r * V];
     const long long total = off[W];
     if (total > (long long)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "broadcast output exceeds 2^31-1 rows");
-    struct Lane { int es; const void* src; std::shared_ptr<DevBuf> recv; DevBuf staged; int col; bool nulls; };
-    std::vector<Lane> lanes;
-    for (int c = 0; c < C; c++) {
-        lanes.push_back(Lane{in.cols[c].elem_size(), in.cols[c].data, nullptr, DevBuf(), c, false});
-        bool any = false;
-        for (int r = 0; r < W; r++) any = any || matrix[(size_t)r * V + 1 + c] != 0;
-        if (any) lanes.push_back(Lane{1, nullptr, nullptr, DevBuf(), c, true});
-    }
-    for (auto& lane : lanes) {
-        lane.recv = std::make_shared<DevBuf>();
-        TG_TRY(lane.recv->alloc(ctx, (size_t)std::max<long long>(total, 1) * lane.es));
+    std::vector<XchgLane> lanes = xchg_lanes(in, null_lanes(matrix, W, V, 1, C));
+    std::vector<std::shared_ptr<DevBuf>> recv(lanes.size());
+    std::vector<DevBuf> staged(lanes.size());
+    std::vector<char*> base(lanes.size());
+    for (size_t l = 0; l < lanes.size(); l++) {
+        XchgLane& lane = lanes[l];
+        const size_t es = lane_bytes(lane);
+        recv[l] = std::make_shared<DevBuf>();
+        TG_TRY(recv[l]->alloc(ctx, (size_t)std::max<long long>(total, 1) * es));
+        base[l] = (char*)recv[l]->p;
         if (lane.nulls) {
-            // this rank's NULL bytes (all zero when its own page has no validity buffer)
-            TG_TRY(lane.staged.alloc(ctx, (size_t)std::max<int64_t>(n, 1)));
-            if (in.cols[lane.col].validity && n > 0)
-                TG_LAUNCH(ctx, validity_to_bytes_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, in.cols[lane.col].validity, n, lane.staged.as<uint8_t>());
-            else TG_CUDA(ctx, cudaMemsetAsync(lane.staged.p, 0, (size_t)std::max<int64_t>(n, 1), ctx->stream));
-            lane.src = lane.staged.p;
+            // this rank's NULL bytes (all zero when its own page has no validity buffer), copied as 1-byte cells
+            TG_TRY(staged[l].alloc(ctx, (size_t)std::max<int64_t>(n, 1)));
+            if (lane.src && n > 0)
+                TG_LAUNCH(ctx, validity_to_bytes_kernel, tg_grid(ctx, n, 1024, 8), 256, 0, (const uint8_t*)lane.src, n, staged[l].as<uint8_t>());
+            else TG_CUDA(ctx, cudaMemsetAsync(staged[l].p, 0, (size_t)std::max<int64_t>(n, 1), ctx->stream));
+            lane.src = staged[l].p;
         }
-        if (n > 0)
-            TG_CUDA(ctx, cudaMemcpyAsync((char*)lane.recv->p + (size_t)off[my_rank] * lane.es, lane.src, (size_t)n * lane.es, cudaMemcpyDeviceToDevice, ctx->stream));
+        if (n > 0) TG_CUDA(ctx, cudaMemcpyAsync(base[l] + (size_t)off[my_rank] * es, lane.src, (size_t)n * es, cudaMemcpyDeviceToDevice, ctx->stream));
     }
     if (W > 1) TG_NCCL(ctx, g_nccl.group_start());
-    for (auto& lane : lanes)
+    for (size_t l = 0; l < lanes.size(); l++)
         for (int r = 0; r < W && W > 1; r++) {
             if (r == my_rank) continue;
-            if (n > 0) TG_NCCL(ctx, g_nccl.send(lane.src, (size_t)n * lane.es, NCCL_INT8, r, ctx->comm, ctx->stream));
+            const size_t es = lane_bytes(lanes[l]);
+            if (n > 0) TG_NCCL(ctx, g_nccl.send(lanes[l].src, (size_t)n * es, NCCL_INT8, r, ctx->comm, ctx->stream));
             long long cnt = matrix[(size_t)r * V];
-            if (cnt > 0) TG_NCCL(ctx, g_nccl.recv((char*)lane.recv->p + (size_t)off[r] * lane.es, (size_t)cnt * lane.es, NCCL_INT8, r, ctx->comm, ctx->stream));
+            if (cnt > 0) TG_NCCL(ctx, g_nccl.recv(base[l] + (size_t)off[r] * es, (size_t)cnt * es, NCCL_INT8, r, ctx->comm, ctx->stream));
         }
     if (W > 1) TG_NCCL(ctx, g_nccl.group_end());
     DevPage outp;
-    outp.rows = total;
-    outp.cols.resize(C);
-    for (auto& lane : lanes) {
-        DevColumn& dst = outp.cols[lane.col];
-        if (!lane.nulls) {
-            dst.type = in.cols[lane.col].type;
-            dst.length = total;
-            dst.own_data = lane.recv;
-            dst.data = lane.recv->p;
-        }
-        else if (total > 0) {
-            tgpu_column bm;
-            memset(&bm, 0, sizeof(bm));
-            bm.type = TGPU_INT8;
-            bm.flags = TGPU_COL_NULLS_BYTEMAP;
-            bm.length = total;
-            bm.data = lane.recv->p;
-            bm.validity = lane.recv->as<uint8_t>();
-            DevColumn packed;
-            TG_TRY(tg_ingest_column(ctx, &bm, true, &packed));
-            dst.own_validity = packed.own_validity;
-            dst.validity = packed.validity;
-        }
-    }
+    TG_TRY(xchg_page(ctx, lanes, base, total, &recv, &outp));
     TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // staged NULL bytes and the borrowed input are the caller's again
     OwnedPage* o = tg_make_owned_page(std::move(outp));
     *out = &o->hdr;
@@ -1145,15 +1145,10 @@ extern "C" int tgpu_exchange_broadcast(tgpu_ctx* ctx, const tgpu_page* page, tgp
 // split-phase exchange: SMs partition, copy engines move, the caller's next kernels overlap the transfer
 // ------------------------------------------------------------------------------------------------
 struct tgpu_exchange {
-    struct Lane {
-        int elem;          // element bytes (0: NULL-byte lane of a nullable column)
-        int col;
-        bool nulls;
-        DevBuf send;       // rows for peer destinations, destination-major
-    };
-    std::vector<Lane> lanes;
-    std::vector<int32_t> col_types;
+    std::vector<XchgLane> lanes;
     std::vector<size_t> region_off;   // of every lane inside this rank's arena
+    std::vector<DevBuf> send;         // per lane: rows for peer destinations, destination-major
+    DevBuf token;                     // the barrier's all-reduce buffer
     int arena = 0;
     long long total_recv = 0;
     cudaEvent_t done = nullptr;
@@ -1166,16 +1161,12 @@ extern "C" int tgpu_exchange_begin(tgpu_ctx* ctx, tgpu_op* partitioner, const tg
     PartitionOp* p = dynamic_cast<PartitionOp*>(partitioner);
     if (!ctx || !p || !page || !out) return TGPU_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    TG_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->comm) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "tgpu_comm_init has not been called");
+    bool general = false;
+    TG_TRY(exchange_prologue(ctx, p, page, &general));
     if (!ctx->comm2) return tg_fail(ctx, TGPU_ERR_NOT_SUPPORTED, "split-phase exchange needs ncclCommSplit (NCCL >= 2.18)");
     if (ctx->arena_peer[0].empty()) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "split-phase exchange needs arenas (tgpu_comm_arena_create/open)");
     if (ctx->exchanges_in_flight >= 2) return tg_fail(ctx, TGPU_ERR_ILLEGAL_STATE, "more than two exchanges in flight on one context");
-    const int W = ctx->world;
-    if (p->partition_count != W) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "partition count %d != world size %d", p->partition_count, W);
-    const int64_t n = page->num_rows;
-    if (n > (int64_t)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INVALID_ARGUMENT, "page has more than 2^31-1 positions");
-    if (exchange_needs_general_path(p, page) || W > XMAXP) {
+    if (general) {
         // shapes the copy-engine form does not carry (variable width, replicated rows): the blocking general exchange runs here, _end
         // hands its page over.  Every rank takes this branch for the same exchange (the shape is a property of the plan, not of the data).
         std::unique_ptr<tgpu_exchange> g(new tgpu_exchange());
@@ -1184,6 +1175,8 @@ extern "C" int tgpu_exchange_begin(tgpu_ctx* ctx, tgpu_op* partitioner, const tg
         *out = g.release();
         return TGPU_OK;
     }
+    const int W = ctx->world, me = ctx->rank;
+    const int64_t n = page->num_rows;
     DevPage in;
     TG_TRY(tg_ingest_page(ctx, page, &in));
     const int C = (int)in.cols.size();
@@ -1213,101 +1206,56 @@ extern "C" int tgpu_exchange_begin(tgpu_ctx* ctx, tgpu_op* partitioner, const tg
         TG_LAUNCH(ctx, xchg_offsets_kernel, W, 256, 0, hist.as<unsigned int>(), grid, W, block_off.as<long long>(), d_totals.as<long long>());
     }
     // 2. count matrix
-    std::vector<long long> matrix((size_t)W * V);
-    DevBuf d_matrix;
-    TG_TRY(d_matrix.alloc(ctx, (size_t)W * V * 8));
-    TG_NCCL(ctx, g_nccl.all_gather(d_totals.p, d_matrix.p, (size_t)V, NCCL_INT64, ctx->comm, ctx->stream));
-    TG_CUDA(ctx, cudaMemcpyAsync(matrix.data(), d_matrix.p, (size_t)W * V * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    TG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    std::vector<long long> send_vec(matrix.begin() + (size_t)ctx->rank * V, matrix.begin() + (size_t)(ctx->rank + 1) * V);
-    std::vector<long long> send_off(W + 1, 0), total_recv_of(W, 0);
+    std::vector<long long> matrix;
+    TG_TRY(count_matrix(ctx, d_totals, V, &matrix));
+    const long long* send_vec = &matrix[(size_t)me * V];
+    std::vector<long long> send_off(W + 1, 0);
     for (int r = 0; r < W; r++) send_off[r + 1] = send_off[r] + send_vec[r];
+    std::vector<XchgLane> lanes = xchg_lanes(in, null_lanes(matrix, W, V, W, C));
+    const ArenaLayout layout(matrix, W, V, me, lanes);
+    if (layout.total_recv_of[me] > (long long)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "exchange output exceeds 2^31-1 rows on rank %d", me);
     for (int d = 0; d < W; d++)
-        for (int r = 0; r < W; r++) total_recv_of[d] += matrix[(size_t)r * V + d];
-    if (total_recv_of[ctx->rank] > (long long)INT32_MAX) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "exchange output exceeds 2^31-1 rows on rank %d", ctx->rank);
+        if (layout.bytes(d) > ctx->arena_bytes) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "rank %d would receive more than its arena holds", d);
     std::unique_ptr<tgpu_exchange> x(new tgpu_exchange());
-    x->total_recv = total_recv_of[ctx->rank];
+    x->lanes = std::move(lanes);
+    x->total_recv = layout.total_recv_of[me];
     x->arena = (int)(ctx->arena_epoch % TGPU_NUM_ARENAS);
-    for (int c = 0; c < C; c++) {
-        x->col_types.push_back(in.cols[c].type);
-        bool any_nulls = false;
-        for (int r = 0; r < W; r++) any_nulls = any_nulls || matrix[(size_t)r * V + W + c] != 0;
-        x->lanes.emplace_back();
-        x->lanes.back().elem = in.cols[c].elem_size();
-        x->lanes.back().col = c;
-        x->lanes.back().nulls = false;
-        if (any_nulls) {
-            x->lanes.emplace_back();
-            x->lanes.back().elem = 0;
-            x->lanes.back().col = c;
-            x->lanes.back().nulls = true;
-        }
-    }
-    const size_t L = x->lanes.size();
-    auto es_of = [&](size_t l) { return (size_t)(x->lanes[l].elem ? x->lanes[l].elem : 1); };
-    auto region_off = [&](int d, size_t lane) {
-        size_t off = 0;
-        for (size_t l = 0; l < lane; l++) off += (((size_t)total_recv_of[d] * es_of(l)) + 255) & ~(size_t)255;
-        return off;
-    };
-    for (int d = 0; d < W; d++)
-        if (region_off(d, L) > ctx->arena_bytes) return tg_fail(ctx, TGPU_ERR_INSUFFICIENT_RESOURCES, "rank %d would receive more than its arena holds", d);
-    for (size_t l = 0; l < L; l++) x->region_off.push_back(region_off(ctx->rank, l));
-    auto before_of = [&](int d) {     // rows of lower-ranked senders come first in destination d
-        long long b = 0;
-        for (int r = 0; r < ctx->rank; r++) b += matrix[(size_t)r * V + d];
-        return b;
-    };
     // 3. scatter: peer-bound rows into send buffers (destination-major), rows that stay into their final place
+    const size_t L = x->lanes.size();
+    x->send.resize(L);
     std::vector<char*> h_dst(L * W);
-    std::vector<const void*> srcs(L);
     for (size_t l = 0; l < L; l++) {
-        const size_t es = es_of(l);
-        TG_TRY(x->lanes[l].send.alloc(ctx, (size_t)std::max<int64_t>(n, 1) * es));
-        const DevColumn& col = in.cols[x->lanes[l].col];
-        srcs[l] = x->lanes[l].nulls ? (const void*)col.validity : col.data;
-        for (int d = 0; d < W; d++) h_dst[l * W + d] = (char*)x->lanes[l].send.p + (size_t)send_off[d] * es;
-        h_dst[l * W + ctx->rank] = (char*)ctx->arena_local[x->arena] + x->region_off[l] + (size_t)before_of(ctx->rank) * es;
+        const size_t es = layout.es[l];
+        x->region_off.push_back(layout.region_off(me, l));
+        TG_TRY(x->send[l].alloc(ctx, (size_t)std::max<int64_t>(n, 1) * es));
+        for (int d = 0; d < W; d++) h_dst[l * W + d] = (char*)x->send[l].p + (size_t)send_off[d] * es;
+        h_dst[l * W + me] = layout.dst(ctx->arena_local[x->arena], me, l);
     }
     DevBuf d_dst;
-    TG_TRY(d_dst.alloc(ctx, h_dst.size() * sizeof(char*)));
-    TG_CUDA(ctx, cudaMemcpyAsync(d_dst.p, h_dst.data(), h_dst.size() * sizeof(char*), cudaMemcpyHostToDevice, ctx->stream));
-    if (n > 0) {
-        XchgCols xc;
-        memset(&xc, 0, sizeof(xc));
-        xc.count = (int32_t)L;
-        for (size_t l = 0; l < L; l++) { xc.elem[l] = x->lanes[l].elem; xc.src[l] = srcs[l]; }
-        xc.dst = d_dst.as<char*>();
-        TG_TRY(xchg_launch_scatter(ctx, geom, ids_from_key ? nullptr : pids.as<uint8_t>(), n, W, block_off.as<long long>(), xc, &k, p->bucket_count, b2p));
-    }
+    XchgCols xc;
+    TG_TRY(xchg_cols(ctx, x->lanes, h_dst, &d_dst, &xc));
+    if (n > 0) TG_TRY(xchg_launch_scatter(ctx, geom, ids_from_key ? nullptr : pids.as<uint8_t>(), n, W, block_off.as<long long>(), xc, &k, p->bucket_count, b2p));
     // 4. hand over to the copy engines.  The event also orders the transfer behind everything enqueued on this context so far:
     //    the readers of the arena this exchange's peers will overwrite NEXT (see the header).
     TG_CUDA(ctx, cudaEventCreateWithFlags(&x->done, cudaEventDisableTiming));
     TG_CUDA(ctx, cudaEventRecord(x->done, ctx->stream));
     TG_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, x->done, 0));
     for (int step = 1; step < W; step++) {
-        const int d = (ctx->rank + step) % W;          // staggered: at any moment every receiver has one sender per step
+        const int d = (me + step) % W;          // staggered: at any moment every receiver has one sender per step
         if (send_vec[d] == 0) continue;
         for (size_t l = 0; l < L; l++) {
-            const size_t es = es_of(l);
-            char* dst = (char*)ctx->arena_peer[x->arena][d] + region_off(d, l) + (size_t)before_of(d) * es;
-            const char* src = (const char*)x->lanes[l].send.p + (size_t)send_off[d] * es;
-            TG_CUDA(ctx, cudaMemcpyAsync(dst, src, (size_t)send_vec[d] * es, cudaMemcpyDefault, ctx->copy_stream));
+            const size_t es = layout.es[l];
+            const char* src = (const char*)x->send[l].p + (size_t)send_off[d] * es;
+            TG_CUDA(ctx, cudaMemcpyAsync(layout.dst(ctx->arena_peer[x->arena][d], d, l), src, (size_t)send_vec[d] * es, cudaMemcpyDefault, ctx->copy_stream));
         }
     }
     // 5. barrier: when it completes here, every peer's copies into this rank's arena have completed
-    DevBuf token;
-    TG_TRY(token.alloc(ctx, 16));
-    TG_CUDA(ctx, cudaMemsetAsync(token.p, 0, 16, ctx->copy_stream));
-    TG_NCCL(ctx, g_nccl.all_reduce(token.p, (char*)token.p + 8, 1, NCCL_INT64, 0 /* ncclSum */, ctx->comm2, ctx->copy_stream));
+    TG_TRY(x->token.alloc(ctx, 16));
+    TG_CUDA(ctx, cudaMemsetAsync(x->token.p, 0, 16, ctx->copy_stream));
+    TG_NCCL(ctx, g_nccl.all_reduce(x->token.p, (char*)x->token.p + 8, 1, NCCL_INT64, 0 /* ncclSum */, ctx->comm2, ctx->copy_stream));
     TG_CUDA(ctx, cudaEventRecord(x->done, ctx->copy_stream));
     // temporaries of this function (pids, histograms, pointer table) are released in stream order on ctx->stream, behind the
     // scatter; the send buffers and the barrier token are used by the copy stream and live in the handle until _end
-    x->lanes.emplace_back();                               // park the token in a pseudo lane
-    x->lanes.back().elem = -1;
-    x->lanes.back().col = -1;
-    x->lanes.back().nulls = false;
-    x->lanes.back().send = std::move(token);
     ctx->arena_epoch++;
     ctx->exchanges_in_flight++;
     *out = x.release();
@@ -1324,33 +1272,10 @@ extern "C" int tgpu_exchange_end(tgpu_ctx* ctx, tgpu_exchange* exchange, tgpu_pa
     if (x->ready) { *out = x->ready; return TGPU_OK; }
     // the received rows are complete once this rank's barrier has run; everything below is ordered behind it on ctx->stream
     TG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, x->done, 0));
+    std::vector<char*> base;
+    for (size_t off : x->region_off) base.push_back((char*)ctx->arena_local[x->arena] + off);
     DevPage outp;
-    outp.rows = x->total_recv;
-    outp.cols.resize(x->col_types.size());
-    size_t li = 0;
-    for (auto& lane : x->lanes) {
-        if (lane.col < 0) continue;
-        DevColumn& dst = outp.cols[lane.col];
-        char* region = (char*)ctx->arena_local[x->arena] + x->region_off[li++];
-        if (!lane.nulls) {
-            dst.type = x->col_types[lane.col];
-            dst.length = x->total_recv;
-            dst.data = region;     // aliases the arena: valid until the second-next exchange on this context
-        }
-        else if (x->total_recv > 0) {
-            tgpu_column bytemap_col;
-            memset(&bytemap_col, 0, sizeof(bytemap_col));
-            bytemap_col.type = TGPU_INT8;
-            bytemap_col.flags = TGPU_COL_NULLS_BYTEMAP;
-            bytemap_col.length = x->total_recv;
-            bytemap_col.data = region;
-            bytemap_col.validity = (const uint8_t*)region;
-            DevColumn packed;
-            TG_TRY(tg_ingest_column(ctx, &bytemap_col, true, &packed));
-            dst.own_validity = packed.own_validity;
-            dst.validity = packed.validity;
-        }
-    }
+    TG_TRY(xchg_page(ctx, x->lanes, base, x->total_recv, nullptr, &outp));     // aliases the arena: valid until the second-next exchange on this context
     OwnedPage* po = tg_make_owned_page(std::move(outp));
     *out = &po->hdr;
     // the send buffers are returned to this context's allocator here: their next use is ordered behind the wait above
